@@ -7,7 +7,7 @@ on synthetic 128x128x3 uint8 video, B x T = 128 x 128 per GPU (BASELINE.json met
 
 One "step" = one forward over a (B, T) = (128, 128) chunk per GPU = 16384 frames, KV memory carried from the previous
 step (so the 128-frame memory is full in the timed region).  Inputs (805 MB of u8 frames per step) are far larger than the
-126 MB L2, so no explicit flush is needed.  Multi-GPU: batch rows are independent -> each rank runs its own (128, 128)
+50 MB L2 of an H100, so no explicit flush is needed.  Multi-GPU: batch rows are independent -> each rank runs its own (128, 128)
 chunk, no data-path collective (weak scaling); timing = max over ranks of CUDA-event time.
 Prints ONE JSON line on rank 0.
 """
@@ -28,9 +28,6 @@ for p in (ROOT, os.path.join(ROOT, "oracle")):
 import torch  # noqa: E402
 
 METRIC = "frames/sec MinecraftPolicy fwd, 128x128x3 BxT=128x128"
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel (conv3x3_zp_kernel, 128->128 @64x64, 2048 frames)
-# from the committed ncu capture (profiles/conv_zp_r2.md, profiles/kernels_r2.csv)
-TRAFFIC_NCU = 2.307e9  # 1.171 GB read + 1.136 GB written (conv3x3_zp_kernel<pair>, 256->256 @32x32, 2048 frames; algorithmic 2.28 GB; profiles/conv_zp_r2.md)
 
 
 def parse():
@@ -48,6 +45,8 @@ def parse():
     ap.add_argument("--bc-width", default="3x", choices=["1x", "2x", "3x"])
     ap.add_argument("--bc-batch", type=int, default=16)
     ap.add_argument("--bc-steps", type=int, default=4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32 / float64), for output-by-output comparison of two builds")
     return ap.parse_args()
 
 
@@ -56,7 +55,7 @@ def peaks():
     if os.path.isfile(path):
         d = json.load(open(path))
         return dict(tflops=d["bf16_tflops_sustained"], hbm=d["hbm_gbs"], source="measured (MEASURED_PEAKS.json, sustained bf16)")
-    return dict(tflops=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md: ~1.4 PF sustained, 6.65 TB/s)")
+    return dict(tflops=989.0, hbm=3350.0, source="fallback (NVIDIA H100 SXM data sheet at 700 W: 989 TFLOP/s dense bf16, 3.35 TB/s HBM3)")
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -172,7 +171,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# extra blocks of the JSON line (VERDICT round 1, item 2): every number that used to be prose in DESIGN.md
+# extra blocks of the JSON line: every number the project reports about itself
 # ------------------------------------------------------------------------------------------------------------------
 def _free():
     import gc
@@ -194,7 +193,7 @@ def _event_ms(fn, steps, warmup):
 
 
 def gpu_eager_baseline(width, dev, B=4, T=128, seconds=6.0):
-    """The honest GPU bar (SURVEY 8d / BASELINE.md 4): the reference ALGORITHM run eagerly by PyTorch on the same B200 -- the oracle
+    """The honest GPU bar (SURVEY 8d / BASELINE.md 4): the reference ALGORITHM run eagerly by PyTorch on the same GPU -- the oracle
     port (same torch ops in the same order as lib/policy.py; the reference itself cannot travel to the GPU box) dispatched to
     cuDNN / cuBLAS / ATen, fp32 with TF32 off and on.  B x T = 128 x 128 does not fit (8 MiB of fp32 per frame for the first conv
     alone), so it runs B sequences of T frames with the KV memory full; per-frame cost is batch independent."""
@@ -443,6 +442,25 @@ def bc_block(args, dev, world, rank, pk):
     return res
 
 # ------------------------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, pd, vpred, ac, rows=256):
+    """What the last timed step returned to its caller, as DIR/<name>.npy: the value prediction and the sampled actions (float64,
+    exact) of every frame, and each action head's log-probabilities (float32) at a fixed, seeded sample of `rows` frames -- all of
+    the buttons head would be 566 MB per step.  The frames and the weights come from fixed seeds, so two builds given the same
+    arguments can be compared output for output."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    B, T = vpred.shape[0], vpred.shape[1]
+    idx = torch.randperm(B * T, generator=torch.Generator().manual_seed(20240601))[:min(rows, B * T)].sort().values
+    arrays = {"vpred": vpred.float(), "frame_index": idx.double()}
+    for k, v in pd.items():
+        arrays[f"logprob_{k}"] = v.float().reshape(B * T, -1)[idx.to(v.device)]
+    for k, v in ac.items():
+        arrays[f"action_{k}"] = v.double()
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
+
+
 def run_ours(args):
     import torch.distributed as dist
 
@@ -520,7 +538,9 @@ def run_ours(args):
     nat.device_check()
     value = world * frames_per_step * args.steps / (ms / 1000.0)
 
-    # dominant kernel = gemm_tc_kernel (tcgen05 implicit-GEMM conv + linear): live CUDA-event durations of every launch
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pd, vpred, ac)
+    # dominant kernel = gemm_tc_kernel (wgmma implicit-GEMM conv + linear): live CUDA-event durations of every launch
     g_ms = sum(a.elapsed_time(b) for a, b, _, _, _ in prof)
     g_fl = sum(f for _, _, f, _, _ in prof)
     conv_ms = sum(a.elapsed_time(b) for a, b, _, k, _ in prof if k == "conv")
@@ -535,7 +555,7 @@ def run_ours(args):
     achieved = g_fl / (g_ms / 1000.0) / 1e12
     flops_frame = pol.net.cfg.forward_flops_per_frame()  # product-side FLOP model (policy.NetConfig), SURVEY 8d
     roofline = {"bound": "tensor", "achieved": achieved, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": achieved / pk["tflops"],
-                "traffic": TRAFFIC_NCU, "kernel": "conv3x3_zp_kernel + gemm_tc_kernel (tcgen05 implicit-GEMM conv3x3 / linear)",
+                "kernel": "conv3x3_zp_kernel + gemm_tc_kernel (wgmma implicit-GEMM conv3x3 / linear)",
                 "peak_source": pk["source"],
                 "launches_per_step": len(prof) // args.steps, "kernel_ms_per_step": g_ms / args.steps,
                 "kernel_share_of_step": g_ms / ms if world == 1 else None,
@@ -591,7 +611,7 @@ def run_ours(args):
                "config": {"workload": f"VPT {args.width} policy (agent.py:16-36 kwargs) forward + action/value heads, B={B} T={T} per GPU "
                                       f"(= BASELINE configs[2] shape), random-init weights, KV memory carried and full",
                           "global_batch": world * B, "seq_len": T, "parallelism": f"batch-sharded x{world}, no collective",
-                          "l2_policy": "inputs (805 MB u8 frames/step) exceed the 126 MB L2; no explicit flush"},
+                          "l2_policy": "inputs (805 MB u8 frames/step) exceed the 50 MB L2; no explicit flush"},
                "roofline": roofline, "cpu_baseline": cb, "e2e": e2e, "gpu_launches": launches, "clocks": clocks}
         out.update(extras)
         print(json.dumps(out))

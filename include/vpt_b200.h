@@ -1,4 +1,4 @@
-/* vpt_b200.h -- C ABI of the B200-native VPT policy forward path (libvpt_b200.so).
+/* vpt_b200.h -- C ABI of the H100-native (sm_90a) VPT policy forward path (libvpt_b200.so).
  *
  * The reference (openai/Video-Pre-Training) is pure Python on top of torch (it has NO FFI of its own, SURVEY.md
  * section 2.1), so each entry point below replaces the torch / ATen call sequence of one reference site; the
@@ -40,7 +40,7 @@ int vpt_device_error(void);
 int vpt_num_sms(void);
 
 /* ----------------------------------------------------------------------------------------------------------
- * Tensor-core GEMM / implicit-GEMM 3x3 convolution (tcgen05.mma, TMA-fed, TMEM accumulators).
+ * Tensor-core GEMM / implicit-GEMM 3x3 convolution (wgmma, TMA-fed, register accumulators).
  *
  *   acc[m][n] = sum_k A[m][k] * B[n][k]                      (bf16 x bf16 -> fp32)
  *   v = a_g * acc - b_g * S1[cls(m)][n] + S2[cls(m)][n]      (a_g,b_g) = (rstd_g, rstd_g*mean_g), or (1,0) if mr==NULL
@@ -80,8 +80,8 @@ typedef struct vpt_gemm_args {
     /* Column segments (fused projections, e.g. Q | K | V | R of lib/xf.py:334-365 as ONE GEMM over the concatenated weight): columns
      * [dst_n0[i], dst_n0[i+1]) go to dst_out[i] (column 0 of that buffer = column dst_n0[i] of the GEMM) with its own leading dimension
      * and dtype; dst_remap[i] != 0 applies the seg_len / seg_stride / seg_off row remap to that segment only.  ndst == 0: out / ld_out /
-     * out_f32 (+ the row remap, if any) describe the single destination.  Every dst_n0[i] must be a multiple of the N tile (256 for
-     * N > 256); statistics partials are not supported with segments. */
+     * out_f32 (+ the row remap, if any) describe the single destination.  Every dst_n0[i] must be a multiple of the N tile: 128 when
+     * N > 64 and every segment start is a multiple of 128, otherwise 64; statistics partials are not supported with segments. */
     int32_t ndst;
     int32_t dst_n0[4];
     void* dst_out[4];
@@ -91,9 +91,9 @@ typedef struct vpt_gemm_args {
 } vpt_gemm_args;
 
 int vpt_gemm_bf16(const vpt_gemm_args* args, void* stream);
-/* Cluster size used when vpt_gemm_args.cluster == 0 (tuning knob; 1, 2 or 4; initial value 2). */
+/* Cluster size used when vpt_gemm_args.cluster == 0 (tuning knob; 1, 2 or 4; initial value 1). */
 int vpt_set_default_cluster(int32_t cluster);
-/* Hardware experiment hook used by tools/desc_experiment.py (A rows loaded `shift` rows early, UMMA descriptor start
+/* Hardware experiment hook used by tools/desc_experiment.py (A rows loaded `shift` rows early, wgmma descriptor start
  * advanced to compensate, base_offset field on/off).  base_offset_mode = -1 (with shift 0) only disables the small-M
  * weight-streaming kernel so that tests can force the tensor-core kernel.  Not for production use. */
 int vpt_debug_set(int32_t shift, int32_t base_offset_mode);
@@ -108,7 +108,8 @@ int vpt_gemm_stat_parts(int32_t N);
  *
  * GroupNorm(1) -> Conv2d 3x3 pad 1 -> ReLU [+ residual] (lib/util.py:75-82 conv flavour, lib/impala_cnn.py:50-52) on ZP
  * tensors.  Same fold as vpt_gemm_bf16(conv=1) (S1/S2 are [9][Cout] border-class tables), but the input rows are
- * fetched ONCE per 64-channel block and reused by all nine taps from shared memory.
+ * fetched ONCE per 64-channel block and reused by all nine taps from shared memory.  W <= 182 (two stages of the 128 + 2*(W+2)-row
+ * input span must fit in shared memory beside the weight pipeline).
  * -------------------------------------------------------------------------------------------------------- */
 typedef struct vpt_conv_zp_args {
     const void* x;            /* bf16 ZP [F][H+1][W+1][Cin] */
@@ -133,18 +134,14 @@ typedef struct vpt_conv_zp_args {
 } vpt_conv_zp_args;
 
 int vpt_conv3x3_zp(const vpt_conv_zp_args* args, void* stream);
-/* SM pairs cooperating on 256-row tiles with tcgen05.mma.cta_group::2 (each CTA stages half of the weight tile):
- * 0 = never, 1 = auto (default: pairs when Cout > 128, where they measure +11-13 %), 2 = always.  Tuning / A-B knob. */
+/* Kernel-variant knob kept for ABI compatibility: this build has a single convolution kernel, so bits 0..3 and 8 have no effect;
+ * bits 4..7 select the epilogue timing experiment of tools/conv_bench.py (0 = off). */
 int vpt_set_conv_pair_mode(int32_t on);
-/* 1 (default): Cout == 128 layers (of launches with >= 32 tiles) run the operand-swapped kernel (channels as UMMA M, 256 pixels as N; see
- * csrc/conv_zp_t.cuh) with its two-phase epilogue on 16 warps; 0: the regular orientation; 6: the two-phase epilogue on 8 warps; 2 / 4 / 5:
- * timing experiment without an epilogue / fragment epilogue / channel-major single-pass epilogue (DESIGN.md section 4).  Changes
- * vpt_conv_zp_stat_parts(.., 128) and vpt_conv_zp_t_stat_floats.  Tuning / A-B knob: results are identical up to fp32 summation order of the statistics. */
+/* Kept for ABI compatibility: this build has no operand-swapped convolution kernel, so every mode runs the regular one. */
 int vpt_set_conv_swap_mode(int32_t on);
 int vpt_conv_zp_stat_parts(int32_t F, int32_t H, int32_t W, int32_t Cout);  /* (few frames use narrower weight tiles, hence more partials per row) */
-/* Cout == 128 with the operand-swapped kernel's experimental fragment epilogue (vpt_set_conv_swap_mode(4)): its statistics partials are per (tile, warp, frame slot),
- * not per row.  vpt_conv_zp_t_stat_floats > 0 <=> pass a float buffer of that many elements as stat_part and finalise it with
- * vpt_conv_zp_t_stats_finalize (mr[f] = mean, rstd over the H*W*128 interior values of frame f). */
+/* vpt_conv_zp_t_stat_floats > 0 would mean: pass a float buffer of that many elements as stat_part and finalise it with
+ * vpt_conv_zp_t_stats_finalize.  No kernel of this build emits such partials: it returns 0 and the finaliser refuses. */
 int64_t vpt_conv_zp_t_stat_floats(int32_t F, int32_t H, int32_t W, int32_t Cout);
 int vpt_conv_zp_t_stats_finalize(const float* part, float* mr, int32_t F, int32_t H, int32_t W, float eps, void* stream);
 
@@ -154,11 +151,10 @@ int vpt_conv_zp_t_stats_finalize(const float* part, float* mr, int32_t F, int32_
  *   img  u8   [F][H][W][3]      w  fp32 [C0][27] ordered (ky, kx, c), already divided by 255
  *   out  bf16 [F][H/2][W/2][C0] (zp=0) or ZP [F][H/2+1][W/2+1][C0] (zp=1)
  *   stat_part float2 [F][vpt_firstconv_stat_parts(F, H, W, C0)]   (H, W multiples of 16; C0 in {64,128,192,256})
- * Two kernels: for W in {32, 64, 128} with H*W <= 16384 the tcgen05 kernel (csrc/firstconv_tc.cuh: operand-swapped implicit GEMM,
- * thread = channel, 3x3/2 max in registers; its partials are per (8 pooled rows, column half, CHANNEL): partial index
- * ((row/8)*2 + half)*C0 + c, so per-channel sums are available to the caller); otherwise the mma.sync kernel (csrc/firstconv.cuh,
- * (H/16)*(W/16) partials per frame).  vpt_set_firstconv_mode(0) forces the mma.sync kernel (A/B knob).
- * out_f32 != 0 (tcgen05 kernel only): `out` is fp32 in the same layout (precision mode, csrc/precise.cuh).
+ * mma.sync kernel (csrc/firstconv.cuh), one CTA per 8x8 tile of pooled outputs; its partials are per (tile, CHANNEL): partial index
+ * tile * C0 + c with (H/16)*(W/16) tiles per frame, so per-channel sums are available to the caller.  vpt_set_firstconv_mode is kept
+ * for ABI compatibility (one kernel: every mode selects it).
+ * out_f32 != 0: `out` is fp32 in the same layout (precision mode, csrc/precise.cuh).
  * -------------------------------------------------------------------------------------------------------- */
 int vpt_firstconv_pool(const uint8_t* img, const float* w, const float* bias, void* out, float* stat_part,
                        int32_t F, int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream);
@@ -191,7 +187,7 @@ int vpt_codec_from_env(const int64_t* buttons, const double* camera, const doubl
 
 /* ----------------------------------------------------------------------------------------------------------
  * fp32-parity precision mode (csrc/precise.cuh; BASELINE north_star "1e-3 rtol fp32", reference arithmetic lib/xf.py:40,55-63).
- * Contractions stay on vpt_gemm_bf16 (tcgen05): operands split into bf16 hi + lo, three accumulating launches per layer
+ * Contractions stay on vpt_gemm_bf16 (wgmma): operands split into bf16 hi + lo, three accumulating launches per layer
  * (hi*hi, lo*hi, hi*lo; fp32 output used as the fp32 residual of the next launch).  These entry points are the fp32 glue between
  * them.  All tensors fp32 row-major [rows][C] unless noted.
  *   vpt_group_stats_f32   mr[g] = (mean, rstd) over `per_group` consecutive elements (GroupNorm(1) per frame / LayerNorm per row)
@@ -331,14 +327,14 @@ int vpt_relu_mask(const void* dout, const void* out, void* dz, int64_t n, void* 
  * pattern is the ReLU mask the backward needs)                                              lib/impala_cnn.py:50-52 */
 int vpt_add_stats(const void* a, const void* b, void* out, float* stat_part, int64_t groups, int64_t elems_per_group, void* stream);
 int vpt_add_stat_parts(int64_t elems_per_group);
-/* Weight-gradient kernel choice: 1 (default) = tap-pairing kernel (csrc/wgrad_tc.cuh: taps whose shifts differ by one row share one
- * activation span and one gradient tile in shared memory, two TMEM accumulators), 0 = one GEMM tile per tap (csrc/gemm_tc.cuh).  A-B knob. */
+/* Weight-gradient kernel choice, kept for ABI compatibility: this build has one weight-gradient kernel (one GEMM tile per tap,
+ * csrc/gemm_tc.cuh), so every mode selects it. */
 int vpt_set_wgrad_mode(int32_t mode);
 /* 1: forward-path kernels are launched with the programmatic-stream-serialization attribute (programmatic dependent launch): the next
  * kernel is scheduled while the previous one drains and blocks in griddepcontrol.wait until that one has completed and flushed, so only
  * launch latency overlaps.  Default 0 (measured neutral on the rollout CUDA graph; results are bit-identical either way). */
 int vpt_set_pdl(int32_t on);
-/* Weight gradient on the tcgen05 GEMM (both operands MN-major, K split over CTAs + fixed-order reduction):
+/* Weight gradient on the wgmma GEMM (both operands MN-major, K split over CTAs + fixed-order reduction):
  *   out fp32 [M][ntaps*N],  out[m][tap*N + n] = sum_{k in [0,R)} a[k][m] * b[k + shifts[tap]][n]   (rows outside [0,R) are 0)
  * a bf16 [R][lda] = output gradient (M columns), b bf16 [R][ldb] = (normalised) layer input (N columns); no transposes needed.
  * Linear: ntaps = 1, shift 0.  3x3 conv on ZP tensors: ntaps = 9, shifts[tap] = (ky-1)*(W+1) + (kx-1), out is [Cout][tap][Cin].

@@ -14,8 +14,8 @@ def require_cuda(t):
 
 
 def gemm_stat_parts(N):
-    nt = (N + 255) // 256
-    bn = (-(-N // nt) + 15) // 16 * 16
+    nt = (N + 127) // 128
+    bn = 64 if -(-N // nt) <= 64 else 128
     return -(-N // bn) * 2
 
 

@@ -23,8 +23,30 @@ def _random_factored(n, rng):
     return dict(buttons=btn, camera=cam)
 
 
-@pytest.mark.skipif(not refshim.available(), reason="/root/reference not present (GPU box)")
+def _codec_matches_golden():
+    import os
+
+    import make_golden
+
+    fx = torch.load(os.path.join(os.path.dirname(__file__), "golden", "codec.pt"), weights_only=False)
+    codec = A.ActionCodec(**A.ACTION_TRANSFORMER_KWARGS)
+    assert codec.n_buttons_joint == fx["n_buttons_joint"] == 8641
+    assert np.array_equal(codec.idx_to_factored, fx["idx_to_factored"])
+    assert np.array_equal(codec.idx_camera_off, fx["idx_camera_off"])
+    joint, fac, env = make_golden.codec_inputs()
+    for got, ref in ((codec.to_factored(joint), fx["to_factored"]), (codec.from_factored(fac), fx["from_factored"]),
+                     (codec.env2policy(env), fx["env2policy"])):
+        assert np.array_equal(got["buttons"], ref["buttons"]) and np.array_equal(got["camera"], ref["camera"])
+    e1, e2 = codec.policy2env(fac), fx["policy2env"]
+    assert set(e1) == set(e2) and all(np.array_equal(e1[k], e2[k]) for k in e1)
+    assert codec.null_buttons_idx == fx["null_buttons_idx"] and codec.camera_null_idx == fx["camera_null_idx"]
+
+
 def test_codec_matches_live_reference():
+    """The action codec against the reference's action mapping / transformer: live where its checkout is present, otherwise
+    against their outputs stored by oracle/make_golden.py on the same seeded batches."""
+    if not refshim.available():
+        return _codec_matches_golden()
     import sys
     ns = refshim.load()
     import lib.actions as ref_actions  # noqa: E402  (importable once refshim.load() has set up sys.path + stubs)

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads without a GPU and exports every symbol include/vpt_b200.h declares."""
+"""CPU: the C-ABI library builds for sm_90a, loads without a GPU and exports every symbol include/vpt_b200.h declares."""
 import ctypes
 import os
 import re
@@ -24,8 +24,8 @@ def test_header_symbols_are_bound_and_exported():
     assert l.vpt_abi_version() == 3
 
 
-def test_library_is_sm100a_tcgen05_tma():
-    """SASS evidence that the hot kernel is the Blackwell-native path (UTCHMMA = tcgen05.mma, UTMALDG = TMA, LDTM = tcgen05.ld)."""
+def test_library_is_sm90a_wgmma_tma():
+    """SASS evidence that the hot kernels are the Hopper-native path (HGMMA = wgmma.mma_async, UTMALDG = TMA, SYNCS = mbarrier)."""
     import shutil
     import subprocess
 
@@ -35,8 +35,8 @@ def test_library_is_sm100a_tcgen05_tma():
         import pytest
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", nat.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnem in ("UTCHMMA", "UTMALDG", "LDTM"):
+    assert "sm_90a" in sass
+    for mnem in ("HGMMA", "UTMALDG", "SYNCS"):
         assert mnem in sass, mnem
 
 

@@ -1,50 +1,60 @@
-"""CPU: pins oracle/vpt_oracle.py against (a) fixtures generated from the unmodified reference, (b) the live reference
-when /root/reference is present, (c) the invariants of SURVEY.md section 4."""
+"""CPU: pins oracle/vpt_oracle.py against (a) the live reference where its checkout is present (oracle/refshim.py), otherwise
+the reference outputs stored in tests/golden by oracle/make_golden.py, (b) the invariants of SURVEY.md section 4."""
 import glob
 import os
 
 import pytest
 import torch
 
+import make_golden
 import refshim
 import vpt_oracle as O
 
-GOLD = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.pt")))
+GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
+GOLD = [os.path.join(GOLDEN, n + ".pt") for n in ("tiny_plain", "tiny_perturbed")]
+
+
+def golden(name):
+    return torch.load(os.path.join(GOLDEN, name + ".pt"), weights_only=False)
+
+
+def seeded_weights(fx):
+    """The weights of a fixture (oracle/make_golden.py): seeded values on the reference's state-dict schema stored with it."""
+    return make_golden.seeded_state_dict(make_golden.template_from(fx["schema"]), fx["wseed"], fx.get("perturbed", False))
 
 
 @pytest.mark.parametrize("path", GOLD, ids=[os.path.basename(p) for p in GOLD])
 def test_oracle_matches_golden(path):
-    fx = torch.load(path)
+    """The oracle against the reference's outputs stored by oracle/make_golden.py (the live comparison where the reference is absent)."""
+    fx = torch.load(path, weights_only=False)
     cfg = O.Cfg(**fx["policy_kwargs"])
-    sd = fx["state_dict"]
+    sd = seeded_weights(fx)
     st = O.initial_state(cfg, fx["B"])
     with torch.no_grad():
-        for ch in fx["chunks"]:
-            (pd, v, _), st = O.agent_policy_forward(sd, cfg, ch["img"], ch["first"], st)
+        for (img, first), ch in zip(make_golden.forward_inputs(fx["B"]), fx["chunks"]):
+            (pd, v, _), st = O.agent_policy_forward(sd, cfg, img, first, st)
             # same torch ops in the same order as the reference -> bit exact on the same machine; 1e-5 across machines
             assert torch.allclose(pd["camera"], ch["camera"], rtol=1e-5, atol=1e-5)
-            assert torch.allclose(pd["buttons"][:, -1:], ch["buttons_last"], rtol=1e-5, atol=1e-5)
+            assert torch.allclose(pd["buttons"][..., make_golden.COLS], ch["buttons"], rtol=1e-5, atol=1e-5)
             assert torch.allclose(v, ch["vpred"], rtol=1e-5, atol=1e-5)
-            assert torch.allclose(st[0][1][0], ch["k0"], rtol=1e-5, atol=1e-6)
-            assert torch.allclose(st[0][1][1], ch["v0"], rtol=1e-5, atol=1e-6)
-            for s, m in zip(st, ch["masks"]):
+            for s, (m, k, vv) in zip(st, ch["state"]):
                 assert torch.equal(s[0], m)
+                assert torch.allclose(s[1][0], k, rtol=1e-5, atol=1e-6) and torch.allclose(s[1][1], vv, rtol=1e-5, atol=1e-6)
+    torch.manual_seed(7)
+    ac = O.sample(pd)
     if torch.equal(pd["camera"], fx["chunks"][-1]["camera"]):  # identical logits -> sampling must be bit exact
-        torch.manual_seed(1234)
-        ac = O.sample(pd)
         assert torch.equal(ac["camera"], fx["sample"]["camera"]) and torch.equal(ac["buttons"], fx["sample"]["buttons"])
-        assert torch.allclose(O.logprob(pd, ac), fx["sample_logprob"])
+    assert torch.allclose(O.logprob(pd, fx["sample"]), fx["sample_logprob"], rtol=1e-5, atol=1e-5)
 
 
 def test_golden_fixtures_exist():
     assert len(GOLD) >= 2
 
 
-@pytest.mark.skipif(not refshim.available(), reason="/root/reference not present (GPU box)")
 @pytest.mark.parametrize("pert", [False, True])
 def test_oracle_matches_live_reference(pert):
-    import make_golden
-
+    if not refshim.available():
+        return test_oracle_matches_golden(GOLD[int(pert)])
     pkw = refshim.policy_kwargs("2x", **refshim.TINY)
     pol = refshim.make_reference_agent_policy(pkw)
     if pert:
@@ -75,9 +85,20 @@ def test_oracle_matches_live_reference(pert):
     assert torch.equal(pol.pi_head.logprob(a1, pd), O.logprob(pd2, a2))
 
 
-@pytest.mark.skipif(not refshim.available(), reason="/root/reference not present (GPU box)")
 def test_oracle_matches_live_reference_128px():
-    """One full-size 128x128 frame through the 1x-width CNN path with reduced transformer (config C1 shape)."""
+    """One full-size 128x128 frame through the 1x-width CNN path with reduced transformer (config C1 shape); against the stored
+    reference outputs (oracle/make_golden.py) where the reference is absent."""
+    if not refshim.available():
+        fx = golden("forward_128px")
+        pkw = fx["policy_kwargs"]
+        cfg = O.Cfg(**pkw)
+        with torch.no_grad():
+            (pd, v, _), _ = O.agent_policy_forward(seeded_weights(fx), cfg, make_golden.img_128px(), torch.zeros(1, 1, dtype=torch.bool),
+                                                   O.initial_state(cfg, 1))
+        for k in ("camera", "buttons"):
+            assert torch.allclose(pd[k], fx[k], rtol=1e-5, atol=1e-5), k
+        assert torch.allclose(v, fx["vpred"], rtol=1e-5, atol=1e-5)
+        return
     pkw = refshim.policy_kwargs("1x", n_recurrence_layers=1)
     pol = refshim.make_reference_agent_policy(pkw)
     sd = {k: v.detach().clone() for k, v in pol.state_dict().items()}
@@ -91,8 +112,8 @@ def test_oracle_matches_live_reference_128px():
 
 
 def _tiny():
-    fx = torch.load(GOLD[0])
-    return fx["state_dict"], O.Cfg(**fx["policy_kwargs"])
+    fx = torch.load(GOLD[0], weights_only=False)
+    return seeded_weights(fx), O.Cfg(**fx["policy_kwargs"])
 
 
 def test_chunk_size_invariance():
@@ -130,13 +151,41 @@ def test_flop_model_matches_survey():
         assert abs(O.forward_flops_per_frame(O.Cfg(**O.widths(w))) / 1e9 - gf) < 1e-3
 
 
-@pytest.mark.skipif(not refshim.available(), reason="/root/reference not present (GPU box)")
+def _gradient_matches_golden():
+    fx = golden("gradient")
+    pkw = fx["policy_kwargs"]
+    cfg = O.Cfg(**pkw)
+    sd = seeded_weights(fx)
+    st_o = O.initial_state(cfg, fx["B"])
+    for (img, first, actions), ch in zip(make_golden.gradient_inputs(fx["B"]), fx["chunks"]):
+        leaf = {k: v.clone().requires_grad_(v.dtype.is_floating_point) for k, v in sd.items()}
+        (pd_o, _, _), st_o = O.agent_policy_forward(leaf, cfg, img, first, st_o)
+        loss_o = -O.logprob(pd_o, actions).mean()
+        loss_o.backward()
+        st_o = [(m, (k.detach(), v.detach())) for (m, (k, v)) in st_o]
+        assert torch.allclose(loss_o.detach(), ch["loss"], rtol=1e-6, atol=0)
+        n_checked = 0
+        for name, ref in ch["grads"].items():
+            gr = leaf[name].grad
+            if ref is None:
+                assert gr is None, name  # value head: untouched by the BC loss in both
+                continue
+            gflat = gr.flatten()
+            # fp32 sums in another order on another host: each sampled element within 1e-5 of the parameter's gradient norm
+            # (measured: <= 1.8e-6 across 1 to 32 CPU threads)
+            assert torch.allclose(gflat[make_golden.grad_sample_index(name, gflat.numel())], ref["sample"], rtol=1e-5, atol=1e-5 * ref["norm"].item()), name
+            assert torch.allclose(gflat.norm(), ref["norm"], rtol=1e-5, atol=1e-8), name
+            n_checked += 1
+        assert n_checked > 80
+
+
 def test_oracle_gradient_matches_live_reference_autograd():
     """The BC step's parity target is autograd through the oracle (tests/test_training.py); this pins that target itself: the
     gradient of the BC loss (behavioural_cloning.py:101-123: -log-prob of the demonstrated action, KV memory detached between
-    chunks) through the unmodified reference equals the gradient through the oracle, parameter by parameter."""
-    import make_golden
-
+    chunks) through the unmodified reference equals the gradient through the oracle, parameter by parameter (against the stored
+    reference loss and gradient samples, oracle/make_golden.py, where the reference is absent)."""
+    if not refshim.available():
+        return _gradient_matches_golden()
     pkw = refshim.policy_kwargs("2x", **refshim.TINY)
     pol = refshim.make_reference_agent_policy(pkw)
     make_golden.perturb(pol)

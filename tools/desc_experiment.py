@@ -1,5 +1,6 @@
-"""One-off hardware experiment: does a K-major SWIZZLE_128B UMMA descriptor whose start address is advanced by s rows
-(s*128 B, not 1024-aligned) read rows s.. of the tile correctly, and does it need the base_offset field?"""
+"""Hardware experiment: does a K-major SWIZZLE_128B wgmma descriptor whose start address is advanced by s rows (s*128 B, not
+1024-aligned) read rows s.. of the tile correctly, and does it need the base_offset field?  csrc/conv_zp.cuh relies on the answer
+(on an H100: correct with base_offset 0 for every shift; setting the field breaks every shift that is not a multiple of 8)."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""video-pre-training_b200 -- B200-native (sm_100a) implementation of the VPT policy forward path.
+"""video-pre-training_b200 -- H100-native (sm_90a) implementation of the VPT policy forward path.
 
 The directory name carries a hyphen (it is fixed by the project layout), so import it through the root-level shim:
 

@@ -15,7 +15,7 @@ HEADER = os.path.join(_ROOT, "include", "vpt_b200.h")
 
 ABI_VERSION = 3  # == VPT_ABI_VERSION in include/vpt_b200.h (checked against the loaded library)
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]
 
 
@@ -25,7 +25,7 @@ def _sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/vpt_b200.cu (unity build) for sm_100a into libvpt_b200.so next to this file."""
+    """Compile csrc/vpt_b200.cu (unity build) for sm_90a into libvpt_b200.so next to this file."""
     if not force and os.path.isfile(LIB_PATH):
         newest = max(os.path.getmtime(p) for p in _sources())
         if os.path.getmtime(LIB_PATH) >= newest:

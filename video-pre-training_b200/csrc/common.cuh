@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: mbarrier / TMA / tcgen05 PTX wrappers, error plumbing.
-// Everything here is written against the PTX ISA for sm_100a (CUDA 12.9); no CUTLASS/CuTe dependency.
+// Shared device helpers for the sm_90a kernels: mbarrier / TMA / wgmma PTX wrappers, error plumbing.
+// Everything here is written against the PTX ISA for sm_90a (CUDA 12.x); no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -197,16 +197,6 @@ __device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, 
         : "memory");
 }
 
-// 2-CTA (cta_group::2) variant: issued by BOTH CTAs of a pair for their own shared memory, but the transaction bytes are
-// credited to the mbarrier of the pair's leader (even) CTA: clearing bit 24 of a shared::cluster address selects it.
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(dst)),
-        "l"((uint64_t)m), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-        : "memory");
-}
-
 // ------------------------------------------------------------------------------------------------------
 // thread-block clusters
 // ------------------------------------------------------------------------------------------------------
@@ -229,111 +219,64 @@ __device__ __forceinline__ void cluster_sync_all() {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA): a warpgroup of 128 threads computes D[64 x N] (+)= A[64 x 16] * B[N x 16]^T with both operands in
+// shared memory (descriptors below) and D in registers.  Fragment of m64nNk16 with fp32 accumulators: register r of warp w,
+// lane l holds row 16*w + l/4 + 8*((r/2)&1), column 8*(r/4) + 2*(l%4) + (r&1).
 // ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_reg_fence(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate; issued by ONE thread for the CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 64] (+)= A * B^T, bf16 inputs, fp32 accumulate.  TA / TB = 1: the operand is MN-major (its M / N index contiguous).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB)
         : "memory");
 }
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 
-// same, arriving on the barrier at this offset in every CTA of the cluster selected by cta_mask
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-
-// ---- cta_group::2: one MMA spans the CTA pair (M = 256: 128 rows per CTA; each CTA supplies half of the B rows) ----
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: rows of 64 bf16 (128 B), 8-row groups 1024 B apart.
-// (bit layout per the PTX ISA "shared memory descriptor": start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-//  version=1 [46,48), layout type [61,64) with 2 = SWIZZLE_128B.)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;             // LBO (unused for swizzled K-major), 16 B
-    d |= (uint64_t)(1024 >> 4) << 32;   // SBO = 8 rows * 128 B
-    d |= (uint64_t)1 << 46;             // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;             // SWIZZLE_128B
-    return d;
-}
-// MN-major, 128-byte-swizzled operand tile (the operand's M / N index is the contiguous one in memory): every K row holds 64
-// consecutive M/N elements (128 B), 8-K-row groups are 1024 B apart (SBO) and the next 64 M/N elements start `lbo_bytes`
-// further (LBO) -- i.e. TMA boxes of {64 elements (inner), K rows} stored back to back.  Canonical layout per the CUTLASS
-// UMMA notes: Swizzle<3,4,3> o ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units.
-__device__ __forceinline__ uint64_t umma_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// 128-byte-swizzled operand tile (bit layout per the PTX ISA "matrix descriptor" of wgmma: start>>4 [0,14), LBO>>4 [16,30),
+// SBO>>4 [32,46), base offset [49,52), swizzle mode [62,64) with 1 = SWIZZLE_128B).
+//   K-major: rows of 64 bf16 (128 B), 8-row groups `sbo` = 1024 B apart; LBO unused.
+//   MN-major: every K row holds 64 consecutive M/N elements (128 B), 8-K-row groups are `sbo` apart and the next 64 M/N elements
+//   start `lbo` further -- i.e. TMA boxes of {64 elements (inner), K rows} stored back to back.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16u, uint32_t sbo_bytes = 1024u) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)(lbo_bytes >> 4) << 16;
     d |= (uint64_t)(sbo_bytes >> 4) << 32;
-    d |= (uint64_t)1 << 46;             // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;             // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;  // SWIZZLE_128B
     return d;
 }
-// Instruction descriptor for kind::f16: D=f32, A=B=bf16, both K-major, M x N tile.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// same with both operands MN-major (bits 15 / 16: transpose A / B)
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16_mn(int M, int N) { return umma_idesc_bf16(M, N) | (1u << 15) | (1u << 16); }
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (quarter*32+i), columns c..c+31.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
+// The 64 x 64 fragment `d` (columns col0.. of the tile) -> rows of a row-major fp32 staging tile `stg` [64][pitch] in shared memory.
+__device__ __forceinline__ void wgmma_frag_store(const float (&d)[32], float* stg, int pitch, int col0) {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    const int r0 = 16 * w + (l >> 2), c0 = col0 + 2 * (l & 3);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        *reinterpret_cast<float2*>(stg + (size_t)r0 * pitch + c0 + 8 * i) = make_float2(d[4 * i], d[4 * i + 1]);
+        *reinterpret_cast<float2*>(stg + (size_t)(r0 + 8) * pitch + c0 + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+    }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// 32 consecutive fp32 values of one staging row (16-byte aligned) as raw words
+__device__ __forceinline__ void stg_ld_32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+        const float4 x = reinterpret_cast<const float4*>(src)[q];
+        v[4 * q] = __float_as_uint(x.x); v[4 * q + 1] = __float_as_uint(x.y); v[4 * q + 2] = __float_as_uint(x.z); v[4 * q + 3] = __float_as_uint(x.w);
+    }
+}
 
 }  // namespace vpt

@@ -1,20 +1,18 @@
-// Implicit-GEMM 3x3 convolution on tcgen05 with the input tile REUSED across the 9 taps from shared memory.
+// Implicit-GEMM 3x3 convolution on wgmma with the input tile REUSED across the 9 taps from shared memory.
 //
-// Measured on B200 (profiles/, DESIGN.md): a tcgen05 GEMM is bound by the bytes TMA can deliver INTO one SM
-// (~50-60 B/clk/SM), not by the tensor pipe, whenever a 128xN tile re-fetches A for every tap.  This kernel removes the
-// 9x A redundancy of implicit GEMM:
+// Implicit GEMM re-fetches the A tile for every tap, which makes a tensor-core convolution bound by the bytes TMA can deliver into
+// one SM rather than by the tensor pipe.  This kernel removes the 9x A redundancy:
 //
 //   * activations live in the "ZP" layout [F][H+1][W+1][C] (bf16) whose row y=H and column x=W are zero: with one shared
 //     zero row / column every 3x3 neighbour of pixel q (a linear row index over the whole tensor) is the row q + dy*(W+1) + dx,
-//     so a tile of 128 (or 256) consecutive rows needs ONE contiguous span of  rows + 2*(W+2)  input rows per 64 channels;
+//     so a tile of 128 consecutive rows needs ONE contiguous span of  rows + 2*(W+2)  input rows per 64 channels;
 //   * the span is fetched once per 64-channel block by plain 2-D TMA (out-of-range rows are zero-filled) and all 9 taps are
-//     issued as UMMAs whose A descriptors start at span + ((dy+1)*(W+1) + dx+1)*128 B.  (Hardware fact, measured with
-//     tools/desc_experiment.py: for K-major SWIZZLE_128B operands the swizzle is a function of the absolute shared-memory
-//     address, so a descriptor start advanced by any multiple of 128 B reads the shifted rows correctly with base_offset 0.)
-//   * weights stream through their own pipeline, one [N][64] tile per (channel block, tap); with N <= 128 one CTA computes
-//     two 128-row sub-tiles per weight tile (M = 256), halving the weight bytes per FLOP as well.
+//     issued as wgmmas whose A descriptors start at span + ((dy+1)*(W+1) + dx+1)*128 B (for K-major SWIZZLE_128B operands the
+//     swizzle is a function of the absolute shared-memory address, so a descriptor start advanced by any multiple of 128 B reads
+//     the shifted rows; tools/desc_experiment.py checks this on the GEMM kernel);
+//   * weights stream through their own pipeline, one [block_n][64] tile per (channel block, tap).
 //
-//   warp 0: A-span TMA producer   warp 1: MMA issuer (+TMEM alloc)   warp 2: weight TMA producer   warps 3..10: epilogue
+//   warps 0..7: two wgmma warpgroups (64 rows each) + epilogue   warp 8: A-span TMA producer   warp 9: weight TMA producer
 // Epilogue = GroupNorm fold (border-class tables), ReLU, residual, bf16 store in ZP layout (border rows are written as
 // zeros, which maintains the layout invariant), per-row (sum, sumsq) partials for the next layer's statistics.
 #pragma once
@@ -23,24 +21,18 @@
 
 namespace vpt {
 
-static int g_cz_pair = 1;
 static int g_cz_dbg = 0;
-static int g_cz_tma = 1;  // pair kernel: TMA-store epilogue (0 = per-thread global stores, the round-1 epilogue; A/B knob)
 
-constexpr int kCzStgChunk = kBlockM * 64;        // one staging buffer: 128 rows x 32 channels bf16 (64-byte rows, SWIZZLE_64B)
-constexpr int kCzStgBytes = 2 * 4 * kCzStgChunk; // 2 epilogue groups x up to 4 chunks
-
-constexpr int kCzThreads = 96 + 32 * kNumEpiWarps;  // 11 warps
+constexpr int kCzThreads = 32 * kNumEpiWarps + 64;  // 10 warps
 constexpr int kCzMaxBStages = 8;
 
 struct ConvZpParams {
     long long Q;  // total rows = F * FS
     int H, W, Wp, FS;
     int N, block_n, num_n_tiles, cin, cin_blocks;
-    int mt;               // 128-row sub-tiles per CTA tile (1 or 2)
     int a_box_rows, a_boxes, a_stage_bytes, b_stages;
     int dbg;              // experiment: 1 = epilogue skips its global stores, 2 = skips the whole epilogue body
-    int tma_epi;          // pair kernel: epilogue I/O through shared memory + TMA (output store, residual prefetch)
+    int bo;               // descriptor experiment: set the base-offset field of the shifted A descriptors
     long long num_m_tiles;
     const float* mr;
     const float* S1;
@@ -54,80 +46,47 @@ struct ConvZpParams {
     const float* res_shift;
 };
 
-// kPair: two CTAs of a cluster (an SM pair) cooperate on a 256-row tile with tcgen05.mma.cta_group::2 -- each CTA stages
-// its own 128 input rows and HALF of the weight tile, so the shared-memory operand traffic per FLOP (the measured limiter
-// of single-CTA UMMA, see DESIGN.md) is halved for the weights.
-template <bool kPair>
+template <int BN>
 __global__ void __launch_bounds__(kCzThreads, 1)
-conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-                  const __grid_constant__ CUtensorMap tmR, const ConvZpParams p) {
+conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvZpParams p) {
     pdl_sync();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    const uint32_t b_rows = (uint32_t)p.block_n / (kPair ? 2 : 1);   // weight rows staged by this CTA
-    const uint32_t b_stage_bytes = b_rows * kBlockK * 2;
-    const uint32_t cta_rank = kPair ? cluster_ctarank() : 0u;
-    const bool leader = (cta_rank == 0);
+    constexpr uint32_t b_stage_bytes = (uint32_t)BN * kBlockK * 2;
     uint8_t* smem_a = smem;                                        // 2 A-span stages
     uint8_t* smem_b = smem + 2 * (size_t)p.a_stage_bytes;          // b_stages weight tiles
-    uint8_t* smem_stage = smem_b + (size_t)p.b_stages * b_stage_bytes;  // tma_epi: output / residual staging (1024-aligned)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stage + (p.tma_epi ? kCzStgBytes : 0));
+    float* stg_all = reinterpret_cast<float*>(smem_b + (size_t)p.b_stages * b_stage_bytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg_all) + kStgBytes);
     uint64_t* a_full = bars;
     uint64_t* a_empty = bars + 2;
     uint64_t* b_full = bars + 4;
     uint64_t* b_empty = bars + 4 + kCzMaxBStages;
-    uint64_t* tmem_full_bar = bars + 4 + 2 * kCzMaxBStages;
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-    uint64_t* slot_ready = tmem_empty_bar + 2;  // [2 groups][4 chunks]: staging buffer free (and its residual tile landed)
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(slot_ready + 8);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kNumEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-        if (p.tma_epi) {
-            tma_prefetch_desc(&tmO);
-            if (p.residual) tma_prefetch_desc(&tmR);
-        }
-        for (int i = 0; i < 8; ++i) mbar_init(&slot_ready[i], 1);
         for (int i = 0; i < 2; ++i) {
             mbar_init(&a_full[i], 1);
-            mbar_init(&a_empty[i], 1);
-            mbar_init(&tmem_full_bar[i], 1);
-            mbar_init(&tmem_empty_bar[i], kNumEpiWarps * (kPair ? 2 : 1));  // pair: both CTAs' epilogues release the leader's MMA
+            mbar_init(&a_empty[i], 2);  // one arrival per consumer warpgroup
         }
         for (int i = 0; i < p.b_stages; ++i) {
             mbar_init(&b_full[i], 1);
-            mbar_init(&b_empty[i], 1);
+            mbar_init(&b_empty[i], 2);
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        if (kPair) {
-            tmem_alloc_pair(tmem_ptr_smem, 512);
-            tmem_relinquish_pair();
-        } else {
-            tmem_alloc(tmem_ptr_smem, 512);
-            tmem_relinquish();
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    if (kPair) cluster_sync_all();  // the peer's barriers exist before anything is signalled across the pair
 
-    const long long num_tiles = p.num_m_tiles * p.num_n_tiles;   // pair mode: tiles of 256 rows, 128 per CTA
-    const int tile_rows = p.mt * kBlockM * (kPair ? 2 : 1);
-    const int cta_row0 = kPair ? (int)cta_rank * kBlockM : 0;      // this CTA's first row inside a tile
-    const long long tile_begin = kPair ? (long long)(blockIdx.x >> 1) : (long long)blockIdx.x;
-    const long long tile_step = kPair ? (long long)(gridDim.x >> 1) : (long long)gridDim.x;
+    const long long num_tiles = p.num_m_tiles * p.num_n_tiles;
+    const long long tile_begin = (long long)blockIdx.x;
+    const long long tile_step = (long long)gridDim.x;
     const int halo = p.Wp + 1;  // rows before / after the tile that the taps reach
 
-    if (warp == 0) {
+    if (warp == kNumEpiWarps) {
         if (lane == 0) {
             // ================= A-span producer =================
             int stage = 0;
@@ -135,264 +94,89 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             bool ok = true;
             for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
                 const long long m_tile = tile / p.num_n_tiles;
-                const long long span0 = m_tile * tile_rows + cta_row0 - halo;
+                const long long span0 = m_tile * kBlockM - halo;
                 for (int cb = 0; cb < p.cin_blocks; ++cb) {
                     if (!(ok = mbar_wait(&a_empty[stage], phase ^ 1u, 0x110u))) break;
-                    // pair: the leader's barrier collects the bytes of BOTH CTAs' spans
-                    if (leader) mbar_expect_tx(&a_full[stage], (uint32_t)p.a_stage_bytes * (kPair ? 2u : 1u));
+                    mbar_expect_tx(&a_full[stage], (uint32_t)p.a_stage_bytes);
                     uint8_t* sa = smem_a + (size_t)stage * p.a_stage_bytes;
-                    for (int b = 0; b < p.a_boxes; ++b) {
-                        if (kPair) tma_load_2d_pair(sa + (size_t)b * p.a_box_rows * 128, &tmA, &a_full[stage], cb * kBlockK, (int)(span0 + (long long)b * p.a_box_rows));
-                        else tma_load_2d(sa + (size_t)b * p.a_box_rows * 128, &tmA, &a_full[stage], cb * kBlockK, (int)(span0 + (long long)b * p.a_box_rows));
-                    }
+                    for (int b = 0; b < p.a_boxes; ++b)
+                        tma_load_2d(sa + (size_t)b * p.a_box_rows * 128, &tmA, &a_full[stage], cb * kBlockK, (int)(span0 + (long long)b * p.a_box_rows));
                     advance(stage, phase, 2);
                 }
             }
         }
-    } else if (warp == 2) {
+    } else if (warp == kNumEpiWarps + 1) {
         if (lane == 0) {
             // ================= weight producer =================
             int stage = 0;
             uint32_t phase = 0;
             bool ok = true;
             for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
-                const int n0 = (int)(tile % p.num_n_tiles) * p.block_n + (int)(cta_rank * b_rows);  // pair: this CTA's half of the rows
+                const int n0 = (int)(tile % p.num_n_tiles) * BN;
                 for (int cb = 0; cb < p.cin_blocks && ok; ++cb) {
                     for (int tap = 0; tap < 9; ++tap) {
                         if (!(ok = mbar_wait(&b_empty[stage], phase ^ 1u, 0x120u))) break;
-                        if (leader) mbar_expect_tx(&b_full[stage], b_stage_bytes * (kPair ? 2u : 1u));
-                        if (kPair) tma_load_2d_pair(smem_b + (size_t)stage * b_stage_bytes, &tmB, &b_full[stage], tap * p.cin + cb * kBlockK, n0);
-                        else tma_load_2d(smem_b + (size_t)stage * b_stage_bytes, &tmB, &b_full[stage], tap * p.cin + cb * kBlockK, n0);
+                        mbar_expect_tx(&b_full[stage], b_stage_bytes);
+                        tma_load_2d(smem_b + (size_t)stage * b_stage_bytes, &tmB, &b_full[stage], tap * p.cin + cb * kBlockK, n0);
                         advance(stage, phase, p.b_stages);
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && leader) {
-            // ================= MMA issuer (pair: the leader CTA issues for both SMs) =================
-            const uint32_t idesc = umma_idesc_bf16(kPair ? 2 * kBlockM : kBlockM, p.block_n);
-            int astage = 0, bstage = 0;
-            uint32_t aphase_s = 0, bphase = 0;
-            int local = 0;
-            bool ok = true;
-            for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step, ++local) {
-                const int as = local & 1;
-                const uint32_t accphase = (uint32_t)(local >> 1) & 1u;
-                if (!(ok = mbar_wait(&tmem_empty_bar[as], accphase ^ 1u, 0x210u))) break;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(as * kAccStageCols);
-                for (int cb = 0; cb < p.cin_blocks && ok; ++cb) {
-                    if (!(ok = mbar_wait(&a_full[astage], aphase_s, 0x310u))) break;
-                    tc_fence_after();
-                    const uint32_t a_base = smem_u32(smem_a + (size_t)astage * p.a_stage_bytes);
-                    for (int tap = 0; tap < 9; ++tap) {
-                        if (!(ok = mbar_wait(&b_full[bstage], bphase, 0x320u))) break;
-                        tc_fence_after();
-                        const uint32_t b_addr = smem_u32(smem_b + (size_t)bstage * b_stage_bytes);
-                        const int row_off = (tap / 3) * p.Wp + (tap % 3);  // (dy+1)*Wp + (dx+1)
-                        if (kPair) {
-                            const uint32_t a_addr = a_base + (uint32_t)row_off * 128u;
-#pragma unroll
-                            for (int k = 0; k < kBlockK / 16; ++k)
-                                umma_bf16_pair(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc,
-                                               (uint32_t)((cb | tap | k) != 0));
-                        } else {
-                            for (int j = 0; j < p.mt; ++j) {
-                                const uint32_t a_addr = a_base + (uint32_t)(row_off + j * kBlockM) * 128u;
-#pragma unroll
-                                for (int k = 0; k < kBlockK / 16; ++k)
-                                    umma_bf16(d_tmem + (uint32_t)(j * p.block_n), umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32),
-                                              idesc, (uint32_t)((cb | tap | k) != 0));
-                            }
-                        }
-                        if (kPair) umma_commit_pair(&b_empty[bstage], 3);  // frees the slot in both CTAs
-                        else umma_commit(&b_empty[bstage]);
-                        advance(bstage, bphase, p.b_stages);
-                    }
-                    if (!ok) break;
-                    if (kPair) umma_commit_pair(&a_empty[astage], 3);
-                    else umma_commit(&a_empty[astage]);
-                    advance(astage, aphase_s, 2);
-                }
-                if (ok) {
-                    if (kPair) umma_commit_pair(&tmem_full_bar[as], 3);  // both CTAs' epilogues read their own 128 rows
-                    else umma_commit(&tmem_full_bar[as]);
-                }
-            }
-        }
-    } else if (kPair && p.tma_epi) {
-        // ================= epilogue (warps 3..10), shared-memory staged: TMA store of the output, TMA prefetch of the residual ======
-        // Round-1 ncu: with per-thread 16-byte global stores / residual loads every epilogue instruction touches 32 different
-        // 128-byte lines (32 L1 wavefronts), on the pipe the UMMA operand fetch needs (l1tex lsu 34-60 %, tensor pipe 71-79 %).
-        // Here a group of 4 warps (128 rows) owns one 128 x 32-channel staging buffer per column chunk (64-byte rows, SWIZZLE_64B:
-        // conflict-free 16-byte accesses): the residual chunk of the NEXT tile is TMA-loaded into the buffer as soon as the
-        // previous store has drained it, the threads add it and overwrite it IN PLACE with the output, one thread issues the TMA
-        // store.  Per chunk: 8 shared-memory instructions of 4 wavefronts instead of 8 global ones of 32.
-        const int ew = warp - 3;
-        const int quarter = warp & 3;
-        const int grp = ew >> 2;  // column half
-        const int nchunks = p.block_n >> 5;
+    } else {
+        // ================= wgmma + epilogue (warps 0..7) =================
+        const int wg = warp >> 2;                     // warpgroup: rows 64*wg .. 64*wg+63 of the tile
+        const int quarter = 2 * wg + (warp & 1);
+        const int grp = (warp >> 1) & 1;              // column half
+        float* stg = stg_all + (size_t)wg * 64 * kStgPitch;
+        const float* my_row = stg + (size_t)((warp & 1) * 32 + lane) * kStgPitch;
+        const int nchunks = BN >> 5;
         const int c_begin = grp == 0 ? 0 : (nchunks + 1) >> 1;
         const int c_end = grp == 0 ? (nchunks + 1) >> 1 : nchunks;
         const int P = p.num_n_tiles * 2;
-        const int r_local = quarter * 32 + lane;
-        const bool leader_t = ((ew & 3) == 0) && lane == 0;
-        uint8_t* stg = smem_stage + (size_t)grp * 4 * kCzStgChunk;
-        uint64_t* slot = slot_ready + grp * 4;
-        const uint32_t my_row = smem_u32(stg) + (uint32_t)r_local * 64u;
-        const uint32_t swz = (uint32_t)((r_local >> 1) & 3);
-        auto setup_slot = [&](int j, long long tile) {  // leader only: buffer j is free -> arm it for `tile`
-            if (tile >= num_tiles) return;
-            if (p.residual) {
-                const long long m_tile = tile / p.num_n_tiles;
-                const int n0 = (int)(tile % p.num_n_tiles) * p.block_n;
-                mbar_expect_tx(&slot[j], (uint32_t)kCzStgChunk);
-                tma_load_2d(stg + (size_t)j * kCzStgChunk, &tmR, &slot[j], n0 + (c_begin + j) * 32, (int)(m_tile * tile_rows + cta_row0));
-            } else {
-                mbar_arrive(&slot[j]);
-            }
-        };
-        if (leader_t)
-            for (int j = 0; j < c_end - c_begin; ++j) setup_slot(j, tile_begin);
-        int local = 0;
-        bool ok = true;
-        for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step, ++local) {
-            const long long m_tile = tile / p.num_n_tiles;
-            const int n_tile = (int)(tile % p.num_n_tiles);
-            const int n0 = n_tile * p.block_n;
-            const int as = local & 1;
-            const uint32_t accphase = (uint32_t)(local >> 1) & 1u;
-            const long long row0 = m_tile * tile_rows + cta_row0;
-            const long long q = row0 + r_local;
-            const bool row_ok = q < p.Q;
-            const long long f = q / p.FS;
-            const int r = (int)(q - f * p.FS);
-            const int y = r / p.Wp, x = r - y * p.Wp;
-            const bool interior = row_ok && (y < p.H) && (x < p.W);
-            float ga = 1.f, gb = 0.f;
-            if (p.mr != nullptr && interior) {
-                const float mean = __ldg(p.mr + 2 * f), rstd = __ldg(p.mr + 2 * f + 1);
-                ga = rstd;
-                gb = rstd * mean;
-            }
-            const int cy = (y == 0) ? 0 : ((y == p.H - 1) ? 2 : 1);
-            const int cx = (x == 0) ? 0 : ((x == p.W - 1) ? 2 : 1);
-            const int cls = interior ? cy * 3 + cx : 0;
-            const float* s1row = p.S1 ? p.S1 + (size_t)cls * p.N : nullptr;
-            const float* s2row = p.S2 ? p.S2 + (size_t)cls * p.N : nullptr;
-            if (p.Ef) {  // per-frame fold table: out = ga * acc + Ef[f][cls][c]
-                s1row = nullptr;
-                s2row = p.Ef + ((size_t)(interior ? f : 0) * 9 + cls) * p.N;
-            }
-            const float* rarow = (p.res_scale && interior) ? p.res_scale + (size_t)f * p.N : nullptr;
-            const float* rbrow = (p.res_scale && interior) ? p.res_shift + (size_t)f * p.N : nullptr;
-            float st_s = 0.f, st_ss = 0.f;
-            if (!(ok = mbar_wait(&tmem_full_bar[as], accphase, 0x410u))) break;
-            tc_fence_after();
-            for (int c = c_begin; c < c_end && ok; ++c) {
-                const int j = c - c_begin;
-                uint32_t acc[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * kAccStageCols + c * 32), acc);
-                tmem_ld_wait();
-                if (c == c_end - 1) {  // accumulator stage fully read: release it to the MMA warp
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive_cluster(&tmem_empty_bar[as], 0);
-                }
-                const int nb = n0 + c * 32;
-                float v[32];
-#pragma unroll
-                for (int qq = 0; qq < 8; ++qq) {
-                    const float4 a1 = s1row ? __ldg(reinterpret_cast<const float4*>(s1row + nb) + qq) : make_float4(0, 0, 0, 0);
-                    const float4 a2 = s2row ? __ldg(reinterpret_cast<const float4*>(s2row + nb) + qq) : make_float4(0, 0, 0, 0);
-                    v[4 * qq + 0] = fmaf(ga, __uint_as_float(acc[4 * qq + 0]), fmaf(-gb, a1.x, a2.x));
-                    v[4 * qq + 1] = fmaf(ga, __uint_as_float(acc[4 * qq + 1]), fmaf(-gb, a1.y, a2.y));
-                    v[4 * qq + 2] = fmaf(ga, __uint_as_float(acc[4 * qq + 2]), fmaf(-gb, a1.z, a2.z));
-                    v[4 * qq + 3] = fmaf(ga, __uint_as_float(acc[4 * qq + 3]), fmaf(-gb, a1.w, a2.w));
-                }
-                if (p.relu == 1) {
-#pragma unroll
-                    for (int jj = 0; jj < 32; ++jj) v[jj] = fmaxf(v[jj], 0.f);
-                }
-                // the staging buffer is free (its previous store has drained) and, with a residual, holds this tile's residual chunk
-                if (!mbar_wait(&slot[j], (uint32_t)local & 1u, 0x420u)) asm volatile("trap;");  // (a break would desynchronise the named barrier)
-                const uint32_t brow = my_row + (uint32_t)j * kCzStgChunk;
-                if (p.residual != nullptr) {
-#pragma unroll
-                    for (int qq = 0; qq < 4; ++qq) {
-                        uint4 rr;
-                        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rr.x), "=r"(rr.y), "=r"(rr.z), "=r"(rr.w) : "r"(brow + (((uint32_t)qq ^ swz) << 4)));
-                        float r8[8] = {bf16_lo(rr.x), bf16_hi(rr.x), bf16_lo(rr.y), bf16_hi(rr.y), bf16_lo(rr.z), bf16_hi(rr.z), bf16_lo(rr.w), bf16_hi(rr.w)};
-                        if (rarow) {  // residual stream recomputed from the un-normalised tensor: a[f][c] * r + b[f][c]
-                            const float4 a0 = __ldg(reinterpret_cast<const float4*>(rarow + nb + 8 * qq)), a1 = __ldg(reinterpret_cast<const float4*>(rarow + nb + 8 * qq) + 1);
-                            const float4 b0 = __ldg(reinterpret_cast<const float4*>(rbrow + nb + 8 * qq)), b1 = __ldg(reinterpret_cast<const float4*>(rbrow + nb + 8 * qq) + 1);
-                            r8[0] = fmaf(a0.x, r8[0], b0.x); r8[1] = fmaf(a0.y, r8[1], b0.y); r8[2] = fmaf(a0.z, r8[2], b0.z); r8[3] = fmaf(a0.w, r8[3], b0.w);
-                            r8[4] = fmaf(a1.x, r8[4], b1.x); r8[5] = fmaf(a1.y, r8[5], b1.y); r8[6] = fmaf(a1.z, r8[6], b1.z); r8[7] = fmaf(a1.w, r8[7], b1.w);
-                        }
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) v[8 * qq + e] += r8[e];
-                    }
-                }
-                if (p.relu == 2) {
-#pragma unroll
-                    for (int jj = 0; jj < 32; ++jj) v[jj] = fmaxf(v[jj], 0.f);
-                }
-                uint32_t pk[16];
-#pragma unroll
-                for (int jj = 0; jj < 16; ++jj) pk[jj] = interior ? pack_bf16(v[2 * jj], v[2 * jj + 1]) : 0u;  // ZP zero row / column
-                if (p.stat_part) {
-#pragma unroll
-                    for (int jj = 0; jj < 16; ++jj) {
-                        const float lo = bf16_lo(pk[jj]), hi = bf16_hi(pk[jj]);
-                        st_s += lo + hi;
-                        st_ss = fmaf(lo, lo, fmaf(hi, hi, st_ss));
-                    }
-                }
-#pragma unroll
-                for (int qq = 0; qq < 4; ++qq)
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(brow + (((uint32_t)qq ^ swz) << 4)), "r"(pk[4 * qq]), "r"(pk[4 * qq + 1]),
-                                 "r"(pk[4 * qq + 2]), "r"(pk[4 * qq + 3])
-                                 : "memory");
-                fence_proxy_async();              // generic-proxy writes -> visible to the TMA store (async proxy)
-                named_bar_sync(1 + grp, 128);     // the whole 128 x 32 chunk is in shared memory
-                if (leader_t) {
-                    tma_store_2d(&tmO, stg + (size_t)j * kCzStgChunk, nb, (int)row0);  // rows >= Q are clipped by TMA
-                    bulk_commit();
-                    if (j > 0) {
-                        bulk_wait_read<1>();      // the previous chunk's store has drained its buffer
-                        setup_slot(j - 1, tile + tile_step);
-                    }
-                }
-            }
-            if (!ok) break;
-            if (leader_t) {
-                bulk_wait_read<0>();
-                setup_slot(c_end - c_begin - 1, tile + tile_step);
-            }
-            if (p.stat_part && row_ok) reinterpret_cast<float2*>(p.stat_part)[(size_t)q * P + n_tile * 2 + grp] = make_float2(st_s, st_ss);
-        }
-        if (leader_t) bulk_wait_all<0>();
-    } else {
-        // ================= epilogue (warps 3..10) =================
-        const int ew = warp - 3;
-        const int quarter = warp & 3;
-        const int grp = ew >> 2;  // mt == 1: column half; mt == 2: 128-row sub-tile
-        const int sub = (p.mt == 2) ? grp : 0;
-        const int nchunks = (p.block_n + 31) >> 5;
-        const int c_begin = (p.mt == 2 || grp == 0) ? 0 : (nchunks + 1) >> 1;
-        const int c_end = (p.mt == 2) ? nchunks : (grp == 0 ? (nchunks + 1) >> 1 : nchunks);
-        const int P = p.num_n_tiles * 2;
         const bool tab_vec = ((p.N & 3) == 0);
-        int local = 0;
+        const bool leader = (threadIdx.x & 127) == 0;
+        int astage = 0, bstage = 0;
+        uint32_t aphase = 0, bphase = 0;
         bool ok = true;
-        for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step, ++local) {
+        for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
             const long long m_tile = tile / p.num_n_tiles;
             const int n_tile = (int)(tile % p.num_n_tiles);
-            const int n0 = n_tile * p.block_n;
-            const int as = local & 1;
-            const uint32_t accphase = (uint32_t)(local >> 1) & 1u;
-            const long long q = m_tile * tile_rows + cta_row0 + sub * kBlockM + quarter * 32 + lane;
+            const int n0 = n_tile * BN;
+            // ---- main loop: 64 rows x BN channels of this warpgroup over (channel block, tap)
+            float frag[BN / 64][32];
+            for (int cb = 0; cb < p.cin_blocks && ok; ++cb) {
+                if (!(ok = mbar_wait(&a_full[astage], aphase, 0x310u))) break;
+                const uint32_t a_base = smem_u32(smem_a + (size_t)astage * p.a_stage_bytes) + (uint32_t)wg * 64u * 128u;
+                int prev = -1;
+                for (int tap = 0; tap < 9; ++tap) {
+                    if (!(ok = mbar_wait(&b_full[bstage], bphase, 0x320u))) break;
+                    const uint32_t b_addr = smem_u32(smem_b + (size_t)bstage * b_stage_bytes);
+                    const int row_off = (tap / 3) * p.Wp + (tap % 3);  // (dy+1)*Wp + (dx+1)
+                    const uint32_t a_addr = a_base + (uint32_t)row_off * 128u;
+                    const uint64_t a_bo = p.bo ? ((uint64_t)((a_addr >> 7) & 7u) << 49) : 0ull;
+                    wgmma_fence();
+                    wg_mma_kblock<false, BN>(frag, a_addr, b_addr, a_bo, (cb | tap) != 0);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (prev >= 0 && leader) mbar_arrive(&b_empty[prev]);
+                    prev = bstage;
+                    advance(bstage, bphase, p.b_stages);
+                }
+                wgmma_wait<0>();
+                if (prev >= 0 && leader) mbar_arrive(&b_empty[prev]);
+                if (leader) mbar_arrive(&a_empty[astage]);
+                advance(astage, aphase, 2);
+            }
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j) wgmma_reg_fence(frag[j]);
+            if (!ok) break;
+            named_bar_sync(1 + wg, 128);
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j) wgmma_frag_store(frag[j], stg, kStgPitch, j * 64);
+            named_bar_sync(1 + wg, 128);
+
+            const long long q = m_tile * kBlockM + quarter * 32 + lane;
             const bool row_ok = q < p.Q;
             // decode the ZP row: frame, y, x
             const long long f = q / p.FS;
@@ -418,15 +202,12 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const float* rbrow = (p.res_scale && interior) ? p.res_shift + (size_t)f * p.N : nullptr;
             float st_s = 0.f, st_ss = 0.f;
 
-            if (!(ok = mbar_wait(&tmem_full_bar[as], accphase, 0x410u))) break;
-            tc_fence_after();
             for (int c = c_begin; c < (p.dbg == 2 ? c_begin : c_end); ++c) {
-                uint32_t acc[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * kAccStageCols + sub * p.block_n + c * 32), acc);
-                tmem_ld_wait();
                 const int nb = n0 + c * 32;
-                const int lim = min(32, min(p.block_n - c * 32, p.N - nb));
+                const int lim = min(32, min(BN - c * 32, p.N - nb));
                 if (!row_ok || lim <= 0) continue;
+                uint32_t acc[32];
+                stg_ld_32(my_row + c * 32, acc);
                 __nv_bfloat16* op = p.out + (size_t)q * p.N + nb;
                 const bool full = (lim == 32) && ((p.N & 7) == 0);
                 if (!interior) {  // zero row / column of the ZP layout
@@ -512,53 +293,22 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         if (j < lim) op[j] = __float2bfloat16_rn(v[j]);
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (kPair) mbar_arrive_cluster(&tmem_empty_bar[as], 0);  // the leader's MMA thread waits on its own barrier
-                else mbar_arrive(&tmem_empty_bar[as]);
-            }
-            if (p.stat_part && row_ok) {
-                float2* sp = reinterpret_cast<float2*>(p.stat_part) + (size_t)q * P + n_tile * 2;
-                if (p.mt == 2) {
-                    sp[0] = make_float2(st_s, st_ss);
-                    sp[1] = make_float2(0.f, 0.f);
-                } else {
-                    sp[grp] = make_float2(st_s, st_ss);
-                }
-            }
+            if (p.stat_part && row_ok) reinterpret_cast<float2*>(p.stat_part)[(size_t)q * P + n_tile * 2 + grp] = make_float2(st_s, st_ss);
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (kPair) cluster_sync_all();  // both CTAs are done with TMEM and with each other's barriers
-    if (warp == 1) {
-        tc_fence_after();
-        if (kPair) tmem_dealloc_pair(tmem_base, 512);
-        else tmem_dealloc(tmem_base, 512);
     }
 }
 
 }  // namespace vpt
 
 namespace vpt {
-extern int g_cz_swap_enabled();
-int launch_conv_zp_t_fwd(const vpt_conv_zp_args* a, void* stream);
-}  // namespace vpt
-
-namespace vpt {
-// Weight-tile width.  A handful of frames (rollout: F = 1, 1089 rows at 32 x 32): the launch is a read of the 1.2 MB weight tensor through
-// the few SMs that have a tile, so narrower weight tiles put more SMs (each fetching a slice) on it -- ~64 CTAs instead of 5.
-static inline bool conv_zp_use_swapped(long long Q) { return (Q + 255) / 256 >= 32; }
+// Weight-tile width.  A handful of frames (rollout: F = 1, 1089 rows at 32 x 32): the launch is a read of the weight tensor through
+// the few SMs that have a tile, so narrower weight tiles put more SMs (each fetching a slice) on it.
 static inline void conv_zp_block_n(long long Q, int N, int* bn, int* nt) {
     choose_block_n(N, bn, nt);
-    const long long tiles = (Q + 255) / 256;
-    if (tiles * *nt >= 32) return;
-    const int want = (int)((64 + tiles - 1) / tiles);
-    int t = *nt;
-    while (t < want && N % (2 * t) == 0 && N / (2 * t) >= 32 && (N / (2 * t)) % 16 == 0) t *= 2;
-    if (N % t == 0) { *nt = t; *bn = N / t; }
+    const long long tiles = (Q + kBlockM - 1) / kBlockM;
+    if (tiles * *nt >= 64 || *bn == 64) return;
+    *bn = 64;
+    *nt = (N + 63) / 64;
 }
 }  // namespace vpt
 
@@ -568,11 +318,9 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     const int H = a->H, W = a->W, C = a->Cin, N = a->Cout;
     VPT_CHECK(a->F > 0 && H >= 2 && W >= 2 && C > 0 && C % 64 == 0 && N > 0 && N % 16 == 0,
               "vpt_conv3x3_zp: need F>0, H,W>=2, Cin %% 64 == 0, Cout %% 16 == 0 (F=%d H=%d W=%d Cin=%d Cout=%d)", a->F, H, W, C, N);
-    VPT_CHECK(W + 1 <= 255, "vpt_conv3x3_zp: W=%d too wide for one shared-memory span", W);
+    // two stages of the 128 + 2*(W+2)-row input span, the fp32 staging tiles and two weight stages must fit in shared memory
+    VPT_CHECK(W <= 182, "vpt_conv3x3_zp: W=%d too wide (at most 182: two input spans of 128 + 2*(W+2) rows must fit in shared memory)", W);
     VPT_CHECK(((uintptr_t)a->x & 15) == 0 && ((uintptr_t)a->w & 15) == 0 && ((uintptr_t)a->out & 15) == 0, "vpt_conv3x3_zp: pointers must be 16-byte aligned");
-    // operand-swapped kernel (conv_zp_t.cuh) for Cout == 128 -- except for a handful of frames: a 256-pixel tile is a serial chain of 72 UMMAs
-    // of ~204 cycles on 17 SMs, 128-row tiles with 32-channel weight slices are 72 UMMAs of ~92 cycles on 136
-    if (N == 128 && g_cz_swap_enabled() && conv_zp_use_swapped((long long)a->F * (H + 1) * (W + 1))) return launch_conv_zp_t_fwd(a, stream);
     ConvZpParams p;
     memset(&p, 0, sizeof(p));
     p.H = H; p.W = W; p.Wp = W + 1; p.FS = (H + 1) * (W + 1);
@@ -580,45 +328,21 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     VPT_CHECK(p.Q < 2147483647LL, "vpt_conv3x3_zp: too many rows for 32-bit TMA coordinates");
     p.N = N; p.cin = C; p.cin_blocks = C / 64;
     conv_zp_block_n(p.Q, N, &p.block_n, &p.num_n_tiles);
-    // measured (tools/conv_bench.py): SM pairs win for 256-wide weight tiles (+11-13 %), a single CTA with two 128-row
-    // sub-tiles wins for <= 128 output channels; g_cz_pair: 0 = never, 1 = auto, 2 = always
-    const bool pair = (g_cz_pair == 2 || (g_cz_pair == 1 && p.block_n > 128)) && (p.block_n % 16 == 0) && (p.Q > 256);
-    // two 128-row sub-tiles per CTA amortise the weight tile -- unless the launch is tiny (single frame): then the tile's UMMA chain IS the
-    // launch time (144 instructions of >= 84 cycles at K = 2304), and one sub-tile per CTA halves it
-    p.mt = (!pair && p.block_n <= 128 && (p.Q + 255) / 256 >= 32) ? 2 : 1;
-    const int cta_rows = p.mt * kBlockM;                  // rows per CTA per tile
-    const int tile_rows = cta_rows * (pair ? 2 : 1);
-    p.num_m_tiles = (p.Q + tile_rows - 1) / tile_rows;
-    const int span = cta_rows + 2 * (p.Wp + 1);
+    p.num_m_tiles = (p.Q + kBlockM - 1) / kBlockM;
+    const int span = kBlockM + 2 * (p.Wp + 1);
     p.a_boxes = (span + 255) / 256;
     p.a_box_rows = ((span + p.a_boxes - 1) / p.a_boxes + 7) / 8 * 8;
     VPT_CHECK(p.a_box_rows <= 256, "vpt_conv3x3_zp: span does not fit the TMA box limit");
     p.a_stage_bytes = p.a_boxes * p.a_box_rows * 128;
-    const uint32_t b_stage_bytes = (uint32_t)(p.block_n / (pair ? 2 : 1)) * kBlockK * 2;
-    p.tma_epi = (pair && g_cz_tma && g_cz_dbg == 0 && N % 32 == 0 && p.block_n % 64 == 0 && ((uintptr_t)a->out & 127) == 0 &&
-                 (!a->residual || ((uintptr_t)a->residual & 127) == 0)) ? 1 : 0;
-    const long long budget = 225 * 1024 - 1024 - 2 * (long long)p.a_stage_bytes - 512 - (p.tma_epi ? kCzStgBytes : 0);
-    int bst = (int)(budget / b_stage_bytes);
+    const uint32_t b_stage_bytes = (uint32_t)p.block_n * kBlockK * 2;
+    const size_t fixed_bytes = 1024 + 2 * (size_t)p.a_stage_bytes + kStgBytes + (4 + 2 * kCzMaxBStages) * 8;
+    int bst = (int)((227 * 1024 - (long long)fixed_bytes) / b_stage_bytes);
     if (bst > kCzMaxBStages) bst = kCzMaxBStages;
     VPT_CHECK(bst >= 2, "vpt_conv3x3_zp: not enough shared memory for the weight pipeline (W=%d Cout=%d)", W, N);
     p.b_stages = bst;
-    const size_t smem_bytes = 1024 + 2 * (size_t)p.a_stage_bytes + (size_t)bst * b_stage_bytes + (p.tma_epi ? kCzStgBytes : 0) +
-                              (4 + 2 * kCzMaxBStages + 4 + 8) * 8 + 16;
+    const size_t smem_bytes = fixed_bytes + (size_t)bst * b_stage_bytes;
 
-    CUtensorMap tmA, tmB, tmO, tmR;
-    memset(&tmO, 0, sizeof(tmO));
-    memset(&tmR, 0, sizeof(tmR));
-    if (p.tma_epi) {  // output / residual: [Q][N] bf16, boxes of 128 rows x 32 channels (64-byte rows, SWIZZLE_64B)
-        cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)p.Q};
-        cuuint64_t strides[1] = {(cuuint64_t)N * 2};
-        cuuint32_t box[2] = {32, (cuuint32_t)kBlockM};
-        int r = make_tmap_bf16(&tmO, a->out, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
-        if (r) return r;
-        if (a->residual) {
-            r = make_tmap_bf16(&tmR, a->residual, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
-            if (r) return r;
-        }
-    }
+    CUtensorMap tmA, tmB;
     {
         cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)p.Q};
         cuuint64_t strides[1] = {(cuuint64_t)C * 2};
@@ -629,7 +353,7 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     {
         cuuint64_t dims[2] = {(cuuint64_t)9 * C, (cuuint64_t)N};
         cuuint64_t strides[1] = {(cuuint64_t)9 * C * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)(p.block_n / (pair ? 2 : 1))};
+        cuuint32_t box[2] = {64, (cuuint32_t)p.block_n};
         int r = make_tmap_bf16(&tmB, a->w, 2, dims, strides, box);
         if (r) return r;
     }
@@ -643,67 +367,52 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     p.stat_part = a->stat_part;
     p.Ef = a->Ef; p.res_scale = a->res_scale; p.res_shift = a->res_shift;
     p.dbg = g_cz_dbg;
+    p.bo = g_dbg_bo > 0 ? 1 : 0;
 
     static bool attr_set = false;
     if (!attr_set) {
-        VPT_CUDA(cudaFuncSetAttribute(conv3x3_zp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        VPT_CUDA(cudaFuncSetAttribute(conv3x3_zp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(conv3x3_zp_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(conv3x3_zp_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
     const long long tiles = p.num_m_tiles * p.num_n_tiles;
-    if (!pair) {
-        long long grid = num_sms();
-        if (grid <= 0) grid = 148;
-        if (grid > tiles) grid = tiles;
-        launch_k(conv3x3_zp_kernel<false>, dim3((unsigned)grid), dim3(kCzThreads), smem_bytes, (cudaStream_t)stream, tmA, tmB, tmO, tmR, p);
-        VPT_LAUNCH_CHECK();
-        return VPT_OK;
-    }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.blockDim = dim3(kCzThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // (see pdl_sync() in common.cuh)
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    static int max_pairs = 0;
-    if (max_pairs == 0) {
-        int n = 0;
-        cfg.gridDim = dim3(num_sms() / 2 * 2);
-        cudaError_t e = cudaOccupancyMaxActiveClusters(&n, conv3x3_zp_kernel<true>, &cfg);
-        if (e != cudaSuccess || n <= 0) {
-            (void)cudaGetLastError();
-            n = num_sms() / 2;
-        }
-        max_pairs = n;
-    }
-    long long pairs = max_pairs;
-    if (pairs > tiles) pairs = tiles;
-    cfg.gridDim = dim3((unsigned)(pairs * 2));
-    cfg.numAttrs = g_pdl ? 2 : 1;
-    VPT_CUDA(cudaLaunchKernelEx(&cfg, conv3x3_zp_kernel<true>, tmA, tmB, tmO, tmR, p));
+    long long grid = num_sms();
+    if (grid <= 0) grid = 132;
+    if (grid > tiles) grid = tiles;
+    if (p.block_n == 64)
+        launch_k(conv3x3_zp_kernel<64>, dim3((unsigned)grid), dim3(kCzThreads), smem_bytes, (cudaStream_t)stream, tmA, tmB, p);
+    else
+        launch_k(conv3x3_zp_kernel<128>, dim3((unsigned)grid), dim3(kCzThreads), smem_bytes, (cudaStream_t)stream, tmA, tmB, p);
+    VPT_LAUNCH_CHECK();
     return VPT_OK;
 }
 
+// Kernel-variant knobs of the C ABI.  This build has one convolution kernel (no CTA-pair or operand-swapped variant), so only the
+// epilogue experiment level (bits 4..7 of the pair mode, tools/conv_bench.py) has an effect; with swap mode 0 everywhere the
+// swapped kernel's statistics layout never applies.
 extern "C" int vpt_set_conv_pair_mode(int32_t on) {
-    vpt::g_cz_tma = (on & 0x100) ? 0 : 1;  // bit 8: disable the TMA-store epilogue (A/B knob)
-    on &= 0xff;
-    vpt::g_cz_dbg = on >> 4;  // bits 4..7: epilogue experiment level (tools/conv_bench.py)
-    on &= 15;
-    vpt::g_cz_pair = on;
+    vpt::g_cz_dbg = (on & 0xff) >> 4;
     return VPT_OK;
+}
+
+extern "C" int vpt_set_conv_swap_mode(int32_t on) {
+    (void)on;
+    return VPT_OK;
+}
+
+extern "C" int64_t vpt_conv_zp_t_stat_floats(int32_t F, int32_t H, int32_t W, int32_t Cout) {
+    (void)F; (void)H; (void)W; (void)Cout;
+    return 0;
+}
+
+extern "C" int vpt_conv_zp_t_stats_finalize(const float* part, float* mr, int32_t F, int32_t H, int32_t W, float eps, void* stream) {
+    (void)part; (void)mr; (void)F; (void)H; (void)W; (void)eps; (void)stream;
+    vpt::set_error("vpt_conv_zp_t_stats_finalize: no convolution kernel of this build emits per-tile partials (vpt_conv_zp_t_stat_floats is 0)");
+    return VPT_ERR_ARG;
 }
 
 extern "C" int vpt_conv_zp_stat_parts(int32_t F, int32_t H, int32_t W, int32_t Cout) {
     const long long Q = (long long)F * (H + 1) * (W + 1);
-    if (Cout == 128 && vpt::g_cz_swap_enabled() && vpt::conv_zp_use_swapped(Q)) return 1;  // swapped kernel: complete row sums (see vpt_conv_zp_t_stat_floats)
     int bn, nt;
     vpt::conv_zp_block_n(Q, Cout, &bn, &nt);
     return nt * 2;

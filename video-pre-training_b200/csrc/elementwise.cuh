@@ -106,7 +106,7 @@ __device__ __forceinline__ uint32_t bf16x2_max(uint32_t a, uint32_t b) {
 // chan_part (optional, needs 256 % C8 == 0 so that a thread keeps one channel group): float2 [F][gridDim.x][C] per-CHANNEL (sum, sumsq)
 // partials of the pooled values -- what the two-norm composition (vpt_norm2_fold) needs instead of a normalisation pass.
 // (CHAN keeps 16 more accumulators: 48 registers -> 5 resident blocks instead of 8, and this kernel lives on loads in flight; two
-//  items per trip and a 4-block bound give each thread twice the loads instead -- measured in profiles/fold_r2.md)
+//  items per trip and a 4-block bound give each thread twice the loads instead)
 // One thread = one 8-channel group of a 2 x 2 block of outputs: the 5 x 5 input window is read once (6.25 loads per output instead of 9)
 // and the maximum is separable -- per input row two horizontal 3-maxima, folded into the two output rows that row belongs to.
 template <bool CHAN>

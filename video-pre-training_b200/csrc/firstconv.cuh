@@ -1,7 +1,7 @@
 // Stack-0 first convolution, fully fused: u8 NHWC frame -> (x/255) conv3x3(3->C0)+bias -> ReLU -> max_pool(3,2,1)
-// -> bf16 NHWC + per-tile statistics partials.
+// -> bf16 NHWC + per-(tile, channel) statistics partials.
 //
-// K = 27 is too small for tcgen05 to matter (the layer is 0.75 % of the FLOPs and bounded by its epilogue / output
+// K = 27 is too small for a warpgroup MMA to matter (the layer is 0.75 % of the FLOPs and bounded by its epilogue / output
 // write), so the contraction runs on warp-level mma.sync m16n8k16: A = the im2col view of the u8 patch (u8 values
 // are exact in bf16; fragments are gathered straight from the patch in shared memory, no im2col copy), B = the fp32
 // weights split as bf16 hi + bf16 lo (K = 27 + 27 -> 64), fp32 accumulate: products are exact and the result is
@@ -9,10 +9,12 @@
 //
 // One CTA = one 8x8 tile of POOLED outputs of one frame = 17x17 conv outputs (19 m16 tiles) from a 19x19x3 patch.
 // ~99 KB of shared memory at C0 = 128 -> two CTAs per SM overlap one CTA's pooling with the other's MMAs.
+// F32OUT (precision mode): the conv tile is kept in fp32 and the output is fp32; the channels then go through the tile 64 at a time.
 #pragma once
+#include <type_traits>
+
 #include "attention.cuh"  // ldsm_x4 / mma_bf16_16816
 #include "common.cuh"
-#include "firstconv_tc.cuh"
 
 namespace vpt {
 
@@ -26,15 +28,19 @@ constexpr int kFcBPitch = 72;                    // bf16 elements per weight row
 constexpr int kFcPatchElems = kFcIn * kFcIn * 3; // 1083
 constexpr int kFcPatchBytes = 2192;              // bf16 patch + one zero element, 16-byte multiple
 
+template <bool F32OUT>
 __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uint8_t* __restrict__ img, const float* __restrict__ w,
-                                                                       const float* __restrict__ bias, __nv_bfloat16* __restrict__ out,
+                                                                       const float* __restrict__ bias, void* __restrict__ out_,
                                                                        float2* __restrict__ stat_part, int H, int W, int C0, long long total_tiles, int zp) {
     pdl_sync();
     extern __shared__ __align__(16) uint8_t fc_smem[];
     __nv_bfloat16* patch = reinterpret_cast<__nv_bfloat16*>(fc_smem);                                  // [19][19][3]
     __nv_bfloat16* Bs = reinterpret_cast<__nv_bfloat16*>(fc_smem + kFcPatchBytes);                     // [C0][72]
-    const int cpitch = C0 + 8;
-    __nv_bfloat16* ctile = Bs + (size_t)C0 * kFcBPitch;                                                // [289][C0+8]
+    using CT = typename std::conditional<F32OUT, float, __nv_bfloat16>::type;
+    const int CB = F32OUT ? 64 : C0;  // channels per pass through the conv tile
+    const int cpitch = CB + 8;
+    CT* ctile = reinterpret_cast<CT*>(Bs + (size_t)C0 * kFcBPitch);                                    // [289][CB+8]
+    CT* const out = reinterpret_cast<CT*>(out_);
     const int tiles_x = (W / 2) / kFcTile, tiles_y = (H / 2) / kFcTile;
     const int tiles = tiles_x * tiles_y;
 
@@ -105,7 +111,10 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
         if (i < kFcPatchElems) patch[i] = __float2bfloat16_rn((float)pre[j]);
     }
     if (tid + gridDim.x < total_tiles) prefetch(tid + gridDim.x);
-    __syncthreads();  // patch (and, first time, weights) visible; previous tile's pooling finished reading ctile
+    const int Ho = H / 2, Wo = W / 2, opitch = Wo + zp;  // ZP layout: one extra zero column / row
+    CT* fout = out + f * (long long)(Ho + zp) * opitch * C0;
+  for (int cg = 0; cg < C0; cg += CB) {
+    __syncthreads();  // patch (and, first time, weights) visible; previous pass's pooling finished reading ctile
 
     for (int mt = warp; mt < kFcMTiles; mt += kFcThreads / 32) {
         // A fragments (rows g and g+8 of this m-tile) for the 4 k-steps, gathered from the patch
@@ -134,7 +143,7 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
             }
         }
         if (tg == 3) af[3][0] = af[3][1] = 0x3F803F80u;  // k = 54, 55: constant 1.0 (x the bias columns of B)
-        for (int nh = 0; nh < C0 / 64; ++nh) {  // 64 output channels at a time
+        for (int nh = cg / 64; nh < (cg + CB) / 64; ++nh) {  // 64 output channels at a time
             float acc[8][4];
 #pragma unroll
             for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
@@ -154,23 +163,37 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 if (pos[rr] >= kFcPos) continue;
-                __nv_bfloat16* crow = ctile + (size_t)pos[rr] * cpitch + nh * 64 + 2 * tg;
+                CT* crow = ctile + (size_t)pos[rr] * cpitch + (nh * 64 - cg) + 2 * tg;
 #pragma unroll
                 for (int nt = 0; nt < 8; ++nt) {
                     const float v0 = inimg[rr] ? acc[nt][2 * rr] : 0.f;
                     const float v1 = inimg[rr] ? acc[nt][2 * rr + 1] : 0.f;
-                    *reinterpret_cast<uint32_t*>(crow + nt * 8) = pack_bf16(v0, v1);
+                    if constexpr (F32OUT) *reinterpret_cast<float2*>(crow + nt * 8) = make_float2(v0, v1);
+                    else *reinterpret_cast<uint32_t*>(crow + nt * 8) = pack_bf16(v0, v1);
                 }
             }
         }
     }
     __syncthreads();
 
-    // ---- 3x3 / stride-2 max over the conv tile, 8 channels (16 B) per item
+    // ---- 3x3 / stride-2 max over the conv tile, 16 B (8 bf16 / 4 fp32 channels) per item
+    if constexpr (F32OUT) {
+        const int C4 = CB / 4;
+        for (int i = threadIdx.x; i < kFcTile * kFcTile * C4; i += kFcThreads) {
+            const int c4 = i % C4, px = (i / C4) % kFcTile, py = i / (C4 * kFcTile);
+            float4 m = make_float4(0.f, 0.f, 0.f, 0.f);  // starting from 0 == applying the ReLU after the max
+#pragma unroll
+            for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+                for (int dx = 0; dx < 3; ++dx) {
+                    const int p = (2 * py + dy) * kFcConv + 2 * px + dx;
+                    const float4 v = *reinterpret_cast<const float4*>(ctile + (size_t)p * cpitch + 4 * c4);
+                    m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
+                }
+            *reinterpret_cast<float4*>(fout + ((long long)(PY0 + py) * opitch + PX0 + px) * C0 + cg + 4 * c4) = m;
+        }
+    } else {
     const int C8 = C0 / 8;
-    float s = 0.f, ss = 0.f;
-    const int Ho = H / 2, Wo = W / 2, opitch = Wo + zp;  // ZP layout: one extra zero column / row
-    __nv_bfloat16* fout = out + f * (long long)(Ho + zp) * opitch * C0;
     for (int i = threadIdx.x; i < kFcTile * kFcTile * C8; i += kFcThreads) {
         const int c8 = i % C8, px = (i / C8) % kFcTile, py = i / (C8 * kFcTile);
         uint4 m = make_uint4(0, 0, 0, 0);  // starting from 0 == applying the ReLU after the max
@@ -184,41 +207,50 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
                 m.z = bf16x2_max(m.z, v.z); m.w = bf16x2_max(m.w, v.w);
             }
         *reinterpret_cast<uint4*>(fout + ((long long)(PY0 + py) * opitch + PX0 + px) * C0 + 8 * c8) = m;
-        const uint32_t w4[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const float a = bf16_lo(w4[q]), b = bf16_hi(w4[q]);
-            s += a + b;
-            ss = fmaf(a, a, fmaf(b, b, ss));
-        }
     }
+    }
+  }
     if (zp) {  // edge tiles write the zero column x = Wo and the zero row y = Ho (plus the corner)
+        const int C8 = C0 * (int)sizeof(CT) / 16;  // 16-byte words per pixel
+        uint4* fo = reinterpret_cast<uint4*>(fout);
         const bool right = (PX0 + kFcTile == Wo), bottom = (PY0 + kFcTile == Ho);
         if (right)
             for (int i = threadIdx.x; i < kFcTile * C8; i += kFcThreads)
-                *reinterpret_cast<uint4*>(fout + ((long long)(PY0 + i / C8) * opitch + Wo) * C0 + 8 * (i % C8)) = make_uint4(0, 0, 0, 0);
+                fo[((long long)(PY0 + i / C8) * opitch + Wo) * C8 + (i % C8)] = make_uint4(0, 0, 0, 0);
         if (bottom)
             for (int i = threadIdx.x; i < (kFcTile + (right ? 1 : 0)) * C8; i += kFcThreads)
-                *reinterpret_cast<uint4*>(fout + ((long long)Ho * opitch + PX0 + i / C8) * C0 + 8 * (i % C8)) = make_uint4(0, 0, 0, 0);
+                fo[((long long)Ho * opitch + PX0 + i / C8) * C8 + (i % C8)] = make_uint4(0, 0, 0, 0);
     }
-    if (stat_part) {
-        const float2 r = block_sum2(s, ss);  // contains __syncthreads: also orders ctile / patch reuse
-        if (threadIdx.x == 0) stat_part[f * tiles + tile] = r;
-    } else {
-        __syncthreads();
+    __syncthreads();  // the tile's pooled outputs are visible to the whole block; ctile / patch may be reused
+    if (stat_part) {  // per-channel (sum, sumsq) of the tile's pooled outputs, in a fixed order
+        for (int c = threadIdx.x; c < C0; c += kFcThreads) {
+            float cs = 0.f, css = 0.f;
+            for (int py = 0; py < kFcTile; ++py)
+                for (int px = 0; px < kFcTile; ++px) {
+                    const CT o = fout[((long long)(PY0 + py) * opitch + PX0 + px) * C0 + c];
+                    float v;
+                    if constexpr (F32OUT) v = o;
+                    else v = __bfloat162float(o);
+                    cs += v;
+                    css = fmaf(v, v, css);
+                }
+            stat_part[(f * tiles + tile) * C0 + c] = make_float2(cs, css);
+        }
     }
   }
 }
 
 }  // namespace vpt
 
+// statistics partials per frame: one per (8x8 pooled tile, channel), index tile * C0 + channel
 extern "C" int vpt_firstconv_stat_parts(int32_t F, int32_t H, int32_t W, int32_t C0) {
-    if (vpt::firstconv_tc_applies(H, W)) return (H / 2 / vpt::kFtStatRows) * 2 * C0;  // per (8 pooled rows, column half, channel)
-    return (H / 16) * (W / 16);
+    (void)F;
+    return (H / 16) * (W / 16) * C0;
 }
 
+// Kernel choice of the C ABI.  This build has one first-convolution kernel, so every mode selects it.
 extern "C" int vpt_set_firstconv_mode(int32_t mode) {
-    vpt::g_fc_mode = mode;  // 1: tcgen05 kernel (firstconv_tc.cuh) where it applies; 0: always the mma.sync kernel
+    (void)mode;
     return VPT_OK;
 }
 
@@ -226,45 +258,26 @@ extern "C" int vpt_firstconv_pool(const uint8_t* img, const float* w, const floa
                                   int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream) {
     using namespace vpt;
     VPT_CHECK(img && w && bias && out && F > 0, "vpt_firstconv_pool: null argument");
-    VPT_CHECK(!out_f32 || firstconv_tc_applies(H, W), "vpt_firstconv_pool: fp32 output needs the tcgen05 kernel (W in {32,64,128}, H*W <= 16384)");
     VPT_CHECK(H % 16 == 0 && W % 16 == 0 && H >= 16 && W >= 16, "vpt_firstconv_pool: H, W must be multiples of 16 (H=%d W=%d)", H, W);
     VPT_CHECK(C0 == 64 || C0 == 128 || C0 == 192 || C0 == 256, "vpt_firstconv_pool: C0=%d not in {64,128,192,256}", C0);
-    if (firstconv_tc_applies(H, W)) {
-        VPT_CHECK(((uintptr_t)img & 15) == 0, "vpt_firstconv_pool: img must be 16-byte aligned");
-        FirstconvTcParams p;
-        memset(&p, 0, sizeof(p));
-        p.img = img; p.w = w; p.bias = bias;
-        p.out = reinterpret_cast<__nv_bfloat16*>(out);
-        p.stat_part = reinterpret_cast<float2*>(stat_part);
-        p.H = H; p.C0 = C0; p.zp = zp ? 1 : 0;
-        p.ncb = (C0 + 127) / 128;
-        p.nbands = firstconv_tc_bands(F, H, p.ncb);
-        p.band_rows = (H / 2) / p.nbands;
-        p.items = (long long)F * p.nbands * p.ncb;
-        if (out_f32) {
-            if (W == 32) return launch_firstconv_tc<32, true>(p, stream);
-            if (W == 64) return launch_firstconv_tc<64, true>(p, stream);
-            return launch_firstconv_tc<128, true>(p, stream);
-        }
-        if (W == 32) return launch_firstconv_tc<32, false>(p, stream);
-        if (W == 64) return launch_firstconv_tc<64, false>(p, stream);
-        return launch_firstconv_tc<128, false>(p, stream);
-    }
     const long long blocks = (long long)F * (H / 16) * (W / 16);
     VPT_CHECK(blocks < 2147483647LL, "vpt_firstconv_pool: too many tiles");
-    const size_t smem = kFcPatchBytes + (size_t)C0 * kFcBPitch * 2 + (size_t)kFcPos * (C0 + 8) * 2;
-    static size_t attr = 0;
-    if (smem > attr) {
-        VPT_CUDA(cudaFuncSetAttribute(firstconv_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
+    const int CB = out_f32 ? 64 : C0;
+    const size_t smem = kFcPatchBytes + (size_t)C0 * kFcBPitch * 2 + (size_t)kFcPos * (CB + 8) * (out_f32 ? 4 : 2);
+    void (*kern)(const uint8_t*, const float*, const float*, void*, float2*, int, int, int, long long, int) =
+        out_f32 ? firstconv_pool_kernel<true> : firstconv_pool_kernel<false>;
+    static size_t attr[2] = {0, 0};
+    if (smem > attr[out_f32 ? 1 : 0]) {
+        VPT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr[out_f32 ? 1 : 0] = smem;
     }
     int per_sm = (int)((227 * 1024) / (smem + 1024));
     if (per_sm > 2) per_sm = 2;
     if (per_sm < 1) per_sm = 1;
     long long grid = (long long)num_sms() * per_sm;
     if (grid > blocks) grid = blocks;
-    launch_k(firstconv_pool_kernel, dim3((unsigned)grid), dim3(kFcThreads), smem, (cudaStream_t)stream, 
-        img, w, bias, reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<float2*>(stat_part), H, W, C0, blocks, zp ? 1 : 0);
+    launch_k(kern, dim3((unsigned)grid), dim3(kFcThreads), smem, (cudaStream_t)stream,
+             img, w, bias, out, reinterpret_cast<float2*>(stat_part), H, W, C0, blocks, zp ? 1 : 0);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
 }

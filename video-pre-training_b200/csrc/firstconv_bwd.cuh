@@ -158,21 +158,7 @@ static inline int firstconv_bwd_blocks(long long F, int H, int W) {
 
 }  // namespace vpt
 
-namespace vpt {
-// tcgen05 variant (firstconv_tc_kernel<W, false, true>): the CTA count it is launched with; two partial slots (column halves) per CTA
-static inline int firstconv_bwd_tc_grid(long long F, int H) {
-    const long long fb = F * firstconv_tc_bands(F, H, 1);
-    long long g = num_sms() > 0 ? num_sms() : 148;
-    if (g > fb) g = fb;
-    return (int)g;
-}
-}  // namespace vpt
-
-extern "C" int vpt_firstconv_bwd_parts(int64_t F, int32_t H, int32_t W) {  // workspace rows: enough for either kernel
-    const int a = vpt::firstconv_bwd_blocks(F, H, W);
-    const int b = vpt::firstconv_tc_applies(H, W) ? 2 * vpt::firstconv_bwd_tc_grid(F, H) : 0;
-    return a > b ? a : b;
-}
+extern "C" int vpt_firstconv_bwd_parts(int64_t F, int32_t H, int32_t W) { return vpt::firstconv_bwd_blocks(F, H, W); }
 
 extern "C" int vpt_firstconv_bwd(const uint8_t* img, const float* w, const float* bias, const void* dy, float* dW, float* db, float* workspace, int64_t F,
                                  int32_t H, int32_t W, int32_t C0, void* stream) {
@@ -180,34 +166,6 @@ extern "C" int vpt_firstconv_bwd(const uint8_t* img, const float* w, const float
     VPT_CHECK(img && w && bias && dy && dW && db && workspace && F > 0, "vpt_firstconv_bwd: null argument");
     VPT_CHECK(H % 2 == 0 && W % (2 * kFbSeg) == 0 && C0 % 32 == 0 && C0 >= 64 && C0 <= 256,
               "vpt_firstconv_bwd: need even H, W %% 16 == 0 and C0 in {64..256} a multiple of 32 (H=%d W=%d C0=%d)", H, W, C0);
-    if (firstconv_tc_applies(H, W) && C0 <= 128) {
-        // tensor-core recompute of the conv map + in-register arg-max + patch gather (csrc/firstconv_tc.cuh, backward epilogue).
-        // Measured (2048 frames of 128x128, B200): C0 = 128: 19.2 ms vs 29.7 ms for the CUDA-core kernel below; C0 = 192 (two padded
-        // 128-channel blocks): 39.7 vs 33.0 ms -- so wider layers keep the CUDA-core kernel.  The gather (27 u8 -> fp32 conversions +
-        // 27 FMAs per pooled element and channel, ~130 instructions) is what bounds it; the tensor-core formulation dW = G^T Patch is the
-        // next step (DESIGN.md section 8).
-        VPT_CHECK(((uintptr_t)img & 15) == 0, "vpt_firstconv_bwd: img must be 16-byte aligned");
-        FirstconvTcParams p;
-        memset(&p, 0, sizeof(p));
-        p.img = img; p.w = w; p.bias = bias;
-        p.dy = reinterpret_cast<const __nv_bfloat16*>(dy);
-        p.bwd_ws = workspace;
-        p.H = H; p.C0 = C0; p.zp = 1;
-        p.ncb = (C0 + 127) / 128;
-        p.nbands = firstconv_tc_bands(F, H, 1);
-        p.band_rows = (H / 2) / p.nbands;
-        p.fb_count = (long long)F * p.nbands;
-        p.items = p.fb_count * p.ncb;
-        const int grid = firstconv_bwd_tc_grid(F, H);
-        int r;
-        if (W == 32) r = launch_firstconv_tc<32, false, true>(p, stream, grid);
-        else if (W == 64) r = launch_firstconv_tc<64, false, true>(p, stream, grid);
-        else r = launch_firstconv_tc<128, false, true>(p, stream, grid);
-        if (r) return r;
-        firstconv_bwd_finalize_kernel<<<(C0 * 28 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(workspace, dW, db, 2 * grid, C0);
-        VPT_LAUNCH_CHECK();
-        return VPT_OK;
-    }
     const int S = firstconv_bwd_blocks(F, H, W);
     if (C0 <= 192)  // <= 170 registers per thread: two blocks per SM hide each other's barrier and window fetch
         firstconv_bwd_kernel<192, 2><<<S, C0, 0, (cudaStream_t)stream>>>(img, w, bias, reinterpret_cast<const __nv_bfloat16*>(dy), workspace, (int)F, H, W, C0);

@@ -1,12 +1,13 @@
-// Persistent, warp-specialised tcgen05 GEMM / implicit-GEMM 3x3 convolution for sm_100a.
+// Persistent, warp-specialised wgmma GEMM / implicit-GEMM 3x3 convolution for sm_90a.
 //
-//   warp 0 (one lane)  : TMA producer  -- A tile (128 rows x 64 bf16, 128B-swizzled) + B tile (block_n x 64)
-//   warp 1 (one lane)  : tcgen05.mma issuer, accumulators in TMEM (2 stages x 256 columns)
-//   warps 2..9         : epilogue -- tcgen05.ld -> norm-fold / bias / ReLU / residual -> bf16|fp32 store + statistics
+//   warps 0..7 (two warpgroups): wgmma consumers -- warpgroup g owns rows 64g..64g+63 of the 128-row tile, accumulates them in
+//                                registers, stages them through shared memory and runs the epilogue on them
+//                                (norm-fold / bias / ReLU / residual -> bf16|fp32 store + statistics)
+//   warp 8 (one lane)          : TMA producer -- A tile (128 rows x 64 bf16, 128B-swizzled) + B tile (block_n x 64)
 //
 // Convolution: the K loop runs over (tap, 64-channel block); the A tile of tap (dy,dx) is ONE 4-D TMA box of the raw
 // NHWC activation tensor at pixel offset (dy,dx) -- TMA zero-fills out-of-image elements, which is exactly pad=1 --
-// landing in shared memory as 128 pixel rows of 128 B, i.e. the canonical K-major SWIZZLE_128B UMMA operand.
+// landing in shared memory as 128 pixel rows of 128 B, i.e. the canonical K-major SWIZZLE_128B wgmma operand.
 // GroupNorm/LayerNorm on the input is folded into the epilogue (see include/vpt_b200.h).
 #pragma once
 #include "common.cuh"
@@ -15,11 +16,13 @@ namespace vpt {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
+constexpr int kMaxBlockN = 128;      // wgmma accumulators of 64 x 128 per warpgroup: 64 fp32 registers per thread
 constexpr int kNumEpiWarps = 8;
-constexpr int kGemmThreads = 64 + 32 * kNumEpiWarps;
+constexpr int kGemmThreads = 32 * kNumEpiWarps + 32;
 constexpr int kMaxStages = 8;
-constexpr int kAccStageCols = 256;
 constexpr uint32_t kStageBytesA = kBlockM * kBlockK * 2;
+constexpr int kStgPitch = kMaxBlockN + 4;                       // fp32 staging row pitch (conflict-free 16-byte row reads)
+constexpr uint32_t kStgBytes = 2u * 64u * kStgPitch * 4u;        // both warpgroups' 64-row staging tiles
 
 struct GemmParams {
     int M, N, K;
@@ -65,56 +68,62 @@ __device__ __forceinline__ void advance(int& stage, uint32_t& phase, int num_sta
     }
 }
 
+// One warpgroup's share of a 128 x BN tile: 64 rows x BN columns of the stage's operands, accumulated over one k block
+// (four k16 steps) into `acc` as BN/64 fragments of 64 x 64.  A rows start at a_addr (K-major: 128-byte rows; MN-major: one
+// {64 M, 64 K} box), B likewise; MN-major boxes of B are 8192 B apart.
+template <bool kMN, int BN>
+__device__ __forceinline__ void wg_mma_kblock(float (&acc)[BN / 64][32], uint32_t a_addr, uint32_t b_addr, uint64_t a_bo, bool accumulate) {
+#pragma unroll
+    for (int k = 0; k < kBlockK / 16; ++k) {
+#pragma unroll
+        for (int j = 0; j < BN / 64; ++j) {
+            if (kMN)  // 16 K rows of 128 B per instruction
+                wgmma_n64<1, 1>(acc[j], gmma_desc_sw128(a_addr + k * 2048, 8192u, 1024u), gmma_desc_sw128(b_addr + j * 8192 + k * 2048, 8192u, 1024u),
+                                (uint32_t)(accumulate || k != 0));
+            else
+                wgmma_n64<0, 0>(acc[j], gmma_desc_sw128(a_addr + k * 32) | a_bo, gmma_desc_sw128(b_addr + j * 8192 + k * 32),
+                                (uint32_t)(accumulate || k != 0));
+        }
+    }
+}
+
 // kWgrad: both operands are MN-major -- A = [K rows][M], B = [K rows][N] row-major activations (K = pixels / tokens), staged
 // as TMA boxes of {64 columns, 64 K rows} -- the tile index additionally enumerates (K split, tap); tiles are
 // [split][m_tile][tap][n_tile] and the B operand is read `tap_shift[tap]` rows further down (TMA zero-fills what falls outside
 // the tensor, which is exactly the zero padding of a 3x3 convolution on the ZP layout).  cluster == 1 in this mode.
-template <bool kWgrad>
+template <bool kWgrad, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     pdl_sync();
     extern __shared__ uint8_t smem_raw[];
-    // carve: [A stages][B stages][barriers]; operand tiles need 1024-byte alignment for SWIZZLE_128B
+    // carve: [A stages][B stages][staging][barriers]; operand tiles need 1024-byte alignment for SWIZZLE_128B
     const uint32_t raw = smem_u32(smem_raw);
     uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    const uint32_t stage_bytes_b = (uint32_t)p.block_n * kBlockK * 2;
+    constexpr uint32_t stage_bytes_b = (uint32_t)BN * kBlockK * 2;
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + (size_t)p.num_stages * kStageBytesA;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + (size_t)p.num_stages * stage_bytes_b);
+    float* stg_all = reinterpret_cast<float*>(smem_b + (size_t)p.num_stages * stage_bytes_b);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg_all) + kStgBytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + kMaxStages;
-    uint64_t* tmem_full_bar = bars + 2 * kMaxStages;
-    uint64_t* tmem_empty_bar = bars + 2 * kMaxStages + 2;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const int CS = p.cluster;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kNumEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < p.num_stages; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], (uint32_t)p.cluster);  // one MMA commit per CTA of the cluster
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full_bar[i], 1);
-            mbar_init(&tmem_empty_bar[i], kNumEpiWarps);
+            mbar_init(&empty_bar[i], (uint32_t)(2 * CS));  // one arrival per consumer warpgroup of every CTA of the cluster
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr_smem, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     // peers must not multicast into / arrive on this CTA's barriers before they are initialised
-    if (p.cluster > 1) cluster_sync_all();
+    if (CS > 1) cluster_sync_all();
 
-    const int CS = p.cluster;
     const int cta_rank = CS > 1 ? (int)cluster_ctarank() : 0;
     const int cluster_id = blockIdx.x / CS, num_clusters = gridDim.x / CS;
     const uint16_t cmask = (uint16_t)((1u << CS) - 1u);
@@ -123,18 +132,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int num_super = tiles_mn * (kWgrad ? p.k_splits : 1);
     const int n_cols = kWgrad ? p.num_n_tiles * p.ntaps : p.num_n_tiles;  // tile columns (wgrad: [tap][n_tile])
 
-    if (warp == 0) {
+    if (warp == kNumEpiWarps) {
         if (lane == 0) {
             // ================= TMA producer =================
             int stage = 0;
             uint32_t phase = 0;
             bool ok = true;
-            const uint32_t slice_rows = (uint32_t)p.block_n / CS, slice_bytes = stage_bytes_b / CS;
+            const uint32_t slice_rows = (uint32_t)BN / CS, slice_bytes = stage_bytes_b / CS;
             for (int st = cluster_id; st < num_super && ok; st += num_clusters) {
                 const int split = kWgrad ? st / tiles_mn : 0, sm = kWgrad ? st - split * tiles_mn : st;
                 const int m_tile = (sm / n_cols) * CS + cta_rank, col = sm % n_cols;
                 const int tap = kWgrad ? col / p.num_n_tiles : 0, n_tile = kWgrad ? col - tap * p.num_n_tiles : col;
-                const int m0 = m_tile * kBlockM, n0 = n_tile * p.block_n;
+                const int m0 = m_tile * kBlockM, n0 = n_tile * BN;
                 int f0 = 0, y0 = 0;
                 if (p.conv) {
                     f0 = m0 / p.px_per_frame;
@@ -151,7 +160,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     if (kWgrad) {
                         tma_load_2d(sa, &tmA, &full_bar[stage], m0, it * kBlockK);
                         tma_load_2d(sa + 8192, &tmA, &full_bar[stage], m0 + 64, it * kBlockK);
-                        for (int bx = 0; bx < p.block_n / 64; ++bx)
+#pragma unroll
+                        for (int bx = 0; bx < BN / 64; ++bx)
                             tma_load_2d(sb + bx * 8192, &tmB, &full_bar[stage], n0 + bx * 64, it * kBlockK + bshift);
                         advance(stage, phase, p.num_stages);
                         continue;
@@ -171,68 +181,62 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ================= MMA issuer =================
-            const uint32_t idesc = kWgrad ? umma_idesc_bf16_mn(kBlockM, p.block_n) : umma_idesc_bf16(kBlockM, p.block_n);
-            const uint32_t wg_lbo = 8192u, wg_sbo = 1024u;  // next 64 M/N columns (one TMA box) / next 8 K rows
-            int stage = 0;
-            uint32_t phase = 0;
-            int local = 0;
-            bool ok = true;
-            for (int st = cluster_id; st < num_super && ok; st += num_clusters, ++local) {
-                const int as = local & 1;
-                const uint32_t aphase = (uint32_t)(local >> 1) & 1u;
-                if (!(ok = mbar_wait(&tmem_empty_bar[as], aphase ^ 1u, 0x200u))) break;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(as * kAccStageCols);
-                int n_it = p.k_iters;
-                if (kWgrad) {
-                    const int it0 = (st / tiles_mn) * p.k_iters_split;
-                    n_it = min(p.k_iters, it0 + p.k_iters_split) - it0;
-                }
-                for (int it = 0; it < n_it; ++it) {
-                    if (!(ok = mbar_wait(&full_bar[stage], phase, 0x300u))) break;
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem_a + (size_t)stage * kStageBytesA) + (uint32_t)p.dbg_shift * 128u;
-                    const uint64_t a_bo = p.dbg_bo ? ((uint64_t)((a_addr >> 7) & 7u) << 49) : 0ull;
-                    const uint32_t b_addr = smem_u32(smem_b + (size_t)stage * stage_bytes_b);
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 16; ++k) {
-                        if (kWgrad)  // 16 K rows of 128 B per instruction
-                            umma_bf16(d_tmem, umma_desc_sw128_mn(a_addr + k * 2048, wg_lbo, wg_sbo),
-                                      umma_desc_sw128_mn(b_addr + k * 2048, wg_lbo, wg_sbo), idesc, (uint32_t)((it | k) != 0));
-                        else
-                            umma_bf16(d_tmem, umma_desc_sw128(a_addr + k * 32) | a_bo, umma_desc_sw128(b_addr + k * 32), idesc,
-                                      (uint32_t)((it | k) != 0));
-                    }
-                    if (CS > 1) umma_commit_mc(&empty_bar[stage], cmask);  // the slot is refilled by every CTA of the cluster
-                    else umma_commit(&empty_bar[stage]);
-                    advance(stage, phase, p.num_stages);
-                }
-                if (ok) umma_commit(&tmem_full_bar[as]);
-            }
-        }
     } else {
-        // ================= epilogue =================
-        const int ew = warp - 2;
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-        const int chalf = ew >> 2;                    // column half
-        const int nchunks = (p.block_n + 31) >> 5;
+        // ================= wgmma + epilogue (warps 0..7) =================
+        const int wg = warp >> 2;                     // warpgroup: rows 64*wg .. 64*wg+63 of the tile
+        const int quarter = 2 * wg + (warp & 1);      // 32-row quarter this warp stores
+        const int chalf = (warp >> 1) & 1;            // column half
+        float* stg = stg_all + (size_t)wg * 64 * kStgPitch;
+        const float* my_row = stg + (size_t)((warp & 1) * 32 + lane) * kStgPitch;
+        const int nchunks = BN >> 5;
         const int c_begin = chalf == 0 ? 0 : (nchunks + 1) >> 1;
         const int c_end = chalf == 0 ? (nchunks + 1) >> 1 : nchunks;
         const int P = p.num_n_tiles * 2;
         const bool tab_vec = (p.conv == 0) || ((p.N & 3) == 0);
         const bool res_vec = ((p.ld_res & 7) == 0);
-        int local = 0;
+        int stage = 0;
+        uint32_t phase = 0;
         bool ok = true;
-        for (int st = cluster_id; st < num_super && ok; st += num_clusters, ++local) {
+        for (int st = cluster_id; st < num_super && ok; st += num_clusters) {
             const int split = kWgrad ? st / tiles_mn : 0, sm = kWgrad ? st - split * tiles_mn : st;
             const int m_tile = (sm / n_cols) * CS + cta_rank, col = sm % n_cols;
             const int tap = kWgrad ? col / p.num_n_tiles : 0, n_tile = kWgrad ? col - tap * p.num_n_tiles : col;
-            const int m0 = m_tile * kBlockM, n0 = n_tile * p.block_n;
-            const int as = local & 1;
-            const uint32_t aphase = (uint32_t)(local >> 1) & 1u;
+            const int m0 = m_tile * kBlockM, n0 = n_tile * BN;
+            // ---- main loop: this warpgroup's 64 x BN accumulators
+            float frag[BN / 64][32];
+            int n_it = p.k_iters;
+            if (kWgrad) {
+                const int it0 = split * p.k_iters_split;
+                n_it = min(p.k_iters, it0 + p.k_iters_split) - it0;
+            }
+            int prev = -1;
+            for (int it = 0; it < n_it; ++it) {
+                if (!(ok = mbar_wait(&full_bar[stage], phase, 0x300u))) break;
+                const uint32_t a_addr = kWgrad ? smem_u32(smem_a + (size_t)stage * kStageBytesA) + (uint32_t)wg * 8192u
+                                               : smem_u32(smem_a + (size_t)stage * kStageBytesA) + (uint32_t)(wg * 64 + p.dbg_shift) * 128u;
+                const uint64_t a_bo = p.dbg_bo ? ((uint64_t)((a_addr >> 7) & 7u) << 49) : 0ull;
+                const uint32_t b_addr = smem_u32(smem_b + (size_t)stage * stage_bytes_b);
+                wgmma_fence();
+                wg_mma_kblock<kWgrad, BN>(frag, a_addr, b_addr, a_bo, it != 0);
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k block's MMAs are done: its stage may be refilled
+                if (prev >= 0 && (threadIdx.x & 127) == 0)
+                    for (int r = 0; r < CS; ++r) mbar_arrive_cluster(&empty_bar[prev], (uint32_t)r);
+                prev = stage;
+                advance(stage, phase, p.num_stages);
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j) wgmma_reg_fence(frag[j]);
+            if (prev >= 0 && (threadIdx.x & 127) == 0)
+                for (int r = 0; r < CS; ++r) mbar_arrive_cluster(&empty_bar[prev], (uint32_t)r);
+            if (!ok) break;
+            // ---- accumulators -> row-major staging tile (the previous tile's epilogue has finished reading it)
+            named_bar_sync(1 + wg, 128);
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j) wgmma_frag_store(frag[j], stg, kStgPitch, j * 64);
+            named_bar_sync(1 + wg, 128);
+
             const int m = m0 + quarter * 32 + lane;
             const bool row_ok = m < p.M;
             // per-row constants
@@ -270,15 +274,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (d_remap) orow = (long long)(m / p.seg_len) * p.seg_stride + p.seg_off + (m % p.seg_len);
             float st_s = 0.f, st_ss = 0.f;
 
-            if (!(ok = mbar_wait(&tmem_full_bar[as], aphase, 0x400u))) break;
-            tc_fence_after();
             for (int c = c_begin; c < c_end; ++c) {
-                uint32_t acc[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * kAccStageCols + c * 32), acc);
-                tmem_ld_wait();
                 const int nb = n0 + c * 32;
-                const int lim = min(32, min(p.block_n - c * 32, p.N - nb));  // valid columns in this chunk
+                const int lim = min(32, min(BN - c * 32, p.N - nb));  // valid columns in this chunk
                 if (!row_ok || lim <= 0) continue;
+                uint32_t acc[32];
+                stg_ld_32(my_row + c * 32, acc);
                 float v[32];
                 const bool full = (lim == 32);
                 // ---- fold: v = ga*acc - gb*S1 + S2
@@ -393,10 +394,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     }
                 }
             }
-            // release the accumulator stage to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty_bar[as]);
             // statistics partials
             if (p.stat_part) {
                 if (p.stat_mode == 1) {
@@ -412,14 +409,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
     }
 
-    tc_fence_before();
-    __syncthreads();
     // no CTA may exit while a peer can still multicast into its shared memory or arrive on its barriers
-    if (p.cluster > 1) cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
+    if (CS > 1) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -460,11 +451,11 @@ static int make_tmap_bf16(CUtensorMap* tm, const void* base, int rank, const cuu
     return VPT_OK;
 }
 
+// N tile: 64 or 128 columns (the wgmma accumulators of a warpgroup hold 64 x block_n fp32 values)
 static inline void choose_block_n(int N, int* block_n, int* n_tiles) {
-    int nt = (N + 255) / 256;
+    int nt = (N + kMaxBlockN - 1) / kMaxBlockN;
     int bn = (N + nt - 1) / nt;
-    bn = (bn + 15) / 16 * 16;
-    if (bn < 16) bn = 16;
+    bn = bn <= 64 ? 64 : kMaxBlockN;
     *block_n = bn;
     *n_tiles = (N + bn - 1) / bn;
 }
@@ -525,10 +516,10 @@ extern "C" int vpt_gemm_bf16(const vpt_gemm_args* a, void* stream) {
     p.M = a->M; p.N = a->N; p.K = a->K;
     choose_block_n(a->N, &p.block_n, &p.num_n_tiles);
     if (a->ndst > 0) {  // segments start on N-tile boundaries: the largest tile width that divides every segment start
-        int bn = 256;
+        int bn = kMaxBlockN;
         for (int i = 1; i < a->ndst && i < 4; ++i)
-            while (bn > 16 && a->dst_n0[i] % bn != 0) bn >>= 1;
-        if (bn > (a->N + 15) / 16 * 16) bn = (a->N + 15) / 16 * 16;
+            if (a->dst_n0[i] % bn != 0) bn = 64;
+        if (a->N <= 64) bn = 64;
         p.block_n = bn;
         p.num_n_tiles = (a->N + bn - 1) / bn;
     }
@@ -582,11 +573,11 @@ extern "C" int vpt_gemm_bf16(const vpt_gemm_args* a, void* stream) {
         if (r) return r;
     }
     const uint32_t stage_bytes = kStageBytesA + (uint32_t)p.block_n * kBlockK * 2;
-    int stages = (int)(200 * 1024 / stage_bytes);
+    const size_t fixed_bytes = 1024 + kStgBytes + 2 * kMaxStages * 8;
+    int stages = (int)((227 * 1024 - fixed_bytes) / stage_bytes);
     if (stages > kMaxStages) stages = kMaxStages;
-    if (stages < 2) stages = 2;
     p.num_stages = stages;
-    const size_t smem_bytes = 1024 + (size_t)stages * stage_bytes + (2 * kMaxStages + 4) * 8 + 16;
+    const size_t smem_bytes = fixed_bytes + (size_t)stages * stage_bytes;
     p.mr = a->mr; p.rows_per_group = a->rows_per_group > 0 ? a->rows_per_group : 1;
     p.S1 = a->mr ? a->S1 : nullptr;
     p.S2 = a->S2;
@@ -607,9 +598,11 @@ extern "C" int vpt_gemm_bf16(const vpt_gemm_args* a, void* stream) {
 
     static bool attr_set = false;
     if (!attr_set) {
-        VPT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
+    void (*kern)(const CUtensorMap, const CUtensorMap, const GemmParams) = p.block_n == 64 ? gemm_tc_kernel<false, 64> : gemm_tc_kernel<false, 128>;
     const int num_super = ((p.num_m_tiles + cs - 1) / cs) * p.num_n_tiles;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -626,22 +619,23 @@ extern "C" int vpt_gemm_bf16(const vpt_gemm_args* a, void* stream) {
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     // persistent grid: as many clusters as can be co-resident (cluster size 4 strands some SMs of the uneven GPCs)
-    static int max_clusters[5] = {0, 0, 0, 0, 0};
-    if (max_clusters[cs] == 0) {
+    static int max_clusters[2][5] = {{0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
+    int& mc = max_clusters[p.block_n == 64 ? 0 : 1][cs];
+    if (mc == 0) {
         int n = 0;
         cfg.gridDim = dim3(num_sms() / cs * cs);
-        cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<false>, &cfg);
+        cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
         if (e != cudaSuccess || n <= 0) {
             (void)cudaGetLastError();
             n = num_sms() / cs;
         }
-        max_clusters[cs] = n;
+        mc = n;
     }
-    int clusters = max_clusters[cs];
+    int clusters = mc;
     if (clusters > num_super) clusters = num_super;
     cfg.gridDim = dim3(clusters * cs);
     cfg.numAttrs = g_pdl ? 2 : 1;
-    VPT_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<false>, tmA, tmB, p));
+    VPT_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p));
     return VPT_OK;
 }
 
@@ -656,17 +650,8 @@ struct WgradPlan {
 
 static WgradPlan wgrad_plan(int M, int N, int ntaps, long long R) {
     WgradPlan w;
-    // whole 64-column TMA boxes; among 256 / 192 / 128 pick the width that pads N the least (N = 384 -> 2 x 192, not 256 + 128)
-    if (N <= 256) {
-        w.block_n = (N + 63) / 64 * 64;
-    } else {
-        int best = 256, best_pad = (N + 255) / 256 * 256 - N;
-        for (int bn = 192; bn >= 128; bn -= 64) {
-            const int pad = (N + bn - 1) / bn * bn - N;
-            if (pad < best_pad) { best = bn; best_pad = pad; }
-        }
-        w.block_n = best;
-    }
+    // whole 64-column TMA boxes, at most kMaxBlockN wide
+    w.block_n = N <= 64 ? 64 : kMaxBlockN;
     w.n_tiles = (N + w.block_n - 1) / w.block_n;
     w.m_tiles = (M + kBlockM - 1) / kBlockM;
     w.k_iters = (int)((R + kBlockK - 1) / kBlockK);
@@ -695,19 +680,10 @@ __global__ void __launch_bounds__(256) sum_splits_kernel(const float4* __restric
 
 }  // namespace vpt
 
-namespace vpt {  // tap-pairing kernel (wgrad_tc.cuh)
-int wgrad_mode();
-long long wgrad_pair_max_splits(int M, int N, int ntaps, long long R);
-int launch_wgrad_pair(const void* a, int64_t lda, const void* b, int64_t ldb, int32_t M, int32_t N, int64_t R, const int32_t* shifts, int32_t ntaps,
-                      float* out, void* workspace, int64_t workspace_bytes, void* stream);
-}  // namespace vpt
-
 extern "C" int64_t vpt_wgrad_workspace_bytes(int32_t M, int32_t N, int32_t ntaps, int64_t R) {
     if (M <= 0 || N <= 0 || ntaps <= 0 || ntaps > 9 || R <= 0) return 0;
     const vpt::WgradPlan w = vpt::wgrad_plan(M, N, ntaps, R);
-    long long splits = w.splits;
-    const long long sp = vpt::wgrad_pair_max_splits(M, N, ntaps, R);  // either kernel may run (vpt_set_wgrad_mode)
-    if (sp > splits) splits = sp;
+    const long long splits = w.splits;
     return splits > 1 ? (int64_t)splits * M * N * ntaps * 4 : 0;
 }
 
@@ -720,7 +696,6 @@ extern "C" int vpt_wgrad_bf16(const void* a, int64_t lda, const void* b, int64_t
               "vpt_wgrad_bf16: M, N and the row strides must be multiples of 8 (M=%d N=%d lda=%lld ldb=%lld)", M, N, (long long)lda, (long long)ldb);
     VPT_CHECK(R < 2147483647LL - 4096, "vpt_wgrad_bf16: too many rows for 32-bit TMA coordinates");
     VPT_CHECK(((uintptr_t)a & 15) == 0 && ((uintptr_t)b & 15) == 0 && ((uintptr_t)out & 15) == 0, "vpt_wgrad_bf16: pointers must be 16-byte aligned");
-    if (wgrad_mode() == 1) return launch_wgrad_pair(a, lda, b, ldb, M, N, R, shifts, ntaps, out, workspace, workspace_bytes, stream);
     const WgradPlan w = wgrad_plan(M, N, ntaps, R);
     const long long out_elems = (long long)M * N * ntaps;
     VPT_CHECK(w.splits == 1 || (workspace && workspace_bytes >= (int64_t)w.splits * out_elems * 4),
@@ -755,14 +730,15 @@ extern "C" int vpt_wgrad_bf16(const void* a, int64_t lda, const void* b, int64_t
         if (r) return r;
     }
     const uint32_t stage_bytes = kStageBytesA + (uint32_t)p.block_n * kBlockK * 2;
-    int stages = (int)(200 * 1024 / stage_bytes);
+    const size_t fixed_bytes = 1024 + kStgBytes + 2 * kMaxStages * 8;
+    int stages = (int)((227 * 1024 - fixed_bytes) / stage_bytes);
     if (stages > kMaxStages) stages = kMaxStages;
-    if (stages < 2) stages = 2;
     p.num_stages = stages;
-    const size_t smem_bytes = 1024 + (size_t)stages * stage_bytes + (2 * kMaxStages + 4) * 8 + 16;
+    const size_t smem_bytes = fixed_bytes + (size_t)stages * stage_bytes;
     static bool attr_set = false;
     if (!attr_set) {
-        VPT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
     const int items = w.m_tiles * w.n_tiles * ntaps * w.splits;
@@ -780,7 +756,7 @@ extern "C" int vpt_wgrad_bf16(const void* a, int64_t lda, const void* b, int64_t
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    VPT_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<true>, tmA, tmB, p));
+    VPT_CUDA(cudaLaunchKernelEx(&cfg, p.block_n == 64 ? gemm_tc_kernel<true, 64> : gemm_tc_kernel<true, 128>, tmA, tmB, p));
     if (w.splits > 1) {
         const long long n4 = out_elems / 4;
         long long blocks = (n4 + 255) / 256;
@@ -789,5 +765,12 @@ extern "C" int vpt_wgrad_bf16(const void* a, int64_t lda, const void* b, int64_t
                                                                               reinterpret_cast<float4*>(out), n4, w.splits);
         VPT_LAUNCH_CHECK();
     }
+    return VPT_OK;
+}
+
+// Weight-gradient kernel choice of the C ABI.  This build has one weight-gradient kernel (the MN-major mode of gemm_tc_kernel), so
+// every mode selects it.
+extern "C" int vpt_set_wgrad_mode(int32_t mode) {
+    (void)mode;
     return VPT_OK;
 }

@@ -1,6 +1,6 @@
 // Small-M linear layer (rollout path, B*T <= 8 tokens): out = epilogue(A[M][K] . W[N][K]^T) with the same epilogue contract as
 // vpt_gemm_bf16.  With one or a few rows the tensor pipe is irrelevant -- the layer is a read of the weight matrix at HBM
-// speed (2x model: 497 MB per step) -- and a 128-row tcgen05 tile would leave all but ceil(N/256) SMs idle.  So: one warp
+// speed (2x model: 497 MB per step) -- and a 128-row tensor-core tile would leave all but ceil(N/256) SMs idle.  So: one warp
 // per output column, lanes stride over K with 16-byte loads of W (streamed, read once) and of the A rows (L1/L2 resident),
 // fp32 FMA, warp-shuffle reduction, scalar epilogue; row statistics by a one-CTA-per-row follow-up in the same [M][P] layout.
 #pragma once

@@ -1,8 +1,8 @@
 // fp32-parity precision mode (BASELINE north_star: "1e-3 rtol fp32"; the reference computes in fp32, lib/xf.py:40,55-63).
 //
-// The contraction work stays on the tcgen05 GEMM / implicit-GEMM kernel (gemm_tc.cuh): every operand is split into bf16 hi + lo
+// The contraction work stays on the wgmma GEMM / implicit-GEMM kernel (gemm_tc.cuh): every operand is split into bf16 hi + lo
 // parts and a layer is THREE accumulating launches  out = A_hi W_hi^T ; out += A_lo W_hi^T ; out = epi(out + A_hi W_lo^T)  with fp32
-// accumulators in TMEM and an fp32 running sum in HBM (the dropped lo*lo term is 2^-18 relative).  Activations are kept in fp32
+// accumulators in registers and an fp32 running sum in HBM (the dropped lo*lo term is 2^-18 relative).  Activations are kept in fp32
 // between layers; the kernels below are the fp32 glue that the bf16 path folds into its epilogues: normalise + split, statistics,
 // max-pool, residual add, and an fp32 attention.  Nothing here is performance-tuned -- this mode exists for the parity
 // configurations (BASELINE configs[0] and the IDM tolerance), the bf16 path is the product.

@@ -1,5 +1,5 @@
-// libvpt_b200.so -- single translation unit (unity build) of the sm_100a kernels behind include/vpt_b200.h.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC vpt_b200.cu -o libvpt_b200.so
+// libvpt_b200.so -- single translation unit (unity build) of the sm_90a kernels behind include/vpt_b200.h.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC vpt_b200.cu -o libvpt_b200.so
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -18,10 +18,8 @@ void set_error(const char* fmt, ...) {
 }  // namespace vpt
 
 #include "gemm_tc.cuh"
-#include "wgrad_tc.cuh"
 #include "gemv_small.cuh"
 #include "conv_zp.cuh"
-#include "conv_zp_t.cuh"
 #include "elementwise.cuh"
 #include "firstconv.cuh"
 #include "conv3d.cuh"

@@ -28,7 +28,7 @@ def _stream():
 
 def require_cuda(t):
     if not t.is_cuda:
-        raise nat.NativeError("vpt_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise nat.NativeError("vpt_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 def _cuda(*ts):
@@ -138,7 +138,7 @@ def firstconv_pool(img, w, bias, C0, zp=True, out_f32=False, want_chan=False):
     nat.check(nat.lib().vpt_firstconv_pool(_p(img), _p(w), _p(bias), _p(out), _p(part), F_, H, W, C0, z, int(out_f32), _stream()), "vpt_firstconv_pool")
     _count()
     mr = stats_finalize(part, F_, P, (H // 2) * (W // 2) * C0)
-    if want_chan:  # the tcgen05 kernel's partials are per (8 pooled rows, column half, channel)
+    if want_chan:  # the kernel's partials are per (8x8 pooled tile, channel)
         return out, mr, (part.view(F_, P // C0, C0, 2) if P % C0 == 0 and P >= C0 else None)
     return out, mr
 

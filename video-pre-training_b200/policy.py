@@ -1,5 +1,5 @@
 """Drop-in replacements for the reference's policy classes (lib/policy.py) whose forward pass runs entirely in the
-hand-written sm_100a kernels of libvpt_b200.so.
+hand-written sm_90a kernels of libvpt_b200.so.
 
     MinecraftPolicy        lib/policy.py:83-224    forward(ob, state_in, context) / initial_state / output_latent_size
     MinecraftAgentPolicy   lib/policy.py:227-339   forward / act / get_output_for_observation / get_logprob_of_action /
@@ -836,7 +836,7 @@ class MinecraftAgentPolicy(_PolicyBase):
     def make_graphed_act(self, batch_size: int, pdl: bool = False):
         """Rollout-latency path (agent.py:190-206, SURVEY f-1): returns a callable with the signature of `act` whose whole
         step (forward + heads + sampling + log-prob + KV-memory roll) is ONE captured CUDA graph replay (pdl: captured with
-        programmatic dependent launch between its kernels -- bit-identical, and measured neutral on B200: 0.953 vs 0.957 ms/step)."""
+        programmatic dependent launch between its kernels -- bit-identical)."""
         return GraphedAct(self, batch_size, pdl=pdl)
 
     @torch.no_grad()

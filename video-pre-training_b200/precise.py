@@ -1,7 +1,7 @@
 """fp32-parity precision mode of the forward path (`policy.set_precision("fp32")`; BASELINE north_star "1e-3 rtol fp32").
 
 The reference computes everything in fp32 (lib/xf.py:40 dtype assert, :55-63 fp32 logits).  The production path here multiplies bf16
-operands (1e-2 tolerance).  This mode keeps every activation in fp32 and runs each contraction on the SAME tcgen05 kernel
+operands (1e-2 tolerance).  This mode keeps every activation in fp32 and runs each contraction on the SAME wgmma kernel
 (`vpt_gemm_bf16`, linear and implicit-GEMM convolution) as three accumulating launches over bf16 hi/lo splits of both operands,
 
     out = A_hi W_hi^T ;  out += A_lo W_hi^T ;  out = epilogue(out + A_hi W_lo^T)          (fp32 accumulators, fp32 running sum)
@@ -77,7 +77,7 @@ class PreparedPrecise:
 
 
 def gemm3(xh, xl, W, M, N, K, *, conv=None, bias=None, relu=False, out_scale=1.0, ld=None):
-    """fp32 [M][ld >= N] = epilogue(x W^T) with x = xh + xl, W = Wh + Wl (bf16 parts): three tcgen05 launches (see the module docstring)."""
+    """fp32 [M][ld >= N] = epilogue(x W^T) with x = xh + xl, W = Wh + Wl (bf16 parts): three wgmma launches (see the module docstring)."""
     Wh, Wl = W
     ld = ld or N
     acc = torch.empty((M, ld), dtype=F32, device=xh.device)

@@ -9,7 +9,7 @@ What each layer type needs (u = gamma * n + beta is the normalised layer input, 
 
     NormConv / NormLinear   dz = dout * [out > 0]              ReLU (residual convs keep their branch output r for this)
                             du = dz (*) W^T                    the forward conv / GEMM kernel on flipped / transposed weights
-                            dW = dz^T (*) u                    `wgrad`: tcgen05 GEMM over the pixel / token dimension
+                            dW = dz^T (*) u                    `wgrad`: wgmma GEMM over the pixel / token dimension
                             dgamma, dbeta = sum du*n, sum du   `col_sums`
                             dx = rstd * (gamma*du - mean(gamma*du) - n * mean(gamma*du*n))      `group_sums` + `norm_bwd_apply`
     max-pool, first conv, attention, softmax heads: their own backward kernels (see include/vpt_b200.h).
@@ -80,7 +80,7 @@ class BCTrainer:
 
     def refresh_weights(self):
         """Re-layout of every kernel-side weight copy (forward folds of policy._Prepared + the heads, backward transposes of
-        `_build_weights`) after an optimizer step.  Eagerly this is ~500 small torch launches (12 ms at 3x width, profiles/bc_step_r1.md);
+        `_build_weights`) after an optimizer step.  Eagerly this is ~500 small torch launches;
         the parameters live at fixed addresses (FlatAdamDP's flat bucket), so from the second refresh on the whole re-layout is ONE captured
         CUDA graph replay writing the same kernel-layout tensors in place.  Called by `loss_and_grad`; a no-op when nothing changed."""
         pol, net = self.policy, self.policy.net
@@ -163,7 +163,7 @@ class BCTrainer:
 
     @staticmethod
     def _wgrad_linear(dz, u, weight_param=None):
-        """dW [out][in] = dz^T u (tcgen05 GEMM over the token dimension); accumulated into `weight_param.grad` when given."""
+        """dW [out][in] = dz^T u (wgmma GEMM over the token dimension); accumulated into `weight_param.grad` when given."""
         dW = ops.wgrad(dz, u)
         if weight_param is not None:
             _acc(weight_param, dW)
