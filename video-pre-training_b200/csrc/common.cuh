@@ -186,6 +186,7 @@ __device__ __forceinline__ void bulk_wait_all() {
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // multicast variant: the box lands at the same shared-memory offset (and signals the same mbarrier offset) in every
 // CTA of the cluster whose bit is set in cta_mask
@@ -246,6 +247,25 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a_desc, uint6
         : "memory");
 }
 
+// D[64 x 128] (+)= A * B^T: one instruction reads the A slab once for all 128 columns (two n64 instructions read it twice).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB)
+        : "memory");
+}
+
+// Warpgroup register budget (setmaxnreg): producer warpgroups give registers back, MMA warpgroups take them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // 128-byte-swizzled operand tile (bit layout per the PTX ISA "matrix descriptor" of wgmma: start>>4 [0,14), LBO>>4 [16,30),
 // SBO>>4 [32,46), base offset [49,52), swizzle mode [62,64) with 1 = SWIZZLE_128B).
 //   K-major: rows of 64 bf16 (128 B), 8-row groups `sbo` = 1024 B apart; LBO unused.
@@ -260,12 +280,14 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t
     return d;
 }
 
-// The 64 x 64 fragment `d` (columns col0.. of the tile) -> rows of a row-major fp32 staging tile `stg` [64][pitch] in shared memory.
-__device__ __forceinline__ void wgmma_frag_store(const float (&d)[32], float* stg, int pitch, int col0) {
+// The 64 x (NR / 2) fragment `d` (columns col0.. of the tile; NR = 32 for n64, 64 for n128) -> rows of a row-major fp32 staging tile
+// `stg` [64][pitch] in shared memory.
+template <int NR>
+__device__ __forceinline__ void wgmma_frag_store(const float (&d)[NR], float* stg, int pitch, int col0) {
     const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
     const int r0 = 16 * w + (l >> 2), c0 = col0 + 2 * (l & 3);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < NR / 4; ++i) {
         *reinterpret_cast<float2*>(stg + (size_t)r0 * pitch + c0 + 8 * i) = make_float2(d[4 * i], d[4 * i + 1]);
         *reinterpret_cast<float2*>(stg + (size_t)(r0 + 8) * pitch + c0 + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
     }

@@ -12,9 +12,17 @@
 //     the shifted rows; tools/desc_experiment.py checks this on the GEMM kernel);
 //   * weights stream through their own pipeline, one [block_n][64] tile per (channel block, tap).
 //
-//   warps 0..7: two wgmma warpgroups (64 rows each) + epilogue   warp 8: A-span TMA producer   warp 9: weight TMA producer
+//   warpgroups 0, 1 (warps 0..7): MMA + epilogue, ping-pong.  Each owns a whole 128-row x BN tile (one m64nBNk16 per 64-row
+//       half and k16 step) and they take alternate tiles of the CTA's persistent sequence.  Named barriers let one warpgroup at a
+//       time issue main-loop MMAs, so one warpgroup's epilogue runs while the other's main loop keeps the tensor pipe busy; a second
+//       pair hands the single fp32 staging tile from one epilogue to the next.  A span and weight stages are released one MMA
+//       group late, so MMAs stay in flight across channel blocks and drain only at the end of a tile.
+//   warpgroup 2: warp 8 = A-span TMA producer, warp 9 = weight TMA producer (both in tile order), registers handed to the MMA
+//       warpgroups with setmaxnreg.
 // Epilogue = GroupNorm fold (border-class tables), ReLU, residual, bf16 store in ZP layout (border rows are written as
-// zeros, which maintains the layout invariant), per-row (sum, sumsq) partials for the next layer's statistics.
+// zeros, which maintains the layout invariant), per-row (sum, sumsq) partials for the next layer's statistics.  One thread per
+// row does the arithmetic; the residual and the bf16 result pass through the warp's staging rows so that global memory sees
+// 64-byte row segments.
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.cuh"
@@ -23,8 +31,13 @@ namespace vpt {
 
 static int g_cz_dbg = 0;
 
-constexpr int kCzThreads = 32 * kNumEpiWarps + 64;  // 10 warps
+constexpr int kCzThreads = 384;  // 3 warpgroups
 constexpr int kCzMaxBStages = 8;
+constexpr int kCzProducerRegs = 24, kCzMmaRegs = 240;  // setmaxnreg budget: 128 * 24 + 256 * 240 <= 64 K registers
+
+// named barriers (0 is __syncthreads): kCzBarOrder + w = warpgroup w may issue its next main loop, kCzBarStg + w = warpgroup w may
+// write the staging tile, kCzBarWg + w = warpgroup w's own staging write -> epilogue read
+constexpr int kCzBarOrder = 1, kCzBarStg = 3, kCzBarWg = 5;
 
 struct ConvZpParams {
     long long Q;  // total rows = F * FS
@@ -46,9 +59,19 @@ struct ConvZpParams {
     const float* res_shift;
 };
 
+// One 64-row half of a tile over one k block (four k16 steps): m64nBNk16, one instruction per k16 step.
+template <int BN>
+__device__ __forceinline__ void cz_mma_k16(float (&acc)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    if constexpr (BN == 128)
+        wgmma_n128<0, 0>(acc, a_desc, b_desc, accumulate);
+    else
+        wgmma_n64<0, 0>(acc, a_desc, b_desc, accumulate);
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kCzThreads, 1)
 conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvZpParams p) {
+    static_assert(BN == 64 || BN == 128, "BN is 64 or 128");
     pdl_sync();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -56,8 +79,8 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr uint32_t b_stage_bytes = (uint32_t)BN * kBlockK * 2;
     uint8_t* smem_a = smem;                                        // 2 A-span stages
     uint8_t* smem_b = smem + 2 * (size_t)p.a_stage_bytes;          // b_stages weight tiles
-    float* stg_all = reinterpret_cast<float*>(smem_b + (size_t)p.b_stages * b_stage_bytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg_all) + kStgBytes);
+    float* stg = reinterpret_cast<float*>(smem_b + (size_t)p.b_stages * b_stage_bytes);  // one 128 x BN fp32 staging tile
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + kStgBytes);
     uint64_t* a_full = bars;
     uint64_t* a_empty = bars + 2;
     uint64_t* b_full = bars + 4;
@@ -66,53 +89,53 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == kNumEpiWarps && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < 2; ++i) {
             mbar_init(&a_full[i], 1);
-            mbar_init(&a_empty[i], 2);  // one arrival per consumer warpgroup
+            mbar_init(&a_empty[i], 1);  // one consumer warpgroup per tile
         }
         for (int i = 0; i < p.b_stages; ++i) {
             mbar_init(&b_full[i], 1);
-            mbar_init(&b_empty[i], 2);
+            mbar_init(&b_empty[i], 1);
         }
         fence_barrier_init();
     }
     __syncthreads();
 
-    const long long num_tiles = p.num_m_tiles * p.num_n_tiles;
-    const long long tile_begin = (long long)blockIdx.x;
-    const long long tile_step = (long long)gridDim.x;
+    // 32-bit tile and row indices: the host keeps Q (and so every row and tile index) below 2^31
+    const int num_tiles = (int)(p.num_m_tiles * p.num_n_tiles);
+    const int tile_begin = (int)blockIdx.x;
+    const int tile_step = (int)gridDim.x;
     const int halo = p.Wp + 1;  // rows before / after the tile that the taps reach
 
-    if (warp == kNumEpiWarps) {
-        if (lane == 0) {
-            // ================= A-span producer =================
+    if (warp >= 8) {
+        setmaxnreg_dec<kCzProducerRegs>();
+        if (warp == 8 && lane == 0) {
+            // ================= A-span producer: one span per (tile, channel block), in tile order =================
             int stage = 0;
             uint32_t phase = 0;
             bool ok = true;
-            for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
-                const long long m_tile = tile / p.num_n_tiles;
-                const long long span0 = m_tile * kBlockM - halo;
+            for (int tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
+                const int m_tile = tile / p.num_n_tiles;
+                const int span0 = m_tile * kBlockM - halo;
                 for (int cb = 0; cb < p.cin_blocks; ++cb) {
                     if (!(ok = mbar_wait(&a_empty[stage], phase ^ 1u, 0x110u))) break;
                     mbar_expect_tx(&a_full[stage], (uint32_t)p.a_stage_bytes);
                     uint8_t* sa = smem_a + (size_t)stage * p.a_stage_bytes;
                     for (int b = 0; b < p.a_boxes; ++b)
-                        tma_load_2d(sa + (size_t)b * p.a_box_rows * 128, &tmA, &a_full[stage], cb * kBlockK, (int)(span0 + (long long)b * p.a_box_rows));
+                        tma_load_2d(sa + (size_t)b * p.a_box_rows * 128, &tmA, &a_full[stage], cb * kBlockK, span0 + b * p.a_box_rows);
                     advance(stage, phase, 2);
                 }
             }
-        }
-    } else if (warp == kNumEpiWarps + 1) {
-        if (lane == 0) {
-            // ================= weight producer =================
+        } else if (warp == 9 && lane == 0) {
+            // ================= weight producer: one [BN][64] tile per (tile, channel block, tap) =================
             int stage = 0;
             uint32_t phase = 0;
             bool ok = true;
-            for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
-                const int n0 = (int)(tile % p.num_n_tiles) * BN;
+            for (int tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
+                const int n0 = (tile % p.num_n_tiles) * BN;
                 for (int cb = 0; cb < p.cin_blocks && ok; ++cb) {
                     for (int tap = 0; tap < 9; ++tap) {
                         if (!(ok = mbar_wait(&b_empty[stage], phase ^ 1u, 0x120u))) break;
@@ -123,178 +146,268 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 }
             }
         }
-    } else {
-        // ================= wgmma + epilogue (warps 0..7) =================
-        const int wg = warp >> 2;                     // warpgroup: rows 64*wg .. 64*wg+63 of the tile
-        const int quarter = 2 * wg + (warp & 1);
-        const int grp = (warp >> 1) & 1;              // column half
-        float* stg = stg_all + (size_t)wg * 64 * kStgPitch;
-        const float* my_row = stg + (size_t)((warp & 1) * 32 + lane) * kStgPitch;
-        const int nchunks = BN >> 5;
-        const int c_begin = grp == 0 ? 0 : (nchunks + 1) >> 1;
-        const int c_end = grp == 0 ? (nchunks + 1) >> 1 : nchunks;
-        const int P = p.num_n_tiles * 2;
-        const bool tab_vec = ((p.N & 3) == 0);
-        const bool leader = (threadIdx.x & 127) == 0;
-        int astage = 0, bstage = 0;
-        uint32_t aphase = 0, bphase = 0;
+        return;
+    }
+
+    // ================= MMA + epilogue: warpgroup wg owns the CTA's tiles 2i + wg of its sequence (ping-pong) =================
+    setmaxnreg_inc<kCzMmaRegs>();
+    const int wg = warp >> 2;
+    const int wwarp = warp & 3;  // this warp's 32-row quarter of the tile in the epilogue
+    float* my_row = stg + (size_t)(wwarp * 32 + lane) * kStgPitch;
+    const int nchunks = BN >> 5;
+    const int c_half = (nchunks + 1) >> 1;  // statistics partial 0 sums chunks [0, c_half), partial 1 the rest
+    const int P = p.num_n_tiles * 2;
+    // with N % 8 == 0 and 16-byte aligned bases, rows of the residual and of res_scale / res_shift are read as 16-byte vectors
+    const bool res_vec = (((uintptr_t)p.residual | (uintptr_t)p.res_scale | (uintptr_t)p.res_shift) & 15) == 0;
+    const int b_per_tile = 9 * p.cin_blocks;
+    for (int s = wg; tile_begin + s * tile_step < num_tiles; s += 2) {
+        const int tile = tile_begin + s * tile_step;
+        const bool has_next = tile + tile_step < num_tiles;  // the other warpgroup has tile s + 1
+        const int m_tile = tile / p.num_n_tiles;
+        const int n_tile = tile % p.num_n_tiles;
+        const int n0 = n_tile * BN;
+        // this tile's place in the producers' FIFOs: both warpgroups consume them in tile order
+        const long long a_it = (long long)s * p.cin_blocks, b_it = (long long)s * b_per_tile;
+        int astage = (int)(a_it & 1), bstage = (int)(b_it % p.b_stages);
+        uint32_t aphase = (uint32_t)((a_it >> 1) & 1), bphase = (uint32_t)((b_it / p.b_stages) & 1);
+
+        // ---- main loop: 128 rows x BN channels over (channel block, tap); the other warpgroup's main loop goes first
+        if (s > 0) named_bar_sync(kCzBarOrder + wg, 256);
+        float frag[2][BN / 2];
         bool ok = true;
-        for (long long tile = tile_begin; tile < num_tiles && ok; tile += tile_step) {
-            const long long m_tile = tile / p.num_n_tiles;
-            const int n_tile = (int)(tile % p.num_n_tiles);
-            const int n0 = n_tile * BN;
-            // ---- main loop: 64 rows x BN channels of this warpgroup over (channel block, tap)
-            float frag[BN / 64][32];
-            for (int cb = 0; cb < p.cin_blocks && ok; ++cb) {
-                if (!(ok = mbar_wait(&a_full[astage], aphase, 0x310u))) break;
-                const uint32_t a_base = smem_u32(smem_a + (size_t)astage * p.a_stage_bytes) + (uint32_t)wg * 64u * 128u;
-                int prev = -1;
-                for (int tap = 0; tap < 9; ++tap) {
-                    if (!(ok = mbar_wait(&b_full[bstage], bphase, 0x320u))) break;
-                    const uint32_t b_addr = smem_u32(smem_b + (size_t)bstage * b_stage_bytes);
-                    const int row_off = (tap / 3) * p.Wp + (tap % 3);  // (dy+1)*Wp + (dx+1)
-                    const uint32_t a_addr = a_base + (uint32_t)row_off * 128u;
-                    const uint64_t a_bo = p.bo ? ((uint64_t)((a_addr >> 7) & 7u) << 49) : 0ull;
-                    wgmma_fence();
-                    wg_mma_kblock<false, BN>(frag, a_addr, b_addr, a_bo, (cb | tap) != 0);
-                    wgmma_commit();
-                    wgmma_wait<1>();
-                    if (prev >= 0 && leader) mbar_arrive(&b_empty[prev]);
-                    prev = bstage;
-                    advance(bstage, bphase, p.b_stages);
+        int prev_b = -1, prev_a = -1;  // stages whose last MMA group is the one in flight: released after the next group's wait
+        for (int cb = 0; cb < p.cin_blocks && ok; ++cb) {
+            if (!(ok = mbar_wait(&a_full[astage], aphase, 0x310u))) break;
+            const uint32_t a_base = smem_u32(smem_a + (size_t)astage * p.a_stage_bytes);
+#pragma unroll 1
+            for (int tap = 0; tap < 9; ++tap) {
+                if (!(ok = mbar_wait(&b_full[bstage], bphase, 0x320u))) break;
+                const uint32_t b_addr = smem_u32(smem_b + (size_t)bstage * b_stage_bytes);
+                const int row_off = (tap / 3) * p.Wp + (tap % 3);  // (dy+1)*Wp + (dx+1)
+                const uint32_t a_addr = a_base + (uint32_t)row_off * 128u;
+                const uint64_t a_bo = p.bo ? ((uint64_t)((a_addr >> 7) & 7u) << 49) : 0ull;  // rows 64.. start 8 KB later: same phase
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBlockK / 16; ++k) {
+                    const uint32_t acc = (uint32_t)((cb | tap | k) != 0);
+                    const uint64_t bd = gmma_desc_sw128(b_addr + k * 32);
+                    cz_mma_k16<BN>(frag[0], gmma_desc_sw128(a_addr + k * 32) | a_bo, bd, acc);
+                    cz_mma_k16<BN>(frag[1], gmma_desc_sw128(a_addr + 64u * 128u + k * 32) | a_bo, bd, acc);
                 }
-                wgmma_wait<0>();
-                if (prev >= 0 && leader) mbar_arrive(&b_empty[prev]);
-                if (leader) mbar_arrive(&a_empty[astage]);
-                advance(astage, aphase, 2);
+                wgmma_commit();
+                wgmma_wait<1>();
+                if ((threadIdx.x & 127) == 0) {
+                    if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
+                    if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                }
+                prev_a = -1;
+                prev_b = bstage;
+                advance(bstage, bphase, p.b_stages);
             }
+            prev_a = astage;
+            advance(astage, aphase, 2);
+        }
+        // every MMA of this tile is issued: the other warpgroup may start its main loop while these drain
+        if (has_next) named_bar_arrive(kCzBarOrder + (wg ^ 1), 256);
+        wgmma_wait<0>();
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j) wgmma_reg_fence(frag[j]);
-            if (!ok) break;
-            named_bar_sync(1 + wg, 128);
+        for (int h = 0; h < 2; ++h) wgmma_reg_fence(frag[h]);
+        if ((threadIdx.x & 127) == 0) {
+            if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
+            if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+        }
+        if (!ok) {
+            if (has_next) named_bar_arrive(kCzBarStg + (wg ^ 1), 256);
+            break;
+        }
+
+        // ---- accumulators -> staging tile, once the other warpgroup's epilogue has finished reading it
+        if (s > 0) named_bar_sync(kCzBarStg + wg, 256);
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j) wgmma_frag_store(frag[j], stg, kStgPitch, j * 64);
-            named_bar_sync(1 + wg, 128);
+        for (int h = 0; h < 2; ++h) wgmma_frag_store(frag[h], stg + (size_t)h * 64 * kStgPitch, kStgPitch, 0);
+        named_bar_sync(kCzBarWg + wg, 128);
 
-            const long long q = m_tile * kBlockM + quarter * 32 + lane;
-            const bool row_ok = q < p.Q;
-            // decode the ZP row: frame, y, x
-            const long long f = q / p.FS;
-            const int r = (int)(q - f * p.FS);
-            const int y = r / p.Wp, x = r - y * p.Wp;
-            const bool interior = row_ok && (y < p.H) && (x < p.W);
-            float ga = 1.f, gb = 0.f;
-            if (p.mr != nullptr && interior) {
-                const float mean = __ldg(p.mr + 2 * f), rstd = __ldg(p.mr + 2 * f + 1);
-                ga = rstd;
-                gb = rstd * mean;
-            }
-            const int cy = (y == 0) ? 0 : ((y == p.H - 1) ? 2 : 1);
-            const int cx = (x == 0) ? 0 : ((x == p.W - 1) ? 2 : 1);
-            const int cls = interior ? cy * 3 + cx : 0;
-            const float* s1row = p.S1 ? p.S1 + (size_t)cls * p.N : nullptr;
-            const float* s2row = p.S2 ? p.S2 + (size_t)cls * p.N : nullptr;
-            if (p.Ef) {  // per-frame fold table: out = ga * acc + Ef[f][cls][c]
-                s1row = nullptr;
-                s2row = p.Ef + ((size_t)(interior ? f : 0) * 9 + cls) * p.N;
-            }
-            const float* rarow = (p.res_scale && interior) ? p.res_scale + (size_t)f * p.N : nullptr;
-            const float* rbrow = (p.res_scale && interior) ? p.res_shift + (size_t)f * p.N : nullptr;
-            float st_s = 0.f, st_ss = 0.f;
+        const int q = m_tile * kBlockM + wwarp * 32 + lane;
+        const bool row_ok = q < p.Q;
+        // decode the ZP row: frame, y, x
+        const int f = q / p.FS;
+        const int r = q - f * p.FS;
+        const int y = r / p.Wp, x = r - y * p.Wp;
+        const bool interior = row_ok && (y < p.H) && (x < p.W);
+        float ga = 1.f, gb = 0.f;
+        if (p.mr != nullptr && interior) {
+            const float mean = __ldg(p.mr + 2 * f), rstd = __ldg(p.mr + 2 * f + 1);
+            ga = rstd;
+            gb = rstd * mean;
+        }
+        const int cy = (y == 0) ? 0 : ((y == p.H - 1) ? 2 : 1);
+        const int cx = (x == 0) ? 0 : ((x == p.W - 1) ? 2 : 1);
+        const int cls = interior ? cy * 3 + cx : 0;
+        const float* s1row = p.S1 ? p.S1 + (size_t)cls * p.N : nullptr;
+        const float* s2row = p.S2 ? p.S2 + (size_t)cls * p.N : nullptr;
+        if (p.Ef) {  // per-frame fold table: out = ga * acc + Ef[f][cls][c]
+            s1row = nullptr;
+            s2row = p.Ef + ((size_t)(interior ? f : 0) * 9 + cls) * p.N;
+        }
+        const float* rarow = (p.res_scale && interior) ? p.res_scale + (size_t)f * p.N : nullptr;
+        const float* rbrow = (p.res_scale && interior) ? p.res_shift + (size_t)f * p.N : nullptr;
+        float st_s0 = 0.f, st_ss0 = 0.f, st_s1 = 0.f, st_ss1 = 0.f;  // statistics partials of the two column groups
 
-            for (int c = c_begin; c < (p.dbg == 2 ? c_begin : c_end); ++c) {
-                const int nb = n0 + c * 32;
-                const int lim = min(32, min(BN - c * 32, p.N - nb));
-                if (!row_ok || lim <= 0) continue;
-                uint32_t acc[32];
+        // Chunks of 32 columns.  Full chunks move their global data through the warp's own staging rows: once every lane holds its
+        // row's fp32 chunk in registers, that chunk's 128 bytes of each row are free, so the residual comes in (bytes 0..63) and the
+        // bf16 result goes out (bytes 64..127) as 64-byte row segments, four lanes per row, instead of one 16-byte piece per row and
+        // lane.  The arithmetic per element is the same on both paths.
+        const int qw = m_tile * kBlockM + wwarp * 32;  // this warp's first row
+        float* wrows = stg + (size_t)(wwarp * 32) * kStgPitch;
+        const int seg = lane & 3;  // 16-byte piece of a 64-byte row segment in the coalesced loads / stores
+#pragma unroll 1
+        for (int c = 0; c < (p.dbg == 2 ? 0 : nchunks); ++c) {
+            const int g = c < c_half ? 0 : 1;
+            const int nb = n0 + c * 32;
+            const int lim = min(32, min(BN - c * 32, p.N - nb));
+            if (lim <= 0) break;
+            const bool full = (lim == 32) && ((p.N & 7) == 0) && res_vec;  // the same for every lane
+            uint32_t acc[32];
+            float v[32];
+            uint32_t pk[16];
+            if (full) {
                 stg_ld_32(my_row + c * 32, acc);
-                __nv_bfloat16* op = p.out + (size_t)q * p.N + nb;
-                const bool full = (lim == 32) && ((p.N & 7) == 0);
-                if (!interior) {  // zero row / column of the ZP layout
-                    if (full) {
-#pragma unroll
-                        for (int qq = 0; qq < 4; ++qq) reinterpret_cast<uint4*>(op)[qq] = make_uint4(0, 0, 0, 0);
-                    } else {
-                        for (int j = 0; j < lim; ++j) op[j] = __float2bfloat16_rn(0.f);
-                    }
-                    continue;
-                }
-                float v[32];
-                if (full && tab_vec) {
-#pragma unroll
-                    for (int qq = 0; qq < 8; ++qq) {
-                        float4 a1 = s1row ? __ldg(reinterpret_cast<const float4*>(s1row + nb) + qq) : make_float4(0, 0, 0, 0);
-                        float4 a2 = s2row ? __ldg(reinterpret_cast<const float4*>(s2row + nb) + qq) : make_float4(0, 0, 0, 0);
-                        v[4 * qq + 0] = fmaf(ga, __uint_as_float(acc[4 * qq + 0]), fmaf(-gb, a1.x, a2.x));
-                        v[4 * qq + 1] = fmaf(ga, __uint_as_float(acc[4 * qq + 1]), fmaf(-gb, a1.y, a2.y));
-                        v[4 * qq + 2] = fmaf(ga, __uint_as_float(acc[4 * qq + 2]), fmaf(-gb, a1.z, a2.z));
-                        v[4 * qq + 3] = fmaf(ga, __uint_as_float(acc[4 * qq + 3]), fmaf(-gb, a1.w, a2.w));
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        float a1 = 0.f, a2 = 0.f;
-                        if (j < lim) {
-                            if (s1row) a1 = __ldg(s1row + nb + j);
-                            if (s2row) a2 = __ldg(s2row + nb + j);
-                        }
-                        v[j] = fmaf(ga, __uint_as_float(acc[j]), fmaf(-gb, a1, a2));
-                    }
-                }
-                if (p.relu == 1) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                }
+                __syncwarp();
                 if (p.residual != nullptr) {
-                    const __nv_bfloat16* rp = p.residual + (size_t)q * p.N + nb;
-                    if (rarow) {
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < lim) v[j] += fmaf(__ldg(rarow + nb + j), __bfloat162float(rp[j]), __ldg(rbrow + nb + j));
-                    } else if (full) {
+                    for (int k = 0; k < 4; ++k) {
+                        const int rr = 8 * k + (lane >> 2);
+                        if (qw + rr < p.Q)
+                            reinterpret_cast<uint4*>(wrows + (size_t)rr * kStgPitch + c * 32)[seg] =
+                                __ldg(reinterpret_cast<const uint4*>(p.residual + (size_t)(qw + rr) * p.N + nb) + seg);
+                    }
+                    __syncwarp();
+                }
+                if (row_ok) {
+                    if (!interior) {  // zero row / column of the ZP layout
 #pragma unroll
-                        for (int qq = 0; qq < 4; ++qq) {
-                            uint4 rr = __ldg(reinterpret_cast<const uint4*>(rp) + qq);
-                            v[8 * qq + 0] += bf16_lo(rr.x); v[8 * qq + 1] += bf16_hi(rr.x);
-                            v[8 * qq + 2] += bf16_lo(rr.y); v[8 * qq + 3] += bf16_hi(rr.y);
-                            v[8 * qq + 4] += bf16_lo(rr.z); v[8 * qq + 5] += bf16_hi(rr.z);
-                            v[8 * qq + 6] += bf16_lo(rr.w); v[8 * qq + 7] += bf16_hi(rr.w);
-                        }
+                        for (int j = 0; j < 16; ++j) pk[j] = 0u;
                     } else {
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < lim) v[j] += __bfloat162float(rp[j]);
+                        for (int qq = 0; qq < 8; ++qq) {  // N % 8 == 0: the fold tables' rows are float4-aligned
+                            float4 a1 = s1row ? __ldg(reinterpret_cast<const float4*>(s1row + nb) + qq) : make_float4(0, 0, 0, 0);
+                            float4 a2 = s2row ? __ldg(reinterpret_cast<const float4*>(s2row + nb) + qq) : make_float4(0, 0, 0, 0);
+                            v[4 * qq + 0] = fmaf(ga, __uint_as_float(acc[4 * qq + 0]), fmaf(-gb, a1.x, a2.x));
+                            v[4 * qq + 1] = fmaf(ga, __uint_as_float(acc[4 * qq + 1]), fmaf(-gb, a1.y, a2.y));
+                            v[4 * qq + 2] = fmaf(ga, __uint_as_float(acc[4 * qq + 2]), fmaf(-gb, a1.z, a2.z));
+                            v[4 * qq + 3] = fmaf(ga, __uint_as_float(acc[4 * qq + 3]), fmaf(-gb, a1.w, a2.w));
+                        }
+                        if (p.relu == 1) {
+#pragma unroll
+                            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+                        }
+                        if (p.residual != nullptr) {
+                            const uint4* rp = reinterpret_cast<const uint4*>(my_row + c * 32);  // this row's residual, staged above
+#pragma unroll
+                            for (int qq = 0; qq < 4; ++qq) {
+                                const uint4 rr = rp[qq];
+                                const float r8[8] = {bf16_lo(rr.x), bf16_hi(rr.x), bf16_lo(rr.y), bf16_hi(rr.y),
+                                                     bf16_lo(rr.z), bf16_hi(rr.z), bf16_lo(rr.w), bf16_hi(rr.w)};
+                                if (rarow) {
+                                    const float4* ra4 = reinterpret_cast<const float4*>(rarow + nb) + 2 * qq;
+                                    const float4* rb4 = reinterpret_cast<const float4*>(rbrow + nb) + 2 * qq;
+                                    const float4 a0 = __ldg(ra4), a1 = __ldg(ra4 + 1), b0 = __ldg(rb4), b1 = __ldg(rb4 + 1);
+                                    const float ra[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+                                    const float rb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+                                    for (int j = 0; j < 8; ++j) v[8 * qq + j] += fmaf(ra[j], r8[j], rb[j]);
+                                } else {
+#pragma unroll
+                                    for (int j = 0; j < 8; ++j) v[8 * qq + j] += r8[j];
+                                }
+                            }
+                        }
+                        if (p.relu == 2) {
+#pragma unroll
+                            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+                        }
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) pk[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
+                        if (p.stat_part) {
+                            float s_ = g ? st_s1 : st_s0, ss_ = g ? st_ss1 : st_ss0;
+#pragma unroll
+                            for (int j = 0; j < 16; ++j) {
+                                const float lo = bf16_lo(pk[j]), hi = bf16_hi(pk[j]);
+                                s_ += lo; ss_ = fmaf(lo, lo, ss_);
+                                s_ += hi; ss_ = fmaf(hi, hi, ss_);
+                            }
+                            if (g) { st_s1 = s_; st_ss1 = ss_; } else { st_s0 = s_; st_ss0 = ss_; }
+                        }
                     }
-                }
-                if (p.relu == 2) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                }
-                uint32_t pk[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) pk[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
-                if (p.stat_part) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float lo = bf16_lo(pk[j]), hi = bf16_hi(pk[j]);
-                        if (2 * j < lim) { st_s += lo; st_ss = fmaf(lo, lo, st_ss); }
-                        if (2 * j + 1 < lim) { st_s += hi; st_ss = fmaf(hi, hi, st_ss); }
-                    }
-                }
-                if (p.dbg == 1) {
-                    if (pk[0] == 0x12345678u) op[0] = __float2bfloat16_rn(0.f);  // keep the values live, store (almost) never
-                } else if (full) {
 #pragma unroll
                     for (int qq = 0; qq < 4; ++qq)
-                        reinterpret_cast<uint4*>(op)[qq] = make_uint4(pk[4 * qq], pk[4 * qq + 1], pk[4 * qq + 2], pk[4 * qq + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (j < lim) op[j] = __float2bfloat16_rn(v[j]);
+                        reinterpret_cast<uint4*>(my_row + c * 32 + 16)[qq] = make_uint4(pk[4 * qq], pk[4 * qq + 1], pk[4 * qq + 2], pk[4 * qq + 3]);
                 }
+                __syncwarp();
+                if (p.dbg != 1) {
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        const int rr = 8 * k + (lane >> 2);
+                        if (qw + rr < p.Q)
+                            reinterpret_cast<uint4*>(p.out + (size_t)(qw + rr) * p.N + nb)[seg] =
+                                reinterpret_cast<const uint4*>(wrows + (size_t)rr * kStgPitch + c * 32 + 16)[seg];
+                    }
+                }
+                continue;
             }
-            if (p.stat_part && row_ok) reinterpret_cast<float2*>(p.stat_part)[(size_t)q * P + n_tile * 2 + grp] = make_float2(st_s, st_ss);
+            // ---- partial chunk (Cout not a multiple of the tile width / of 8): element by element, straight to global memory
+            if (!row_ok) continue;
+            stg_ld_32(my_row + c * 32, acc);
+            __nv_bfloat16* op = p.out + (size_t)q * p.N + nb;
+            if (!interior) {
+                for (int j = 0; j < lim; ++j) op[j] = __float2bfloat16_rn(0.f);
+                continue;
+            }
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                float a1 = 0.f, a2 = 0.f;
+                if (j < lim) {
+                    if (s1row) a1 = __ldg(s1row + nb + j);
+                    if (s2row) a2 = __ldg(s2row + nb + j);
+                }
+                v[j] = fmaf(ga, __uint_as_float(acc[j]), fmaf(-gb, a1, a2));
+            }
+            if (p.relu == 1) {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+            }
+            if (p.residual != nullptr) {
+                const __nv_bfloat16* rp = p.residual + (size_t)q * p.N + nb;
+#pragma unroll
+                for (int j = 0; j < 32; ++j)
+                    if (j < lim) v[j] += rarow ? fmaf(__ldg(rarow + nb + j), __bfloat162float(rp[j]), __ldg(rbrow + nb + j)) : __bfloat162float(rp[j]);
+            }
+            if (p.relu == 2) {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+            }
+#pragma unroll
+            for (int j = 0; j < 16; ++j) pk[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
+            if (p.stat_part) {
+                float s_ = g ? st_s1 : st_s0, ss_ = g ? st_ss1 : st_ss0;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const float lo = bf16_lo(pk[j]), hi = bf16_hi(pk[j]);
+                    if (2 * j < lim) { s_ += lo; ss_ = fmaf(lo, lo, ss_); }
+                    if (2 * j + 1 < lim) { s_ += hi; ss_ = fmaf(hi, hi, ss_); }
+                }
+                if (g) { st_s1 = s_; st_ss1 = ss_; } else { st_s0 = s_; st_ss0 = ss_; }
+            }
+            if (p.dbg != 1) {
+#pragma unroll
+                for (int j = 0; j < 32; ++j)
+                    if (j < lim) op[j] = __float2bfloat16_rn(v[j]);
+            }
         }
+        // the staging tile is free for the other warpgroup's next tile
+        if (has_next) named_bar_arrive(kCzBarStg + (wg ^ 1), 256);
+        if (p.stat_part && row_ok)
+            reinterpret_cast<float4*>(p.stat_part)[((size_t)q * P + n_tile * 2) >> 1] = make_float4(st_s0, st_ss0, st_s1, st_ss1);
     }
 }
 
@@ -325,7 +438,7 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     memset(&p, 0, sizeof(p));
     p.H = H; p.W = W; p.Wp = W + 1; p.FS = (H + 1) * (W + 1);
     p.Q = (long long)a->F * p.FS;
-    VPT_CHECK(p.Q < 2147483647LL, "vpt_conv3x3_zp: too many rows for 32-bit TMA coordinates");
+    VPT_CHECK(p.Q <= 2147483647LL - kBlockM, "vpt_conv3x3_zp: too many rows for 32-bit row indices and TMA coordinates");
     p.N = N; p.cin = C; p.cin_blocks = C / 64;
     conv_zp_block_n(p.Q, N, &p.block_n, &p.num_n_tiles);
     p.num_m_tiles = (p.Q + kBlockM - 1) / kBlockM;
