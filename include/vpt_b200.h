@@ -383,6 +383,30 @@ int vpt_attention_bwd(const void* Q, const void* Kf, const void* Vf, const float
 int vpt_softmax_bwd(const float* logp, const int64_t* idx, float scale, void* out, int64_t ld_out, int32_t col0, int64_t rows, int32_t n,
                     void* stream);
 
+/* ----------------------------------------------------------------------------------------------------------
+ * Backward of the inverse dynamics model (IDM) step (training.py, IDMTrainer)
+ * ---------------------------------------------------------------------------------------------------------- */
+/* Weight / bias gradient of vpt_conv3d_t5.  dy bf16 ZP [B*T][H+1][W+1][C] is the gradient wrt the conv3d OUTPUT with the ReLU
+ * mask already applied (the norm backward in front zeroes it where the taped output is 0); the ZP zero row / column and the
+ * temporal taps outside [0, T) of a frame's own sequence contribute nothing.
+ *   dW fp32 [C][15] ordered (dt, c) for the /255-scaled kernel weights (reference layout: dW_ref[C][c][dt] = dW[C][dt][c] / 255)
+ *   db fp32 [C]      workspace: vpt_conv3d_t5_bwd_workspace(B*T, H, W, C) floats.  Deterministic (per-block partials, fixed-order sum).
+ *   C a multiple of 8, <= 256, C/8 dividing 256. */
+int64_t vpt_conv3d_t5_bwd_workspace(int64_t F, int32_t H, int32_t W, int32_t C);
+int vpt_conv3d_t5_bwd(const uint8_t* img, const void* dy, float* dW, float* db, float* workspace, int32_t B, int32_t T, int32_t H, int32_t W,
+                      int32_t C, void* stream);
+/* Backward of vpt_attention with causal = 0 (mask "none", maxlen = 0: every query sees the t keys of its chunk, logits q.k / D).
+ * Q, K, V, dO bf16 [B*t][h]; writes d q | d k | d v into out bf16 [B*t][ld_out] at columns 0 | h | 2h.  t <= 128, D = 128.
+ * workspace: vpt_attention_full_bwd_workspace(B, t, heads) floats.  No atomics: bit-reproducible. */
+int64_t vpt_attention_full_bwd_workspace(int32_t B, int32_t t, int32_t heads);
+int vpt_attention_full_bwd(const void* Q, const void* K, const void* V, const void* dO, void* out, int64_t ld_out, float* workspace, int32_t B,
+                           int32_t t, int32_t heads, void* stream);
+/* Factored categorical head (`groups` sub-actions of n classes each, logp fp32 [rows][ld_logp] holding the groups side by side):
+ *   out[r][col0 + g*n + j] = (exp(logp[r][g*n + j]) - [j == idx[r][g]]) * scale   (bf16)
+ *   lp[r] (+)= sum_g logp[r][g*n + idx[r][g]]     (fp32, skipped when lp is NULL)                 lib/action_head.py:176-184 */
+int vpt_softmax_nll_bwd_grouped(const float* logp, int64_t ld_logp, const int64_t* idx, int32_t groups, int32_t n, float scale, void* out,
+                                int64_t ld_out, int32_t col0, float* lp, int32_t accumulate, int64_t rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -29,6 +29,8 @@ void set_error(const char* fmt, ...) {
 #include "resize.cuh"
 #include "backward.cuh"
 #include "attention_bwd.cuh"
+#include "attention_full_bwd.cuh"
+#include "idm_bwd.cuh"
 #include "firstconv_bwd.cuh"
 #include "precise.cuh"
 #include "codec.cuh"

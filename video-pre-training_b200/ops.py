@@ -487,10 +487,30 @@ def firstconv_bwd(img, w, bias, dy, C0):
 
 def attention_bwd(Q, Kf, Vf, R, b_nd, first_u8, smask, dO, out, B, t, maxlen, heads, causal=True):
     """Backward of `attention`: d q | d k | d v | d R written side by side into out[:, 0:h | h:2h | 2h:3h | 3h:3h+10*heads]
-    (bf16, chunk rows only: the KV memory is detached state); returns d b_nd fp32 [nbasis][maxlen]."""
+    (bf16, chunk rows only: the KV memory is detached state); returns d b_nd fp32 [nbasis][maxlen].
+    causal=False (the IDM's mask "none", maxlen = 0, t <= 128): d q | d k | d v only; R, b_nd, first_u8 and smask are unused and
+    None is returned."""
     _cuda(Q, Kf, Vf, R, b_nd, dO, out)
     if not causal:
-        raise NotImplementedError("attention_bwd: only the causal policy attention is trained")
+        h = Q.shape[-1]
+        for name, x in (("Q", Q), ("K", Kf), ("V", Vf), ("dO", dO), ("out", out)):
+            if x.dtype != BF16 or x.stride(-1) != 1 or x.data_ptr() % 16:
+                raise ValueError(f"attention_bwd(causal=False): {name} must be bf16 with unit column stride and 16-byte aligned")
+        for name, x in (("Q", Q), ("K", Kf), ("V", Vf), ("dO", dO)):
+            if not x.is_contiguous():
+                raise ValueError(f"attention_bwd(causal=False): {name} must be contiguous (rows of h = heads * 128 elements)")
+        if h != heads * 128:
+            raise ValueError(f"attention_bwd(causal=False): h = {h} != heads * 128 = {heads * 128}")
+        if maxlen != 0 or tuple(Kf.shape) != (B, t, h) or Vf.shape != Kf.shape or tuple(Q.shape) != (B * t, h) or dO.shape != Q.shape:
+            raise ValueError(f"attention_bwd(causal=False): needs maxlen == 0 and Q / dO [B*t, h], K / V [B, t, h] (got maxlen={maxlen}, "
+                             f"Q {tuple(Q.shape)}, K {tuple(Kf.shape)}, dO {tuple(dO.shape)})")
+        if out.dim() != 2 or out.shape[0] != B * t or out.shape[1] < 3 * h or out.stride(0) % 8:
+            raise ValueError(f"attention_bwd(causal=False): out must be [B*t, >= 3h] with a row stride that is a multiple of 8 (got {tuple(out.shape)})")
+        ws = torch.empty((nat.lib().vpt_attention_full_bwd_workspace(B, t, heads),), dtype=F32, device=Q.device)
+        nat.check(nat.lib().vpt_attention_full_bwd(_p(Q), _p(Kf), _p(Vf), _p(dO), _p(out), out.stride(0), _p(ws), B, t, heads, _stream()),
+                  "vpt_attention_full_bwd")
+        _count(2)
+        return None
     nbasis = b_nd.shape[0]
     ws = torch.empty((2, B * heads, t, maxlen), dtype=F32, device=Q.device)  # P and dS by relative distance d
     db = torch.empty((nbasis, maxlen), dtype=F32, device=Q.device)
@@ -509,6 +529,9 @@ def softmax_bwd(logp, idx, scale, out, col0):
               "vpt_softmax_bwd")
     _count()
     return out
+
+
+from .ops_idm import conv3d_t5_bwd, softmax_nll_bwd_grouped  # noqa: E402,F401  (IDM backward ops, csrc/idm_bwd.cuh)
 
 
 # ---- on-device action codec (csrc/codec.cuh) -----------------------------------------------------------------------------

@@ -169,6 +169,8 @@ class FlatAdamDP:
     def step(self, max_grad_norm=None):
         base = self.flat_g.data_ptr()
         for p in self.params:
+            if p.numel() == 0:  # an empty parameter (the IDM's b_nd (10, 0)) has no slice to alias
+                continue
             if p.grad is None or not (base <= p.grad.data_ptr() < base + self.flat_g.numel() * 4):
                 raise RuntimeError("FlatAdamDP.step: a parameter's .grad no longer aliases the flat gradient bucket (use FlatAdamDP.zero_grad(), "
                                    "not module.zero_grad(set_to_none=True))")

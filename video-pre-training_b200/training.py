@@ -20,7 +20,7 @@ and `value_head.*` receives no gradient (None in the reference: the BC loss neve
 import torch
 
 from . import ops
-from .policy import BF16, F32, MinecraftAgentPolicy
+from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy
 
 
 def _rot(W):
@@ -54,6 +54,10 @@ class BCTrainer:
         cfg = policy.net.cfg
         if cfg.conv3d_out is not None or cfg.first_conv_norm or cfg.mask_style != "clipped_causal":
             raise NotImplementedError("BCTrainer: only the causal policy models are trained by the reference")
+        self._init_state(policy)
+
+    def _init_state(self, policy):
+        """The trainer's own state (shared with IDMTrainer, whose policy check differs)."""
         self.policy = policy
         self._wprep = None
         self._wprep_fp = None
@@ -324,9 +328,14 @@ class BCTrainer:
         self._wgrad_linear(dy, S["a"], P[f"{o}.proj_layer.weight"])
         _acc(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
         # attention: gradients wrt q | k | v | R side by side (one buffer = one dgrad GEMM + one wgrad GEMM for all four)
+        causal = cfg.mask_style == "clipped_causal"
         dqkvr = torch.zeros((N, self.kcat), dtype=BF16, device=dy.device)
-        db_nd = ops.attention_bwd(S["q"], S["full_k"], S["full_v"], S["R"], P[f"{o}.b_nd"].detach().float().contiguous(), first_u8, S["smask"],
-                                  da, dqkvr, B, t, maxlen, heads)
+        if causal:
+            db_nd = ops.attention_bwd(S["q"], S["full_k"], S["full_v"], S["R"], P[f"{o}.b_nd"].detach().float().contiguous(), first_u8, S["smask"],
+                                      da, dqkvr, B, t, maxlen, heads)
+        else:  # mask "none" (IDM): q | k | v only; R meets an empty band (b_nd is (10, 0)), so its parameters get exact zeros
+            ops.attention_bwd(S["q"], S["full_k"], S["full_v"], None, None, None, None, da, dqkvr, B, t, 0, heads, causal=False)
+            db_nd = torch.zeros_like(P[f"{o}.b_nd"], dtype=F32)
         _acc(P[f"{o}.b_nd"], db_nd)
         dxhat = self._gemm(dqkvr, W["qkvr_t"], h, residual=dy)
         dWc = self._wgrad_linear(dqkvr, S["xhat"])
@@ -334,9 +343,13 @@ class BCTrainer:
         _acc(P[f"{o}.q_layer.weight"], dWc[0:h])
         _acc(P[f"{o}.k_layer.weight"], dWc[h:2 * h])
         _acc(P[f"{o}.v_layer.weight"], dWc[2 * h:3 * h])
-        _acc(P[f"{o}.r_layer.weight"], dWc[3 * h:3 * h + nr])
         _acc(P[f"{o}.q_layer.bias"], dbc[0:h])
-        _acc(P[f"{o}.r_layer.bias"], dbc[3 * h:3 * h + nr])
+        if causal:
+            _acc(P[f"{o}.r_layer.weight"], dWc[3 * h:3 * h + nr])
+            _acc(P[f"{o}.r_layer.bias"], dbc[3 * h:3 * h + nr])
+        else:
+            _acc(P[f"{o}.r_layer.weight"], torch.zeros_like(P[f"{o}.r_layer.weight"], dtype=F32))
+            _acc(P[f"{o}.r_layer.bias"], torch.zeros_like(P[f"{o}.r_layer.bias"], dtype=F32))
         # pre_r_ln (plain norm of the block input)
         ident = lambda v: v
         g = P[f"{b}.pre_r_ln.weight"]
@@ -344,7 +357,8 @@ class BCTrainer:
                               relu_x=(l == 0))  # block 0's input is relu(img_process.linear)
 
     def _cnn_bwd(self, dout, tape, wts, P):
-        """Backward of lib/impala_cnn.py:187-195; `dout` is the gradient wrt the last stack's output (ZP)."""
+        """Backward of lib/impala_cnn.py:187-195; `dout` is the gradient wrt the last stack's output (ZP).  Returns the gradient wrt the
+        CNN input when stack 0's first conv is a normalised one (the IDM: the conv3d output, ReLU backward applied), else None."""
         cfg = self.policy.net.cfg
         pfx = "img_process.cnn"
         ident = lambda v: v
@@ -373,15 +387,166 @@ class BCTrainer:
             dy1 = self._norm_bwd(dx.view(R, C), rec["y1"].view(R, C), rec["mr1"], g.detach().float().contiguous(), (H + 1) * (W + 1), H * W * C,
                                  (g, ident), (P[f"{s}.n.bias"], ident), zp=(H, W, C)).view(rec["y1"].shape)
             self._dbg(f"{s}.pool", dy1)
-            if i == 0:
+            if i == 0 and not cfg.first_conv_norm:
                 st = self.policy.net.prepared().stacks[0]
                 dWk, db = ops.firstconv_bwd(tape["frames"], st["fc_w"], st["fc_b"], dy1, C)
                 # kernel weights are W[c0][ky][kx][c] / 255 (lib/policy.py:44 folded in)
                 _acc(P[f"{s}.firstconv.layer.weight"], (dWk / 255.0).view(C, 3, 3, 3).permute(0, 3, 1, 2))
                 _acc(P[f"{s}.firstconv.layer.bias"], db)
-            else:
-                dfull = ops.maxpool3s2_bwd(dy1, rec["full"])  # includes the ReLU in front of the pool
-                del dy1
-                dx = self._normconv_bwd(dfull, rec["x_in"], rec["mr_in"], rec["H_in"], rec["W_in"], wts["stacks"][i]["first"],
-                                        f"{s}.firstconv", P)
-                del dfull
+                return None
+            dfull = ops.maxpool3s2_bwd(dy1, rec["full"])  # includes the ReLU in front of the pool
+            del dy1
+            # (IDM stack 0: the input is the ReLU output of the conv3d pre-stage; its ReLU backward rides on this norm's apply pass)
+            dx = self._normconv_bwd(dfull, rec["x_in"], rec["mr_in"], rec["H_in"], rec["W_in"], wts["stacks"][i]["first"],
+                                    f"{s}.firstconv", P, relu_x=(i == 0))
+            del dfull
+        return dx
+
+
+class IDMTrainer(BCTrainer):
+    """Training step of the inverse dynamics model (`InverseActionPolicy`, lib/policy.py:342-467) with the same hand-written backward as
+    `BCTrainer`:  `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions)` accumulates d loss / d param into `.grad`.
+
+        loss = -(1 / (B*T)) * sum_{b,t} sum_heads sum_sub-actions log_softmax(logits / temperature)[action]
+
+    `actions` = {"buttons": int (B,T,20), "camera": int (B,T,2)}, the layout `InverseActionPolicy.predict` returns.  The backward runs
+    heads -> final_ln on relu(recurrent output) -> the unmasked transformer blocks -> img_process.linear -> dense -> ImpalaCNN ->
+    the conv3d pre-stage.  Which parameters get which gradient follows the reference's autograd: `lastlayer.*` gets None (its
+    output is discarded, lib/policy.py:390-391); `r_layer.*` gets zeros and `b_nd` an empty (10, 0) gradient (R meets an empty band).
+
+    One call holds whole sequences (the temporal conv needs the neighbouring frames) and at most `net.idm_chunk_frames` (512) frames,
+    i.e. B = 4 at T = 128: the training forward keeps the whole CNN tape of one call.  Larger batches accumulate over calls
+    (`.grad` accumulates, as with BCTrainer).  bf16 only.  `first` and the state do nothing with mask "none": the state stays
+    (None, (B,0,h), (B,0,h))."""
+
+    max_t = 128  # frames per sequence the unmasked attention backward supports
+
+    def __init__(self, policy: InverseActionPolicy):
+        if not isinstance(policy, InverseActionPolicy):
+            raise TypeError("IDMTrainer trains an InverseActionPolicy (lib/policy.py:406-467)")
+        cfg = policy.net.cfg
+        if cfg.conv3d_out is None or cfg.mask_style != "none" or cfg.maxlen != 0:
+            raise NotImplementedError("IDMTrainer: needs the IDM configuration (conv3d pre-stage, attention mask 'none', no KV memory)")
+        if cfg.timesteps is not None and cfg.timesteps > self.max_t:
+            raise NotImplementedError(f"IDMTrainer: the unmasked attention backward supports chunks of at most {self.max_t} frames")
+        self._init_state(policy)  # (BCTrainer.__init__ refuses the IDM by design)
+
+    @staticmethod
+    def optimizer_params(policy):
+        """The parameters to hand to `FlatAdamDP`, in the order that makes its bucket split like BC's: `conv3d_layer.*` first, then the
+        policy's parameters in registration order without `lastlayer.*` (no gradient, lib/policy.py:390-391).  The gradients that are
+        final when `upper_grads_ready` fires then form the bucket slice [opt.offset_of(net.img_process.cnn.dense.norm.weight), opt.n):
+        the conv3d pre-stage, whose gradient comes last, is registered after the transformer and would otherwise sit inside it."""
+        named = [(n, p) for n, p in policy.named_parameters() if not n.startswith("net.lastlayer.")]
+        return [p for n, p in named if n.startswith("net.conv3d_layer.")] + [p for n, p in named if not n.startswith("net.conv3d_layer.")]
+
+    def _build_weights(self):
+        """Backward-side layouts: every stack's first conv is normalised (rotated like the block convs), Q | K | V only, no lastlayer."""
+        pol, net = self.policy, self.policy.net
+        cfg = net.cfg
+        P = dict(net.named_parameters())
+        w = dict(stacks=[], layers=[])
+        pfx = "img_process.cnn"
+        for i in range(len(cfg.chans)):
+            s = f"{pfx}.stacks.{i}"
+            w["stacks"].append(dict(convs=[_rot(P[f"{s}.blocks.{j}.conv{k}.layer.weight"]) for j in range(2) for k in range(2)],
+                                    first=_rot(P[f"{s}.firstconv.layer.weight"])))
+        Hf, Wf = cfg.final_hw
+        C2 = cfg.chans[-1]
+
+        def perm(v):  # reference C,H,W flatten order -> ZP (h, w, c) order (as BCTrainer._build_weights)
+            v = v.reshape(*v.shape[:-1], C2, Hf, Wf).movedim(-3, -1)
+            v = torch.nn.functional.pad(v, (0, 0, 0, 1, 0, 1))
+            return v.reshape(*v.shape[:-3], -1)
+
+        w["dense_t"] = _tr(perm(P[f"{pfx}.dense.layer.weight"].detach()))
+        w["dense_g"] = perm(P[f"{pfx}.dense.norm.weight"].detach()).float().contiguous()
+        w["dense_b"] = perm(P[f"{pfx}.dense.norm.bias"].detach()).float().contiguous()
+        w["linear_t"] = _tr(P["img_process.linear.layer.weight"])
+        h = cfg.hidsize
+        self.kcat = 3 * h
+        for l in range(cfg.n_layers):
+            o = f"recurrent_layer.blocks.{l}.r.orc_block"
+            b = f"recurrent_layer.blocks.{l}"
+            cat = torch.cat([P[f"{o}.q_layer.weight"], P[f"{o}.k_layer.weight"], P[f"{o}.v_layer.weight"]], 0)
+            w["layers"].append(dict(qkvr_t=_tr(cat), proj_t=_tr(P[f"{o}.proj_layer.weight"]), mlp0_t=_tr(P[f"{b}.mlp0.layer.weight"]),
+                                    mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
+        self.ntot = sum(getattr(pol.pi_head, name).linear_layer.weight.shape[0] for name in pol.head_specs)
+        self.ld_logits = (self.ntot + 7) // 8 * 8
+        cat = torch.cat([getattr(pol.pi_head, name).linear_layer.weight for name in pol.head_specs], 0)
+        w["heads_t"] = _tr(cat, self.ld_logits)
+        return w
+
+    def loss_and_grad(self, img, first, state_in, actions, upper_grads_ready=None):
+        """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` and `conv3d_layer.*` is final
+        (the CNN backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`.  Build the optimizer from
+        `optimizer_params(policy)` so that those final gradients are one contiguous bucket slice."""
+        pol, net = self.policy, self.policy.net
+        cfg = net.cfg
+        self.refresh_weights()
+        wts = self._weights()
+        P = dict(net.named_parameters())
+        B, t = img.shape[:2]
+        N = B * t
+        h = cfg.hidsize
+        if N > net.idm_chunk_frames:
+            raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls")
+        if t > self.max_t:  # checked before the forward: nothing is accumulated into .grad by a call that cannot finish
+            raise NotImplementedError(f"IDMTrainer: at most {self.max_t} frames per sequence (got T = {t})")
+        # ---------------- forward (the inference kernels, recording what the backward needs) ----------------
+        tape = dict(stacks=[], blocks=[])
+        net._tape = tape
+        try:
+            lat_bf16, _, state_out = net._forward_impl(img, first, state_in, use_lastlayer=False)
+        finally:
+            net._tape = None
+        if self.keep_tape:
+            self.last_tape = tape
+        pd, _ = pol._heads(lat_bf16, B, t)
+        # ---------------- loss + d logits (one launch per factored head) ----------------
+        hp = pol._heads_prepared()
+        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=img.device)
+        scale = 1.0 / (pol.temperature * N)
+        logp = None
+        for name, (shape, n) in pol.head_specs.items():
+            c0, width = hp["cols"][name]
+            groups = width // n
+            idx = actions[name].reshape(N, groups).to(torch.int64)
+            logp = ops.softmax_nll_bwd_grouped(pd[name].reshape(N, groups, n), idx, scale, dlog, c0, lp=logp)
+        loss = -logp.sum() / N
+        # ---------------- heads ----------------
+        dWh = ops.wgrad(dlog, lat_bf16)[: self.ntot]
+        dbh = ops.col_sums(dlog)[1]
+        for name in pol.head_specs:
+            c0, width = hp["cols"][name]
+            lin = getattr(pol.pi_head, name).linear_layer
+            _acc(lin.weight, dWh[c0:c0 + width])
+            _acc(lin.bias, dbh[c0:c0 + width])
+        dlat = self._gemm(dlog, wts["heads_t"], h)
+        self._dbg("latent", dlat)
+        del dlog
+        # ---------------- final_ln on relu(recurrent output) (lib/policy.py:389-392; lastlayer is not on the path) ----------------
+        ident = lambda v: v
+        fg = P["final_ln.weight"]
+        last = tape["blocks"][-1]
+        dx = self._norm_bwd(dlat, last["z"], last["mr_z"], fg.detach().float().contiguous(), 1, h, (fg, ident), (P["final_ln.bias"], ident),
+                            relu_x=True)
+        # ---------------- transformer blocks, last to first ----------------
+        for l in reversed(range(cfg.n_layers)):
+            self._dbg(f"recurrent_layer.blocks.{l}" if l < cfg.n_layers - 1 else "recurrent_out", dx)
+            dx = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t, last=(l == cfg.n_layers - 1))
+        # ---------------- img_process.linear, dense ----------------
+        dz = self._normlinear_bwd(dx, tape["xd"], tape["mr_d"], wts["linear_t"], "img_process.linear", P, relu_x=True)
+        dcnn = self._dense_bwd(dz, tape, wts, P)
+        if upper_grads_ready is not None:
+            upper_grads_ready()
+        # ---------------- ImpalaCNN, last stack to first, then the conv3d pre-stage ----------------
+        dx3 = self._cnn_bwd(dcnn, tape, wts, P)
+        self._dbg("conv3d", dx3)
+        C3 = cfg.conv3d_out
+        dW3, db3 = ops.conv3d_t5_bwd(img.contiguous(), dx3, C3)
+        del dx3
+        # kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
+        _acc(P["conv3d_layer.layer.weight"], (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
+        _acc(P["conv3d_layer.layer.bias"], db3)
+        return loss, state_out
