@@ -407,6 +407,29 @@ int vpt_attention_full_bwd(const void* Q, const void* K, const void* V, const vo
 int vpt_softmax_nll_bwd_grouped(const float* logp, int64_t ld_logp, const int64_t* idx, int32_t groups, int32_t n, float scale, void* out,
                                 int64_t ld_out, int32_t col0, float* lp, int32_t accumulate, int64_t rows, void* stream);
 
+/* ----------------------------------------------------------------------------------------------------------
+ * RL fine-tuning step (training.py, RLTrainer): gradient of  L_pi + vf_coef * L_v + kl_coef * KL(pi_ref || pi)  wrt the
+ * temperature-scaled logits and the value head's raw output.  No atomics: bit-reproducible.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* Per-row PPO coefficient: ratio = exp(lp - old_lp); clipped = (A > 0 && ratio > eps_hi) || (A < 0 && ratio < eps_lo) (ties unclipped);
+ *   c[r] = clipped ? 0 : ratio * A * inv_n,   pi_loss[r] = -min(ratio * A, clamp(ratio, eps_lo, eps_hi) * A),   clipped[r] = 1 / 0  (fp32) */
+int vpt_ppo_coef(const float* lp, const float* old_lp, const float* adv, int64_t rows, float eps_lo, float eps_hi, float inv_n, float* c,
+                 float* pi_loss, float* clipped, void* stream);
+/* One categorical head: logp / logq fp32 [rows][ld] (log-softmax of the policy / the frozen reference policy; logq may be NULL),
+ *   out[r][col0 + j] = (c[r] * (exp(logp) - [j == idx[r]]) + k * (exp(logp) - exp(logq))) * inv_temp     (bf16)
+ *   kl[r] (+)= sum_j exp(logq_j) * (logq_j - logp_j)   (fp32, fixed order; 0 without logq)             lib/action_head.py:209-220 */
+int vpt_rl_head_bwd(const float* logp, int64_t ld_logp, const float* logq, int64_t ld_logq, const int64_t* idx, const float* c, float k,
+                    float inv_temp, int32_t n, void* out, int64_t ld_out, int32_t col0, float* kl, int32_t accumulate, int64_t rows, void* stream);
+/* sums float64 [2] = (sum x, sum x^2) over x fp32 [rows] (one block, fixed order) */
+int vpt_ewma_sums(const float* x, int64_t rows, double* sums, void* stream);
+/* Value head (lib/scaled_mse_head.py:37-43 in training mode): updates the EWMA normaliser in place from the batch statistics
+ * sums / count (lib/normalize_ewma.py:41-55: s = s * w + stat * one_minus_w, fp32), then with the UPDATED statistics
+ *   out[r][col] = scale * (vpred[r] - target[r])  (bf16),   sq_err[r] = (vpred[r] - target[r])^2,
+ *   target = (returns - mean) / sqrt(var),  mean = running_mean / max(deb, 1e-5),  var = max(running_mean_sq / max(deb, 1e-5) - mean^2, 1e-2) */
+int vpt_value_bwd(const float* vpred, const float* returns, const double* sums, double count, float* running_mean, float* running_mean_sq,
+                  float* debiasing_term, float w, float one_minus_w, float scale, void* out, int64_t ld_out, int32_t col, float* sq_err,
+                  int64_t rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

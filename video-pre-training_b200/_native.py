@@ -143,6 +143,11 @@ SIGNATURES = {
     "vpt_attention_full_bwd_workspace": (_L, [_I, _I, _I]),
     "vpt_attention_full_bwd": (_I, [_P, _P, _P, _P, _P, _L, _P, _I, _I, _I, _P]),
     "vpt_softmax_nll_bwd_grouped": (_I, [_P, _L, _P, _I, _I, _F, _P, _L, _I, _P, _I, _L, _P]),
+    # RL fine-tuning (training.py, RLTrainer)
+    "vpt_ppo_coef": (_I, [_P, _P, _P, _L, _F, _F, _F, _P, _P, _P, _P]),
+    "vpt_rl_head_bwd": (_I, [_P, _L, _P, _L, _P, _P, _F, _F, _I, _P, _L, _I, _P, _I, _L, _P]),
+    "vpt_ewma_sums": (_I, [_P, _L, _P, _P]),
+    "vpt_value_bwd": (_I, [_P, _P, _P, _D, _P, _P, _P, _F, _F, _F, _P, _L, _I, _P, _L, _P]),
 }
 
 _lib = None

@@ -680,7 +680,8 @@ class _PolicyBase(nn.Module):
         return self._hpprep
 
     def _heads_fp(self):
-        return tuple((p.data_ptr(), p._version) for n, p in self.named_parameters() if not n.startswith("net."))
+        """Versions of the head weights (the EWMA normaliser is not folded into any kernel-layout copy: `denormalize` keys it itself)."""
+        return tuple((p.data_ptr(), p._version) for n, p in self.named_parameters() if not n.startswith(("net.", "value_head.normalizer.")))
 
     def _build_heads_prepared(self):
         ws, bs, cols, c0 = [], [], OrderedDict(), 0

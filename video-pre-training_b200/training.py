@@ -16,8 +16,12 @@ What each layer type needs (u = gamma * n + beta is the normalised layer input, 
 
 The KV memory carried in `state_in` is detached exactly like behavioural_cloning.py:111 (`tree_map(lambda x: x.detach())`),
 and `value_head.*` receives no gradient (None in the reference: the BC loss never touches it).
+
+`RLTrainer` replaces only the loss (a clipped policy gradient, the value head's scaled MSE and a KL penalty to a frozen reference
+policy); everything below the logits gradient is the BC backward.
 """
 import torch
+import torch.distributed as dist
 
 from . import ops
 from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy
@@ -73,8 +77,13 @@ class BCTrainer:
             self.debug_grads[name] = g
 
     # -- backward-side weight layouts (re-made whenever a parameter changes, like policy._Prepared) -------------------
+    def _weights_fp(self):
+        """Versions of the parameters the kernel-layout copies are made from: all but the EWMA normaliser, which an RL step updates on
+        every call and which no copy holds (`denormalize` keys it itself)."""
+        return tuple((p.data_ptr(), p._version) for n, p in self.policy.named_parameters() if not n.startswith("value_head.normalizer."))
+
     def _weights(self):
-        fp = tuple((p.data_ptr(), p._version) for p in self.policy.parameters())
+        fp = self._weights_fp()
         if self._wprep is not None and fp == self._wprep_fp:
             return self._wprep
         with torch.no_grad():
@@ -90,7 +99,7 @@ class BCTrainer:
         pol, net = self.policy, self.policy.net
         from .policy import _Prepared, _fingerprint
         fp_net, fp_heads = _fingerprint(net), pol._heads_fp()
-        fp_all = tuple((p.data_ptr(), p._version) for p in pol.parameters())
+        fp_all = self._weights_fp()
         if net._prep is not None and net._prep_fp == fp_net and pol._hprep is not None and pol._hprep_fp == fp_heads and self._wprep is not None \
                 and self._wprep_fp == fp_all:
             return
@@ -151,10 +160,15 @@ class BCTrainer:
                                     mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
         w["last_t"] = _tr(P["lastlayer.layer.weight"])
         self.ntot = sum(getattr(pol.pi_head, name).linear_layer.weight.shape[0] for name in pol.head_specs)
-        self.ld_logits = (self.ntot + 7) // 8 * 8
-        cat = torch.cat([getattr(pol.pi_head, name).linear_layer.weight for name in pol.head_specs], 0)
-        w["heads_t"] = _tr(cat, self.ld_logits)
+        lins = self._head_layers()
+        self.ld_logits = (sum(lin.weight.shape[0] for lin in lins) + 7) // 8 * 8
+        w["heads_t"] = _tr(torch.cat([lin.weight for lin in lins], 0), self.ld_logits)
         return w
+
+    def _head_layers(self):
+        """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order."""
+        pol = self.policy
+        return [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
 
     # -- generic pieces -------------------------------------------------------------------------------------------------
     @staticmethod
@@ -219,15 +233,17 @@ class BCTrainer:
     def loss_and_grad(self, img, first, state_in, actions, upper_grads_ready=None):
         """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` is final (the ImpalaCNN
         backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`."""
+        lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
+        loss, dlog = self._bc_dlog(pd, actions, img.shape[0] * img.shape[1])
+        self._backward_from_dlog(dlog, lat_bf16, tape, img.shape[0], img.shape[1], upper_grads_ready)
+        return loss, state_out
+
+    def _taped_forward(self, img, first, state_in):
+        """The inference kernels, recording what the backward needs -> (latent bf16, pd, vpred, tape, state_out)."""
         pol, net = self.policy, self.policy.net
-        cfg = net.cfg
         self.refresh_weights()
-        wts = self._weights()
-        P = dict(net.named_parameters())
+        self._weights()
         B, t = img.shape[:2]
-        N = B * t
-        h = cfg.hidsize
-        # ---------------- forward (the inference kernels, recording what the backward needs) ----------------
         state_in = [(m, (k.detach(), v.detach())) for (m, (k, v)) in state_in]  # behavioural_cloning.py:111
         tape = dict(stacks=[], blocks=[])
         net._tape = tape
@@ -237,10 +253,14 @@ class BCTrainer:
             net._tape = None
         if self.keep_tape:
             self.last_tape = tape
-        pd, _ = pol._heads(lat_bf16, B, t)
-        # ---------------- loss + d logits ----------------
+        pd, vpred = pol._heads(lat_bf16, B, t)
+        return lat_bf16, pd, vpred, tape, state_out
+
+    def _bc_dlog(self, pd, actions, N):
+        """The BC loss -mean log p(action) over the N frames and its gradient wrt the logits, bf16 [N][ld_logits]."""
+        pol = self.policy
         hp = pol._heads_prepared()
-        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=img.device)
+        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=pol.net.final_ln.weight.device)
         scale = 1.0 / (pol.temperature * N)
         logp = None
         for name, (shape, n) in pol.head_specs.items():
@@ -251,15 +271,24 @@ class BCTrainer:
             lp = ops.gather_logprob(pd[name].reshape(N, n), idx)
             logp = lp if logp is None else logp + lp
             ops.softmax_bwd(pd[name].reshape(N, n), idx, scale, dlog, c0)
-        loss = -logp.sum() / N
+        return -logp.sum() / N, dlog
+
+    def _backward_from_dlog(self, dlog, lat_bf16, tape, B, t, upper_grads_ready):
+        """Everything below the logits: the head weights, then final_ln, lastlayer, the transformer, the dense layer and the ImpalaCNN."""
+        cfg = self.policy.net.cfg
+        wts = self._weights()
+        P = dict(self.policy.net.named_parameters())
+        h = cfg.hidsize
         # ---------------- heads ----------------
-        dWh = ops.wgrad(dlog, lat_bf16)[: self.ntot]
+        lins = self._head_layers()
+        dWh = ops.wgrad(dlog, lat_bf16)
         dbh = ops.col_sums(dlog)[1]
-        for name in pol.head_specs:
-            c0, width = hp["cols"][name]
-            lin = getattr(pol.pi_head, name).linear_layer
-            _acc(lin.weight, dWh[c0:c0 + width])
-            _acc(lin.bias, dbh[c0:c0 + width])
+        c0 = 0
+        for lin in lins:
+            m = lin.weight.shape[0]
+            _acc(lin.weight, dWh[c0:c0 + m])
+            _acc(lin.bias, dbh[c0:c0 + m])
+            c0 += m
         dlat = self._gemm(dlog, wts["heads_t"], h)
         self._dbg("latent", dlat)
         del dlog
@@ -281,7 +310,6 @@ class BCTrainer:
             upper_grads_ready()
         # ---------------- ImpalaCNN, last stack to first ----------------
         self._cnn_bwd(dcnn, tape, wts, P)
-        return loss, state_out
 
     def _dense_bwd(self, dz, tape, wts, P):
         cfg = self.policy.net.cfg
@@ -401,6 +429,89 @@ class BCTrainer:
                                     f"{s}.firstconv", P, relu_x=(i == 0))
             del dfull
         return dx
+
+
+class RLTrainer(BCTrainer):
+    """RL fine-tuning step of `MinecraftAgentPolicy`: a clipped policy-gradient (PPO) loss, the value head's loss and a KL penalty to the
+    frozen pretrained policy, with the hand-written backward of `BCTrainer`.  Over the N = B*T frames of one call:
+
+        lp      = sum over heads of log pi(a)                     (get_logprob_of_action, lib/policy.py:271-279)
+        ratio   = exp(lp - old_logprob)
+        L_pi    = -mean min(ratio * A, clamp(ratio, 1 - clip, 1 + clip) * A)
+        L_v     = mean (vpred - normalizer(returns))^2            (ScaledMSEHead.loss in training mode, lib/scaled_mse_head.py:37-43:
+                                                                   the EWMA normaliser is updated with this batch first)
+        L_kl    = mean KL(pi_ref || pi)                           (get_kl_of_action_dists(pd_ref, pd), lib/policy.py:281-285)
+        loss    = L_pi + vf_coef * L_v + kl_coef * L_kl
+
+    `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions, old_logprob, advantages, returns, pd_ref, vf_coef=..,
+    kl_coef=..)` accumulates d loss / d param into `.grad` (the value head included) and updates the normaliser once in place; under
+    `torch.distributed` its batch statistics are all-reduced first, so every rank holds the normaliser of the global batch.
+    `old_logprob`, `advantages` and `returns` are fp32 (B, T), `returns` in the denormalised space; `pd_ref` is what the frozen
+    reference policy's forward returns for the same frames (None only with kl_coef == 0).  `trainer.stats` holds 0-d device tensors
+    pi_loss, vf_loss, kl_ref and clipfrac of the last call.  Hand every parameter with `requires_grad` to the optimizer (the three
+    normaliser tensors have none)."""
+
+    ewma_beta = 0.99999  # NormalizeEwma's default (lib/normalize_ewma.py:9; per_element_update=False, norm over (B, T))
+
+    def __init__(self, policy: MinecraftAgentPolicy):
+        super().__init__(policy)
+        self.stats = None
+
+    def _head_layers(self):
+        """The value head's output is one more column of the logits gradient (after the action heads), so that the dgrad GEMM, `wgrad`
+        and `col_sums` of the heads give d latent, dW_v and db_v as well."""
+        return super()._head_layers() + [self.policy.value_head.linear]
+
+    def loss_and_grad(self, img, first, state_in, actions, old_logprob, advantages, returns, pd_ref=None, *, vf_coef, kl_coef, clip=0.2,
+                      upper_grads_ready=None):
+        """`upper_grads_ready` as in `BCTrainer.loss_and_grad`."""
+        pol = self.policy
+        B, t = img.shape[:2]
+        N = B * t
+        for name, x in (("old_logprob", old_logprob), ("advantages", advantages), ("returns", returns)):
+            if x.dtype != F32 or tuple(x.shape) != (B, t) or x.device != img.device:
+                raise ValueError(f"RLTrainer: {name} must be fp32 {(B, t)} on {img.device} (got {x.dtype} {tuple(x.shape)} on {x.device})")
+        if pd_ref is None and kl_coef != 0:
+            raise ValueError("RLTrainer: kl_coef != 0 needs pd_ref, the frozen reference policy's action distributions")
+        if pd_ref is not None:
+            for name, (shape, n) in pol.head_specs.items():
+                if pd_ref[name].dtype != F32 or pd_ref[name].numel() != N * n:
+                    raise ValueError(f"RLTrainer: pd_ref[{name!r}] must be fp32 with {N} x {n} log-probs (got {tuple(pd_ref[name].shape)})")
+        # check every head before the forward: nothing is accumulated into .grad by a call that cannot finish
+        if any(getattr(pol.pi_head, name).linear_layer.weight.shape[0] != n for name, (shape, n) in pol.head_specs.items()):
+            raise NotImplementedError("RLTrainer: heads with several sub-actions are not trained by the reference")
+        lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, first, state_in)
+        loss, dlog = self._rl_dlog(pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N)
+        self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
+        return loss, state_out
+
+    def _rl_dlog(self, pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N):
+        pol = self.policy
+        hp = pol._heads_prepared()
+        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=vpred.device)
+        idx, logp = {}, None
+        for name, (shape, n) in pol.head_specs.items():
+            idx[name] = actions[name].reshape(N).to(torch.int64).contiguous()
+            lp = ops.gather_logprob(pd[name].reshape(N, n), idx[name])
+            logp = lp if logp is None else logp + lp
+        c, pi_loss, clipped = ops.ppo_coef(logp, old_logprob.reshape(N).contiguous(), advantages.reshape(N).contiguous(), clip)
+        kl = None
+        for name, (shape, n) in pol.head_specs.items():
+            q = None if pd_ref is None else pd_ref[name].reshape(N, n)
+            kl = ops.rl_head_bwd(pd[name].reshape(N, n), idx[name], c, q, kl_coef / N, 1.0 / pol.temperature, dlog, hp["cols"][name][0], kl)
+        # value head: the normaliser sees the global batch (one 2-element all-reduce under data parallelism), then the scaled MSE
+        ret = returns.reshape(N).contiguous()
+        sums = ops.ewma_sums(ret)
+        count = N
+        if dist.is_available() and dist.is_initialized():
+            dist.all_reduce(sums)
+            count = N * dist.get_world_size()
+        nz = pol.value_head.normalizer
+        sq = ops.value_bwd(vpred.reshape(N), ret, sums, count, nz.running_mean, nz.running_mean_sq, nz.debiasing_term, self.ewma_beta,
+                           2.0 * vf_coef / N, dlog, self.ntot)
+        self.stats = dict(pi_loss=pi_loss.mean(), vf_loss=sq.mean(), kl_ref=kl.mean(), clipfrac=clipped.mean())
+        loss = self.stats["pi_loss"] + vf_coef * self.stats["vf_loss"] + kl_coef * self.stats["kl_ref"]
+        return loss, dlog
 
 
 class IDMTrainer(BCTrainer):
