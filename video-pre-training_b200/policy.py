@@ -266,6 +266,22 @@ def _fold_linear(W, gamma=None, beta=None, bias=None):
     return Wb, S1, (S2.float().contiguous() if S2 is not None else None)
 
 
+def _dense_to_zp(v, cfg: NetConfig):
+    """The `dense` layer's input dimension (last axis of `v`): the reference flatten order c*H*W + h*W + w (lib/impala_cnn.py:192-193)
+    -> our ZP layout [Hf+1][Wf+1][C2], i.e. (h, w, c) order with zero columns where the layout holds its zero row / column."""
+    Hf, Wf = cfg.final_hw
+    v = v.reshape(*v.shape[:-1], cfg.chans[-1], Hf, Wf).movedim(-3, -1)  # (..., Hf, Wf, C2)
+    v = torch.nn.functional.pad(v, (0, 0, 0, 1, 0, 1))                     # (..., Hf+1, Wf+1, C2)
+    return v.reshape(*v.shape[:-3], -1)
+
+
+def _dense_from_zp(v, cfg: NetConfig):
+    """Inverse of `_dense_to_zp`: ZP (h, w, c) order -> the reference C,H,W flatten order, dropping the pad row / column."""
+    Hf, Wf = cfg.final_hw
+    v = v.reshape(*v.shape[:-1], Hf + 1, Wf + 1, cfg.chans[-1])[..., :Hf, :Wf, :]
+    return v.movedim(-1, -3).reshape(*v.shape[:-3], -1)
+
+
 class _Prepared:
     """Device-side, kernel-layout copy of the parameters of one MinecraftPolicy (+ optional heads)."""
 
@@ -295,14 +311,7 @@ class _Prepared:
                     q = f"{s}.blocks.{j}.conv{k}"
                     st["convs"].append(_fold_conv(g(f"{q}.layer.weight"), g(f"{q}.norm.weight"), g(f"{q}.norm.bias")))
             self.stacks.append(st)
-        C2 = cfg.chans[-1]
-        Hf, Wf = cfg.final_hw
-        # dense: reference flatten order is c*H*W + h*W + w (lib/impala_cnn.py:192-193); ours is the ZP layout
-        # [Hf+1][Wf+1][C2] -> permute to (h, w, c) and insert zero columns where the layout holds its zero row / column
-        def perm(v):
-            v = v.reshape(*v.shape[:-1], C2, Hf, Wf).movedim(-3, -1)          # (..., Hf, Wf, C2)
-            v = torch.nn.functional.pad(v, (0, 0, 0, 1, 0, 1))                # (..., Hf+1, Wf+1, C2)
-            return v.reshape(*v.shape[:-3], -1)
+        perm = lambda v: _dense_to_zp(v, cfg)
         self.dense = _fold_linear(perm(g(f"{p}.dense.layer.weight")), perm(g(f"{p}.dense.norm.weight")), perm(g(f"{p}.dense.norm.bias")))
         self.linear = _fold_linear(g("img_process.linear.layer.weight"), g("img_process.linear.norm.weight"), g("img_process.linear.norm.bias"))
         self.layers = []

@@ -1,9 +1,17 @@
-"""Behavioural-cloning step of `MinecraftAgentPolicy` (behavioural_cloning.py:101-123): forward with a tape, the
-negative log-likelihood loss of the demonstrated actions, and a hand-written backward through the same CUDA ops the forward
-uses -- no autograd graph.  Gradients land in `param.grad` (fp32, reference parameter layout), so `parallel.FlatAdamDP`
-(one NCCL all-reduce over the flat gradient bucket + one fused Adam launch) finishes the step.
+"""Training steps of `MinecraftAgentPolicy` (behavioural cloning, RL fine-tuning) and `InverseActionPolicy`: forward with a tape, the
+loss, and a hand-written backward through the same CUDA ops the forward uses -- no autograd graph.  Gradients land in `param.grad`
+(fp32, reference parameter layout), so `parallel.FlatAdamDP` (one NCCL all-reduce over the flat gradient bucket + one fused Adam
+launch) finishes the step.
 
-    loss = -(1 / (B*T)) * sum_{b,t} sum_heads log_softmax(logits_head / temperature)[action]      (lib/action_head.py:176-184)
+The three trainers share one path and differ only in the loss:
+
+    _taped_forward        the inference kernels, recording what the backward needs
+    loss                  the loss and d loss / d logits, bf16 [N][ld_logits] with one column block per `_head_layers()` entry
+                            BCTrainer   -mean log p(demonstrated action)                        (behavioural_cloning.py:101-123)
+                            RLTrainer   clipped policy gradient + value-head MSE + KL penalty    (the value head is one more column)
+                            IDMTrainer  -mean sum over sub-actions log p(action)                  (factored heads)
+    _backward_from_dlog   the head weights, final_ln [-> lastlayer], the transformer, img_process.linear, dense and the ImpalaCNN;
+                          the IDM then adds its conv3d pre-stage
 
 What each layer type needs (u = gamma * n + beta is the normalised layer input, n = (x - mean) * rstd):
 
@@ -15,16 +23,13 @@ What each layer type needs (u = gamma * n + beta is the normalised layer input, 
     max-pool, first conv, attention, softmax heads: their own backward kernels (see include/vpt_b200.h).
 
 The KV memory carried in `state_in` is detached exactly like behavioural_cloning.py:111 (`tree_map(lambda x: x.detach())`),
-and `value_head.*` receives no gradient (None in the reference: the BC loss never touches it).
-
-`RLTrainer` replaces only the loss (a clipped policy gradient, the value head's scaled MSE and a KL penalty to a frozen reference
-policy); everything below the logits gradient is the BC backward.
+and `value_head.*` receives no gradient from the BC loss (None in the reference: the BC loss never touches it).
 """
 import torch
 import torch.distributed as dist
 
 from . import ops
-from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy
+from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy, _dense_from_zp, _dense_to_zp
 
 
 def _rot(W):
@@ -49,32 +54,32 @@ def _acc(p, g):
         p.grad.add_(g)
 
 
-class BCTrainer:
-    """`loss, state_out = trainer.loss_and_grad(img, first, state_in, actions)` accumulates d loss / d param into `.grad`."""
+class _Trainer:
+    """The machinery the trainers share: backward-side weight layouts and their re-layout after an optimizer step, the taped forward
+    and the backward from d logits.  A subclass checks its policy before calling `_Trainer.__init__` and supplies the loss."""
 
-    def __init__(self, policy: MinecraftAgentPolicy):
-        if not isinstance(policy, MinecraftAgentPolicy):
-            raise TypeError("BCTrainer trains a MinecraftAgentPolicy (behavioural_cloning.py:54-62)")
-        cfg = policy.net.cfg
-        if cfg.conv3d_out is not None or cfg.first_conv_norm or cfg.mask_style != "clipped_causal":
-            raise NotImplementedError("BCTrainer: only the causal policy models are trained by the reference")
-        self._init_state(policy)
+    use_lastlayer = True  # the model's forward runs `lastlayer` between the transformer and final_ln
 
-    def _init_state(self, policy):
-        """The trainer's own state (shared with IDMTrainer, whose policy check differs)."""
+    def __init__(self, policy):
         self.policy = policy
         self._wprep = None
         self._wprep_fp = None
-        self.debug_grads = None  # set to a dict to capture d loss / d activation under the forward's tap names (tests)
         self.keep_tape = False   # tests: keep the last forward's tape in `self.last_tape` (tests/forced_replica.py)
         self.last_tape = None
         self.graph_relayout = True  # re-layout of the kernel-side weights after an optimizer step as one CUDA graph replay
         self._rl_graph = None
         self._rl_seen = 0
+        cfg = policy.net.cfg
+        h = cfg.hidsize
+        # columns of the attention's input gradient: q | k | v, and R (10 basis rows per head) with the clipped_causal mask, padded to 8
+        self.kcat = (3 * h + 10 * cfg.heads + 7) // 8 * 8 if cfg.mask_style == "clipped_causal" else 3 * h
+        self.ntot = sum(getattr(policy.pi_head, name).linear_layer.weight.shape[0] for name in policy.head_specs)  # action logits
+        self.ld_logits = (sum(lin.weight.shape[0] for lin in self._head_layers()) + 7) // 8 * 8  # columns of the logits gradient
 
-    def _dbg(self, name, g):
-        if self.debug_grads is not None:
-            self.debug_grads[name] = g
+    def _head_layers(self):
+        """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order."""
+        pol = self.policy
+        return [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
 
     # -- backward-side weight layouts (re-made whenever a parameter changes, like policy._Prepared) -------------------
     def _weights_fp(self):
@@ -126,7 +131,8 @@ class BCTrainer:
         self._wprep, self._wprep_fp = wprep, fp_all
 
     def _build_weights(self):
-        pol, net = self.policy, self.policy.net
+        """The dgrad weights of every layer the backward runs through (builds weights only: it also runs inside the graph capture)."""
+        net = self.policy.net
         cfg = net.cfg
         P = dict(net.named_parameters())
         w = dict(stacks=[], layers=[])
@@ -134,41 +140,25 @@ class BCTrainer:
         for i in range(len(cfg.chans)):
             s = f"{pfx}.stacks.{i}"
             st = dict(convs=[_rot(P[f"{s}.blocks.{j}.conv{k}.layer.weight"]) for j in range(2) for k in range(2)])
-            if i > 0:
+            if i > 0 or cfg.first_conv_norm:  # (stack 0's plain first conv has its own backward kernel, ops.firstconv_bwd)
                 st["first"] = _rot(P[f"{s}.firstconv.layer.weight"])
             w["stacks"].append(st)
-        Hf, Wf = cfg.final_hw
-        C2 = cfg.chans[-1]
-
-        def perm(v):  # reference C,H,W flatten order -> ZP (h, w, c) order with zero columns at the pad row / column
-            v = v.reshape(*v.shape[:-1], C2, Hf, Wf).movedim(-3, -1)
-            v = torch.nn.functional.pad(v, (0, 0, 0, 1, 0, 1))
-            return v.reshape(*v.shape[:-3], -1)
-
-        w["dense_t"] = _tr(perm(P[f"{pfx}.dense.layer.weight"].detach()))
-        w["dense_g"] = perm(P[f"{pfx}.dense.norm.weight"].detach()).float().contiguous()
-        w["dense_b"] = perm(P[f"{pfx}.dense.norm.bias"].detach()).float().contiguous()
+        perm = lambda v: _dense_to_zp(v.detach(), cfg)
+        w["dense_t"] = _tr(perm(P[f"{pfx}.dense.layer.weight"]))
+        w["dense_g"] = perm(P[f"{pfx}.dense.norm.weight"]).float().contiguous()
+        w["dense_b"] = perm(P[f"{pfx}.dense.norm.bias"]).float().contiguous()
         w["linear_t"] = _tr(P["img_process.linear.layer.weight"])
-        h, heads = cfg.hidsize, cfg.heads
-        nr = 10 * heads
-        self.kcat = (3 * h + nr + 7) // 8 * 8
+        qkvr = ("q", "k", "v", "r") if cfg.mask_style == "clipped_causal" else ("q", "k", "v")  # R only where the mask has a band
         for l in range(cfg.n_layers):
             o = f"recurrent_layer.blocks.{l}.r.orc_block"
             b = f"recurrent_layer.blocks.{l}"
-            cat = torch.cat([P[f"{o}.q_layer.weight"], P[f"{o}.k_layer.weight"], P[f"{o}.v_layer.weight"], P[f"{o}.r_layer.weight"]], 0)
+            cat = torch.cat([P[f"{o}.{c}_layer.weight"] for c in qkvr], 0)
             w["layers"].append(dict(qkvr_t=_tr(cat, self.kcat), proj_t=_tr(P[f"{o}.proj_layer.weight"]), mlp0_t=_tr(P[f"{b}.mlp0.layer.weight"]),
                                     mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
-        w["last_t"] = _tr(P["lastlayer.layer.weight"])
-        self.ntot = sum(getattr(pol.pi_head, name).linear_layer.weight.shape[0] for name in pol.head_specs)
-        lins = self._head_layers()
-        self.ld_logits = (sum(lin.weight.shape[0] for lin in lins) + 7) // 8 * 8
-        w["heads_t"] = _tr(torch.cat([lin.weight for lin in lins], 0), self.ld_logits)
+        if self.use_lastlayer:
+            w["last_t"] = _tr(P["lastlayer.layer.weight"])
+        w["heads_t"] = _tr(torch.cat([lin.weight for lin in self._head_layers()], 0), self.ld_logits)
         return w
-
-    def _head_layers(self):
-        """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order."""
-        pol = self.policy
-        return [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
 
     # -- generic pieces -------------------------------------------------------------------------------------------------
     @staticmethod
@@ -188,17 +178,17 @@ class BCTrainer:
         return dW
 
     @staticmethod
-    def _norm_bwd(du, x, mr, gamma, rows_per_group, count, g_param, b_param, zp=None, add=None, relu_x=False):
-        """Backward of n = (x - mean) * rstd, u = gamma * n + beta given du: accumulates dgamma / dbeta, returns dx (+ add).
+    def _norm_bwd(du, x, mr, gamma, rows_per_group, count, g_param, b_param, grad_map=None, zp=None, add=None, relu_x=False):
+        """Backward of n = (x - mean) * rstd, u = gamma * n + beta given du: accumulates dgamma / dbeta into `g_param` / `b_param`
+        (through `grad_map` when the kernel-side gamma has another layout), returns dx (+ add).
         relu_x: x is the output of a ReLU whose backward is applied to the result in the same pass."""
         if rows_per_group > 1:  # GroupNorm frames: column sums and group sums share one pass over (du, x)
             cs, ms = ops.norm_sums(du, x, mr, gamma, rows_per_group, count)
         else:
             cs = ops.col_sums(du, x, mr, rows_per_group)
             ms = ops.group_sums(du, x, mr, gamma, rows_per_group, count)
-        if g_param is not None:
-            _acc(g_param[0], g_param[1](cs[0]))
-            _acc(b_param[0], b_param[1](cs[1]))
+        _acc(g_param, cs[0] if grad_map is None else grad_map(cs[0]))
+        _acc(b_param, cs[1] if grad_map is None else grad_map(cs[1]))
         return ops.norm_bwd_apply(du, x, mr, gamma, ms, rows_per_group, zp=zp, add=add, relu_x=relu_x)
 
     def _normconv_bwd(self, dz, x, mr, H, W, W_rot, names, P, add=None, relu_x=False):
@@ -214,8 +204,7 @@ class BCTrainer:
         dWk = ops.wgrad(dz.view(R, Cout), u.view(R, Cin), shifts)  # [Cout][tap][Cin]
         del u
         _acc(P[names + ".layer.weight"], dWk.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
-        ident = lambda v: v
-        return self._norm_bwd(du.view(R, Cin), x.view(R, Cin), mr, g32, (H + 1) * (W + 1), H * W * Cin, (gam, ident), (bet, ident),
+        return self._norm_bwd(du.view(R, Cin), x.view(R, Cin), mr, g32, (H + 1) * (W + 1), H * W * Cin, gam, bet,
                               zp=(H, W, Cin), add=None if add is None else add.view(R, Cin), relu_x=relu_x).view(x.shape)
 
     def _normlinear_bwd(self, dz, x, mr, Wt, names, P, add=None, relu_x=False):
@@ -226,18 +215,9 @@ class BCTrainer:
         u, _, _ = ops.affine_norm(x, mr, g32, b32, rows_per_group=1)
         self._wgrad_linear(dz, u, P[names + ".layer.weight"])
         del u
-        ident = lambda v: v
-        return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], (gam, ident), (bet, ident), add=add, relu_x=relu_x)
+        return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], gam, bet, add=add, relu_x=relu_x)
 
     # -- the step ---------------------------------------------------------------------------------------------------------
-    def loss_and_grad(self, img, first, state_in, actions, upper_grads_ready=None):
-        """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` is final (the ImpalaCNN
-        backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`."""
-        lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
-        loss, dlog = self._bc_dlog(pd, actions, img.shape[0] * img.shape[1])
-        self._backward_from_dlog(dlog, lat_bf16, tape, img.shape[0], img.shape[1], upper_grads_ready)
-        return loss, state_out
-
     def _taped_forward(self, img, first, state_in):
         """The inference kernels, recording what the backward needs -> (latent bf16, pd, vpred, tape, state_out)."""
         pol, net = self.policy, self.policy.net
@@ -248,7 +228,7 @@ class BCTrainer:
         tape = dict(stacks=[], blocks=[])
         net._tape = tape
         try:
-            lat_bf16, _, state_out = net._forward_impl(img, first, state_in)
+            lat_bf16, _, state_out = net._forward_impl(img, first, state_in, use_lastlayer=self.use_lastlayer)
         finally:
             net._tape = None
         if self.keep_tape:
@@ -256,60 +236,44 @@ class BCTrainer:
         pd, vpred = pol._heads(lat_bf16, B, t)
         return lat_bf16, pd, vpred, tape, state_out
 
-    def _bc_dlog(self, pd, actions, N):
-        """The BC loss -mean log p(action) over the N frames and its gradient wrt the logits, bf16 [N][ld_logits]."""
-        pol = self.policy
-        hp = pol._heads_prepared()
-        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=pol.net.final_ln.weight.device)
-        scale = 1.0 / (pol.temperature * N)
-        logp = None
-        for name, (shape, n) in pol.head_specs.items():
-            c0, width = hp["cols"][name]
-            if width != n:
-                raise NotImplementedError("BCTrainer: heads with several sub-actions are not trained by the reference")
-            idx = actions[name].reshape(N).to(torch.int64)
-            lp = ops.gather_logprob(pd[name].reshape(N, n), idx)
-            logp = lp if logp is None else logp + lp
-            ops.softmax_bwd(pd[name].reshape(N, n), idx, scale, dlog, c0)
-        return -logp.sum() / N, dlog
-
     def _backward_from_dlog(self, dlog, lat_bf16, tape, B, t, upper_grads_ready):
-        """Everything below the logits: the head weights, then final_ln, lastlayer, the transformer, the dense layer and the ImpalaCNN."""
+        """Everything below the logits: the head weights, then final_ln [, lastlayer], the transformer, the dense layer and the ImpalaCNN.
+        Returns the gradient wrt the CNN input when stack 0's first conv is a normalised one (the IDM: the conv3d output), else None."""
         cfg = self.policy.net.cfg
         wts = self._weights()
         P = dict(self.policy.net.named_parameters())
         h = cfg.hidsize
         # ---------------- heads ----------------
-        lins = self._head_layers()
         dWh = ops.wgrad(dlog, lat_bf16)
         dbh = ops.col_sums(dlog)[1]
         c0 = 0
-        for lin in lins:
+        for lin in self._head_layers():
             m = lin.weight.shape[0]
             _acc(lin.weight, dWh[c0:c0 + m])
             _acc(lin.bias, dbh[c0:c0 + m])
             c0 += m
         dlat = self._gemm(dlog, wts["heads_t"], h)
-        self._dbg("latent", dlat)
         del dlog
-        # ---------------- final_ln (plain norm) + lastlayer ----------------
-        ident = lambda v: v
-        fg = P["final_ln.weight"]
+        # ---------------- final_ln (plain norm) on lastlayer's output, or on relu(recurrent output) without lastlayer ----------------
         # (xl, z_last, x0, xd and the convs' h are ReLU outputs that feed a norm: their ReLU backward rides on that norm's apply pass)
-        dz = self._norm_bwd(dlat, tape["xl"], tape["mr_xl"], fg.detach().float().contiguous(), 1, h, (fg, ident), (P["final_ln.bias"], ident),
-                            relu_x=True)
-        dx = self._normlinear_bwd(dz, tape["z_last"], tape["mr_zl"], wts["last_t"], "lastlayer", P, relu_x=True)
+        if self.use_lastlayer:
+            x, mr = tape["xl"], tape["mr_xl"]
+        else:  # lib/policy.py:389-392: the last block's z, relu fused into its epilogue
+            x, mr = tape["blocks"][-1]["z"], tape["blocks"][-1]["mr_z"]
+        fg = P["final_ln.weight"]
+        dx = self._norm_bwd(dlat, x, mr, fg.detach().float().contiguous(), 1, h, fg, P["final_ln.bias"], relu_x=True)
+        if self.use_lastlayer:
+            dx = self._normlinear_bwd(dx, tape["z_last"], tape["mr_zl"], wts["last_t"], "lastlayer", P, relu_x=True)
         # ---------------- transformer blocks, last to first ----------------
         for l in reversed(range(cfg.n_layers)):
-            self._dbg(f"recurrent_layer.blocks.{l}" if l < cfg.n_layers - 1 else "recurrent_out", dx)
-            dx = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t, last=(l == cfg.n_layers - 1))
+            dx = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t)
         # ---------------- img_process.linear, dense ----------------
         dz = self._normlinear_bwd(dx, tape["xd"], tape["mr_d"], wts["linear_t"], "img_process.linear", P, relu_x=True)
         dcnn = self._dense_bwd(dz, tape, wts, P)
         if upper_grads_ready is not None:
             upper_grads_ready()
         # ---------------- ImpalaCNN, last stack to first ----------------
-        self._cnn_bwd(dcnn, tape, wts, P)
+        return self._cnn_bwd(dcnn, tape, wts, P)
 
     def _dense_bwd(self, dz, tape, wts, P):
         cfg = self.policy.net.cfg
@@ -323,17 +287,13 @@ class BCTrainer:
         u, _, _ = ops.affine_norm(x, tape["mr_c"], wts["dense_g"], wts["dense_b"], rows_per_group=1)
         dWz = self._wgrad_linear(dz, u)  # [out][Kd] in ZP column order
         del u
-
-        def unperm(v):  # ZP (h, w, c) order -> the reference's C,H,W flatten order (dropping the pad row / column)
-            v = v.reshape(*v.shape[:-1], Hf + 1, Wf + 1, C2)[..., :Hf, :Wf, :]
-            return v.movedim(-1, -3).reshape(*v.shape[:-3], -1)
-
+        unperm = lambda v: _dense_from_zp(v, cfg)
         _acc(P[pfx + ".layer.weight"], unperm(dWz))
         del dWz
-        return self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, (P[pfx + ".norm.weight"], unperm),
-                              (P[pfx + ".norm.bias"], unperm), zp=(Hf, Wf, C2)).view(N, Hf + 1, Wf + 1, C2)
+        return self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, P[pfx + ".norm.weight"], P[pfx + ".norm.bias"],
+                              grad_map=unperm, zp=(Hf, Wf, C2)).view(N, Hf + 1, Wf + 1, C2)
 
-    def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t, last):
+    def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t):
         """Backward of lib/util.py:193-211 (see policy.MinecraftPolicy._block for the forward in the same notation)."""
         cfg = self.policy.net.cfg
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
@@ -341,7 +301,7 @@ class BCTrainer:
         o = f"{b}.r.orc_block"
         N = B * t
         nr = 10 * heads
-        dz = dzo  # (last block: z is relu(..) (lib/policy.py:211 fused into its epilogue); lastlayer's norm backward already masked dzo)
+        dz = dzo  # (last block: z is relu(..) (lib/policy.py:211 fused into its epilogue); the norm backward above already masked dzo)
         # mlp1: z = y + hmid W1^T + b1
         dh = self._gemm(dz, W["mlp1_t"], h * cfg.pointwise_ratio)
         self._wgrad_linear(dz, S["hmid"], P[f"{b}.mlp1.layer.weight"])
@@ -379,9 +339,8 @@ class BCTrainer:
             _acc(P[f"{o}.r_layer.weight"], torch.zeros_like(P[f"{o}.r_layer.weight"], dtype=F32))
             _acc(P[f"{o}.r_layer.bias"], torch.zeros_like(P[f"{o}.r_layer.bias"], dtype=F32))
         # pre_r_ln (plain norm of the block input)
-        ident = lambda v: v
         g = P[f"{b}.pre_r_ln.weight"]
-        return self._norm_bwd(dxhat, S["x"], S["mr_x"], g.detach().float().contiguous(), 1, h, (g, ident), (P[f"{b}.pre_r_ln.bias"], ident),
+        return self._norm_bwd(dxhat, S["x"], S["mr_x"], g.detach().float().contiguous(), 1, h, g, P[f"{b}.pre_r_ln.bias"],
                               relu_x=(l == 0))  # block 0's input is relu(img_process.linear)
 
     def _cnn_bwd(self, dout, tape, wts, P):
@@ -389,7 +348,6 @@ class BCTrainer:
         CNN input when stack 0's first conv is a normalised one (the IDM: the conv3d output, ReLU backward applied), else None."""
         cfg = self.policy.net.cfg
         pfx = "img_process.cnn"
-        ident = lambda v: v
         dx = dout
         for i in reversed(range(len(cfg.chans))):
             rec = tape["stacks"][i]
@@ -399,7 +357,6 @@ class BCTrainer:
             R = dx.shape[0] * (H + 1) * (W + 1)
             for j in (1, 0):
                 blk = rec["blocks"][j]
-                self._dbg(f"{s}.blocks.{j}", dx)
                 x_in = rec["blocks"][j - 1]["x"] if j == 1 else rec["x0"]
                 mr_in = rec["blocks"][j - 1]["mr"] if j == 1 else rec["mr0"]
                 # x_out = x_in + relu(conv1(GN(h)));  h = relu(conv0(GN(x_in)))
@@ -409,12 +366,10 @@ class BCTrainer:
                 del dz1
                 dx = self._normconv_bwd(dz0, x_in, mr_in, H, W, wts["stacks"][i]["convs"][2 * j], f"{s}.blocks.{j}.conv0", P, add=dx)
                 del dz0
-            self._dbg(f"{s}.n", dx)
             # x0 = GN_n(y1) (plain norm)
             g = P[f"{s}.n.weight"]
             dy1 = self._norm_bwd(dx.view(R, C), rec["y1"].view(R, C), rec["mr1"], g.detach().float().contiguous(), (H + 1) * (W + 1), H * W * C,
-                                 (g, ident), (P[f"{s}.n.bias"], ident), zp=(H, W, C)).view(rec["y1"].shape)
-            self._dbg(f"{s}.pool", dy1)
+                                 g, P[f"{s}.n.bias"], zp=(H, W, C)).view(rec["y1"].shape)
             if i == 0 and not cfg.first_conv_norm:
                 st = self.policy.net.prepared().stacks[0]
                 dWk, db = ops.firstconv_bwd(tape["frames"], st["fc_w"], st["fc_b"], dy1, C)
@@ -431,9 +386,55 @@ class BCTrainer:
         return dx
 
 
+class BCTrainer(_Trainer):
+    """Behavioural-cloning step of `MinecraftAgentPolicy` (behavioural_cloning.py:101-123):
+    `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions)` accumulates d loss / d param into `.grad`.
+
+        loss = -(1 / (B*T)) * sum_{b,t} sum_heads log_softmax(logits_head / temperature)[action]      (lib/action_head.py:176-184)
+    """
+
+    def __init__(self, policy: MinecraftAgentPolicy):
+        if not isinstance(policy, MinecraftAgentPolicy):
+            raise TypeError(f"{type(self).__name__} trains a MinecraftAgentPolicy (behavioural_cloning.py:54-62)")
+        cfg = policy.net.cfg
+        if cfg.conv3d_out is not None or cfg.first_conv_norm or cfg.mask_style != "clipped_causal":
+            raise NotImplementedError(f"{type(self).__name__}: only the causal policy models are trained by the reference")
+        super().__init__(policy)
+
+    def _check_heads(self):
+        """Every head must have a single sub-action.  Checked before the forward: nothing is accumulated into .grad by a call that
+        cannot finish."""
+        pol = self.policy
+        if any(getattr(pol.pi_head, name).linear_layer.weight.shape[0] != n for name, (shape, n) in pol.head_specs.items()):
+            raise NotImplementedError(f"{type(self).__name__}: heads with several sub-actions are not trained by the reference")
+
+    def loss_and_grad(self, img, first, state_in, actions, upper_grads_ready=None):
+        """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` is final (the ImpalaCNN
+        backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`."""
+        self._check_heads()
+        lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
+        loss, dlog = self._bc_dlog(pd, actions, img.shape[0] * img.shape[1])
+        self._backward_from_dlog(dlog, lat_bf16, tape, img.shape[0], img.shape[1], upper_grads_ready)
+        return loss, state_out
+
+    def _bc_dlog(self, pd, actions, N):
+        """The BC loss -mean log p(action) over the N frames and its gradient wrt the logits, bf16 [N][ld_logits]."""
+        pol = self.policy
+        hp = pol._heads_prepared()
+        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=pol.net.final_ln.weight.device)
+        scale = 1.0 / (pol.temperature * N)
+        logp = None
+        for name, (shape, n) in pol.head_specs.items():
+            idx = actions[name].reshape(N).to(torch.int64)
+            lp = ops.gather_logprob(pd[name].reshape(N, n), idx)
+            logp = lp if logp is None else logp + lp
+            ops.softmax_bwd(pd[name].reshape(N, n), idx, scale, dlog, hp["cols"][name][0])
+        return -logp.sum() / N, dlog
+
+
 class RLTrainer(BCTrainer):
     """RL fine-tuning step of `MinecraftAgentPolicy`: a clipped policy-gradient (PPO) loss, the value head's loss and a KL penalty to the
-    frozen pretrained policy, with the hand-written backward of `BCTrainer`.  Over the N = B*T frames of one call:
+    frozen pretrained policy, with the shared hand-written backward.  Over the N = B*T frames of one call:
 
         lp      = sum over heads of log pi(a)                     (get_logprob_of_action, lib/policy.py:271-279)
         ratio   = exp(lp - old_logprob)
@@ -477,9 +478,7 @@ class RLTrainer(BCTrainer):
             for name, (shape, n) in pol.head_specs.items():
                 if pd_ref[name].dtype != F32 or pd_ref[name].numel() != N * n:
                     raise ValueError(f"RLTrainer: pd_ref[{name!r}] must be fp32 with {N} x {n} log-probs (got {tuple(pd_ref[name].shape)})")
-        # check every head before the forward: nothing is accumulated into .grad by a call that cannot finish
-        if any(getattr(pol.pi_head, name).linear_layer.weight.shape[0] != n for name, (shape, n) in pol.head_specs.items()):
-            raise NotImplementedError("RLTrainer: heads with several sub-actions are not trained by the reference")
+        self._check_heads()
         lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, first, state_in)
         loss, dlog = self._rl_dlog(pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N)
         self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
@@ -514,9 +513,9 @@ class RLTrainer(BCTrainer):
         return loss, dlog
 
 
-class IDMTrainer(BCTrainer):
-    """Training step of the inverse dynamics model (`InverseActionPolicy`, lib/policy.py:342-467) with the same hand-written backward as
-    `BCTrainer`:  `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions)` accumulates d loss / d param into `.grad`.
+class IDMTrainer(_Trainer):
+    """Training step of the inverse dynamics model (`InverseActionPolicy`, lib/policy.py:342-467) with the shared hand-written backward:
+    `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions)` accumulates d loss / d param into `.grad`.
 
         loss = -(1 / (B*T)) * sum_{b,t} sum_heads sum_sub-actions log_softmax(logits / temperature)[action]
 
@@ -531,6 +530,7 @@ class IDMTrainer(BCTrainer):
     (None, (B,0,h), (B,0,h))."""
 
     max_t = 128  # frames per sequence the unmasked attention backward supports
+    use_lastlayer = False  # the IDM's forward discards lastlayer's output (lib/policy.py:390-391)
 
     def __init__(self, policy: InverseActionPolicy):
         if not isinstance(policy, InverseActionPolicy):
@@ -540,7 +540,7 @@ class IDMTrainer(BCTrainer):
             raise NotImplementedError("IDMTrainer: needs the IDM configuration (conv3d pre-stage, attention mask 'none', no KV memory)")
         if cfg.timesteps is not None and cfg.timesteps > self.max_t:
             raise NotImplementedError(f"IDMTrainer: the unmasked attention backward supports chunks of at most {self.max_t} frames")
-        self._init_state(policy)  # (BCTrainer.__init__ refuses the IDM by design)
+        super().__init__(policy)
 
     @staticmethod
     def optimizer_params(policy):
@@ -551,72 +551,35 @@ class IDMTrainer(BCTrainer):
         named = [(n, p) for n, p in policy.named_parameters() if not n.startswith("net.lastlayer.")]
         return [p for n, p in named if n.startswith("net.conv3d_layer.")] + [p for n, p in named if not n.startswith("net.conv3d_layer.")]
 
-    def _build_weights(self):
-        """Backward-side layouts: every stack's first conv is normalised (rotated like the block convs), Q | K | V only, no lastlayer."""
-        pol, net = self.policy, self.policy.net
-        cfg = net.cfg
-        P = dict(net.named_parameters())
-        w = dict(stacks=[], layers=[])
-        pfx = "img_process.cnn"
-        for i in range(len(cfg.chans)):
-            s = f"{pfx}.stacks.{i}"
-            w["stacks"].append(dict(convs=[_rot(P[f"{s}.blocks.{j}.conv{k}.layer.weight"]) for j in range(2) for k in range(2)],
-                                    first=_rot(P[f"{s}.firstconv.layer.weight"])))
-        Hf, Wf = cfg.final_hw
-        C2 = cfg.chans[-1]
-
-        def perm(v):  # reference C,H,W flatten order -> ZP (h, w, c) order (as BCTrainer._build_weights)
-            v = v.reshape(*v.shape[:-1], C2, Hf, Wf).movedim(-3, -1)
-            v = torch.nn.functional.pad(v, (0, 0, 0, 1, 0, 1))
-            return v.reshape(*v.shape[:-3], -1)
-
-        w["dense_t"] = _tr(perm(P[f"{pfx}.dense.layer.weight"].detach()))
-        w["dense_g"] = perm(P[f"{pfx}.dense.norm.weight"].detach()).float().contiguous()
-        w["dense_b"] = perm(P[f"{pfx}.dense.norm.bias"].detach()).float().contiguous()
-        w["linear_t"] = _tr(P["img_process.linear.layer.weight"])
-        h = cfg.hidsize
-        self.kcat = 3 * h
-        for l in range(cfg.n_layers):
-            o = f"recurrent_layer.blocks.{l}.r.orc_block"
-            b = f"recurrent_layer.blocks.{l}"
-            cat = torch.cat([P[f"{o}.q_layer.weight"], P[f"{o}.k_layer.weight"], P[f"{o}.v_layer.weight"]], 0)
-            w["layers"].append(dict(qkvr_t=_tr(cat), proj_t=_tr(P[f"{o}.proj_layer.weight"]), mlp0_t=_tr(P[f"{b}.mlp0.layer.weight"]),
-                                    mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
-        self.ntot = sum(getattr(pol.pi_head, name).linear_layer.weight.shape[0] for name in pol.head_specs)
-        self.ld_logits = (self.ntot + 7) // 8 * 8
-        cat = torch.cat([getattr(pol.pi_head, name).linear_layer.weight for name in pol.head_specs], 0)
-        w["heads_t"] = _tr(cat, self.ld_logits)
-        return w
-
     def loss_and_grad(self, img, first, state_in, actions, upper_grads_ready=None):
         """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` and `conv3d_layer.*` is final
         (the CNN backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`.  Build the optimizer from
         `optimizer_params(policy)` so that those final gradients are one contiguous bucket slice."""
-        pol, net = self.policy, self.policy.net
-        cfg = net.cfg
-        self.refresh_weights()
-        wts = self._weights()
-        P = dict(net.named_parameters())
+        net = self.policy.net
         B, t = img.shape[:2]
         N = B * t
-        h = cfg.hidsize
+        # checked before the forward: nothing is accumulated into .grad by a call that cannot finish
         if N > net.idm_chunk_frames:
             raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls")
-        if t > self.max_t:  # checked before the forward: nothing is accumulated into .grad by a call that cannot finish
+        if t > self.max_t:
             raise NotImplementedError(f"IDMTrainer: at most {self.max_t} frames per sequence (got T = {t})")
-        # ---------------- forward (the inference kernels, recording what the backward needs) ----------------
-        tape = dict(stacks=[], blocks=[])
-        net._tape = tape
-        try:
-            lat_bf16, _, state_out = net._forward_impl(img, first, state_in, use_lastlayer=False)
-        finally:
-            net._tape = None
-        if self.keep_tape:
-            self.last_tape = tape
-        pd, _ = pol._heads(lat_bf16, B, t)
-        # ---------------- loss + d logits (one launch per factored head) ----------------
+        lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
+        loss, dlog = self._idm_dlog(pd, actions, N)
+        dx3 = self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
+        # the conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
+        C3 = net.cfg.conv3d_out
+        dW3, db3 = ops.conv3d_t5_bwd(img.contiguous(), dx3, C3)
+        del dx3
+        _acc(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
+        _acc(net.conv3d_layer.layer.bias, db3)
+        return loss, state_out
+
+    def _idm_dlog(self, pd, actions, N):
+        """The loss -mean sum log p(action) over the N frames and every sub-action, and its gradient wrt the logits, bf16 [N][ld_logits]
+        (one launch per factored head)."""
+        pol = self.policy
         hp = pol._heads_prepared()
-        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=img.device)
+        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=pol.net.final_ln.weight.device)
         scale = 1.0 / (pol.temperature * N)
         logp = None
         for name, (shape, n) in pol.head_specs.items():
@@ -624,40 +587,4 @@ class IDMTrainer(BCTrainer):
             groups = width // n
             idx = actions[name].reshape(N, groups).to(torch.int64)
             logp = ops.softmax_nll_bwd_grouped(pd[name].reshape(N, groups, n), idx, scale, dlog, c0, lp=logp)
-        loss = -logp.sum() / N
-        # ---------------- heads ----------------
-        dWh = ops.wgrad(dlog, lat_bf16)[: self.ntot]
-        dbh = ops.col_sums(dlog)[1]
-        for name in pol.head_specs:
-            c0, width = hp["cols"][name]
-            lin = getattr(pol.pi_head, name).linear_layer
-            _acc(lin.weight, dWh[c0:c0 + width])
-            _acc(lin.bias, dbh[c0:c0 + width])
-        dlat = self._gemm(dlog, wts["heads_t"], h)
-        self._dbg("latent", dlat)
-        del dlog
-        # ---------------- final_ln on relu(recurrent output) (lib/policy.py:389-392; lastlayer is not on the path) ----------------
-        ident = lambda v: v
-        fg = P["final_ln.weight"]
-        last = tape["blocks"][-1]
-        dx = self._norm_bwd(dlat, last["z"], last["mr_z"], fg.detach().float().contiguous(), 1, h, (fg, ident), (P["final_ln.bias"], ident),
-                            relu_x=True)
-        # ---------------- transformer blocks, last to first ----------------
-        for l in reversed(range(cfg.n_layers)):
-            self._dbg(f"recurrent_layer.blocks.{l}" if l < cfg.n_layers - 1 else "recurrent_out", dx)
-            dx = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t, last=(l == cfg.n_layers - 1))
-        # ---------------- img_process.linear, dense ----------------
-        dz = self._normlinear_bwd(dx, tape["xd"], tape["mr_d"], wts["linear_t"], "img_process.linear", P, relu_x=True)
-        dcnn = self._dense_bwd(dz, tape, wts, P)
-        if upper_grads_ready is not None:
-            upper_grads_ready()
-        # ---------------- ImpalaCNN, last stack to first, then the conv3d pre-stage ----------------
-        dx3 = self._cnn_bwd(dcnn, tape, wts, P)
-        self._dbg("conv3d", dx3)
-        C3 = cfg.conv3d_out
-        dW3, db3 = ops.conv3d_t5_bwd(img.contiguous(), dx3, C3)
-        del dx3
-        # kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
-        _acc(P["conv3d_layer.layer.weight"], (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
-        _acc(P["conv3d_layer.layer.bias"], db3)
-        return loss, state_out
+        return -logp.sum() / N, dlog
