@@ -4,8 +4,8 @@
 Every class runs the launches the forward makes at that shape, with the same arguments (per-frame GroupNorm fold `mr` + `S1/S2`,
 block 0's two-norm composition `Ef` / `res_scale, res_shift`, the residual on each block's second conv, statistics partials where
 the forward asks for them), and is timed with CUDA events around the kernel launches only (no statistics finalize).  Each class is
-timed with the epilogue on and with the epilogue body switched off (vpt_set_conv_pair_mode(0x20): main loop + accumulator staging
-only), so the gap is what the epilogue costs.
+timed with the epilogue on and with the epilogue body switched off (vpt_set_conv_pair_mode(0x20): the main loop only; the
+accumulators are dropped), so the gap is what the epilogue costs.
     python tools/conv_bench.py [--frames 2048] [--reps 3] [--json OUT]"""
 import argparse
 import ctypes as C

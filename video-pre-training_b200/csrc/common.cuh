@@ -292,6 +292,20 @@ __device__ __forceinline__ void wgmma_frag_store(const float (&d)[NR], float* st
         *reinterpret_cast<float2*>(stg + (size_t)(r0 + 8) * pitch + c0 + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
     }
 }
+// One 32-column chunk (columns 32 * C .. 32 * C + 31 of the fragment: registers 16 * C .. 16 * C + 15) of the calling warp's 16 rows
+// of `d` -> rows 0..15 of the warp's own row-major fp32 block `blk` [16][pitch].  Only the calling warp's rows are touched, so
+// __syncwarp orders the block.  C is a template parameter: a run-time index into the fragment would put it in local memory.
+template <int C, int NR>
+__device__ __forceinline__ void wgmma_frag_store_chunk(const float (&d)[NR], float* blk, int pitch) {
+    static_assert(16 * C + 16 <= NR, "chunk outside the fragment");
+    const int l = threadIdx.x & 31;
+    float* dst = blk + (size_t)(l >> 2) * pitch + 2 * (l & 3);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(d[16 * C + 4 * i], d[16 * C + 4 * i + 1]);
+        *reinterpret_cast<float2*>(dst + (size_t)8 * pitch + 8 * i) = make_float2(d[16 * C + 4 * i + 2], d[16 * C + 4 * i + 3]);
+    }
+}
 // 32 consecutive fp32 values of one staging row (16-byte aligned) as raw words
 __device__ __forceinline__ void stg_ld_32(const float* src, uint32_t (&v)[32]) {
 #pragma unroll

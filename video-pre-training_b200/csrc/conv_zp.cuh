@@ -14,15 +14,19 @@
 //
 //   warpgroups 0, 1 (warps 0..7): MMA + epilogue, ping-pong.  Each owns a whole 128-row x BN tile (one m64nBNk16 per 64-row
 //       half and k16 step) and they take alternate tiles of the CTA's persistent sequence.  Named barriers let one warpgroup at a
-//       time issue main-loop MMAs, so one warpgroup's epilogue runs while the other's main loop keeps the tensor pipe busy; a second
-//       pair hands the single fp32 staging tile from one epilogue to the next.  A span and weight stages are released one MMA
-//       group late, so MMAs stay in flight across channel blocks and drain only at the end of a tile.
+//       time issue main-loop MMAs, so one warpgroup's epilogue runs while the other's main loop keeps the tensor pipe busy.  That
+//       pair is the only synchronisation between the warpgroups: the epilogues share nothing, so both can run at once.  A span and
+//       weight stages are released one MMA group late, so MMAs stay in flight across channel blocks and drain only at the end of
+//       a tile.
 //   warpgroup 2: warp 8 = A-span TMA producer, warp 9 = weight TMA producer (both in tile order), registers handed to the MMA
 //       warpgroups with setmaxnreg.
 // Epilogue = GroupNorm fold (border-class tables), ReLU, residual, bf16 store in ZP layout (border rows are written as
 // zeros, which maintains the layout invariant), per-row (sum, sumsq) partials for the next layer's statistics.  One thread per
-// row does the arithmetic; the residual and the bf16 result pass through the warp's staging rows so that global memory sees
-// 64-byte row segments.
+// row does the arithmetic.  The accumulators stay in registers through the epilogue; an epilogue warp takes the 32 rows its own
+// fragment holds (rows 16w .. 16w+15 of each 64-row half) and passes them, 32 columns at a time, through a 32 x 32 fp32 block of
+// shared memory that no other warp touches, so __syncwarp is all the epilogue needs.  The residual and the bf16 result pass
+// through the same block so that global memory sees 64-byte row segments; a chunk's residual is loaded a chunk ahead (the first
+// one while the tile's last MMAs drain).
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.cuh"
@@ -35,9 +39,13 @@ constexpr int kCzThreads = 384;  // 3 warpgroups
 constexpr int kCzMaxBStages = 8;
 constexpr int kCzProducerRegs = 24, kCzMmaRegs = 240;  // setmaxnreg budget: 128 * 24 + 256 * 240 <= 64 K registers
 
-// named barriers (0 is __syncthreads): kCzBarOrder + w = warpgroup w may issue its next main loop, kCzBarStg + w = warpgroup w may
-// write the staging tile, kCzBarWg + w = warpgroup w's own staging write -> epilogue read
-constexpr int kCzBarOrder = 1, kCzBarStg = 3, kCzBarWg = 5;
+// named barriers (0 is __syncthreads): kCzBarOrder + w = warpgroup w may issue its next main loop
+constexpr int kCzBarOrder = 1;
+
+// epilogue staging: one 32-row x 32-column fp32 block per MMA warp.  Pitch 36 floats = 144 B keeps rows 16-byte aligned and puts
+// eight lanes reading consecutive rows on eight distinct 16-byte bank groups.
+constexpr int kCzStgPitch = 36;
+constexpr uint32_t kCzStgBytes = 8u * 32u * kCzStgPitch * 4u;
 
 struct ConvZpParams {
     long long Q;  // total rows = F * FS
@@ -68,6 +76,22 @@ __device__ __forceinline__ void cz_mma_k16(float (&acc)[BN / 2], uint64_t a_desc
         wgmma_n64<0, 0>(acc, a_desc, b_desc, accumulate);
 }
 
+// Chunk c (32 columns) of the calling warp's rows of both halves of a tile -> the warp's staging block, rows 0..15 from half 0 and
+// 16..31 from half 1.  The switch turns the run-time chunk index into the constant register indices the fragment needs.
+template <int BN>
+__device__ __forceinline__ void cz_stage_chunk(const float (&frag)[2][BN / 2], int c, float* wrows) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float* blk = wrows + (size_t)h * 16 * kCzStgPitch;
+        switch (c) {
+            case 0: wgmma_frag_store_chunk<0>(frag[h], blk, kCzStgPitch); break;
+            case 1: wgmma_frag_store_chunk<1>(frag[h], blk, kCzStgPitch); break;
+            case 2: if constexpr (BN == 128) wgmma_frag_store_chunk<2>(frag[h], blk, kCzStgPitch); break;
+            case 3: if constexpr (BN == 128) wgmma_frag_store_chunk<3>(frag[h], blk, kCzStgPitch); break;
+        }
+    }
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kCzThreads, 1)
 conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvZpParams p) {
@@ -79,17 +103,16 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr uint32_t b_stage_bytes = (uint32_t)BN * kBlockK * 2;
     uint8_t* smem_a = smem;                                        // 2 A-span stages
     uint8_t* smem_b = smem + 2 * (size_t)p.a_stage_bytes;          // b_stages weight tiles
-    float* stg = reinterpret_cast<float*>(smem_b + (size_t)p.b_stages * b_stage_bytes);  // one 128 x BN fp32 staging tile
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + kStgBytes);
+    float* stg = reinterpret_cast<float*>(smem_b + (size_t)p.b_stages * b_stage_bytes);  // the MMA warps' staging blocks
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + kCzStgBytes);
     uint64_t* a_full = bars;
     uint64_t* a_empty = bars + 2;
     uint64_t* b_full = bars + 4;
     uint64_t* b_empty = bars + 4 + kCzMaxBStages;
 
     const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
 
-    if (warp == 8 && lane == 0) {
+    if (threadIdx.x == 8 * 32) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < 2; ++i) {
@@ -112,7 +135,7 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
     if (warp >= 8) {
         setmaxnreg_dec<kCzProducerRegs>();
-        if (warp == 8 && lane == 0) {
+        if (threadIdx.x == 8 * 32) {
             // ================= A-span producer: one span per (tile, channel block), in tile order =================
             int stage = 0;
             uint32_t phase = 0;
@@ -129,7 +152,7 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     advance(stage, phase, 2);
                 }
             }
-        } else if (warp == 9 && lane == 0) {
+        } else if (threadIdx.x == 9 * 32) {
             // ================= weight producer: one [BN][64] tile per (tile, channel block, tap) =================
             int stage = 0;
             uint32_t phase = 0;
@@ -152,13 +175,23 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ================= MMA + epilogue: warpgroup wg owns the CTA's tiles 2i + wg of its sequence (ping-pong) =================
     setmaxnreg_inc<kCzMmaRegs>();
     const int wg = warp >> 2;
-    const int wwarp = warp & 3;  // this warp's 32-row quarter of the tile in the epilogue
-    float* my_row = stg + (size_t)(wwarp * 32 + lane) * kStgPitch;
-    const int nchunks = BN >> 5;
-    const int c_half = (nchunks + 1) >> 1;  // statistics partial 0 sums chunks [0, c_half), partial 1 the rest
+    const int lane = threadIdx.x & 31;
+    // Epilogue rows follow the fragment: warp w of a warpgroup holds rows 16w .. 16w+15 of each 64-row half, and those 32 rows are
+    // the ones it finishes.  Row i of the warp's staging block is tile row 64 * (i / 16) + 16w + i % 16; lane l works on row l.
+    const int wrow0 = (warp & 3) * 16;
+    float* wrows = stg + (size_t)warp * 32 * kCzStgPitch;
+    float* my_row = wrows + (size_t)lane * kCzStgPitch;
+    const int my_trow = ((lane >> 4) << 6) + wrow0 + (lane & 15);
+    // the coalesced residual loads / result stores take four lanes per row, eight block rows per step, four steps
+    const int seg = lane & 3;  // 16-byte piece of a 64-byte row segment
+    const int seg_row0 = lane >> 2, seg_trow0 = wrow0 + seg_row0;
+    const auto seg_row = [&](int k) { return seg_row0 + 8 * k; };                             // block row of step k
+    const auto seg_trow = [&](int k) { return seg_trow0 + ((k >> 1) << 6) + ((k & 1) << 3); };  // and its tile row
+    constexpr int nchunks = BN >> 5;
+    constexpr int c_half = (nchunks + 1) >> 1;  // statistics partial 0 sums chunks [0, c_half), partial 1 the rest
     const int P = p.num_n_tiles * 2;
     // with N % 8 == 0 and 16-byte aligned bases, rows of the residual and of res_scale / res_shift are read as 16-byte vectors
-    const bool res_vec = (((uintptr_t)p.residual | (uintptr_t)p.res_scale | (uintptr_t)p.res_shift) & 15) == 0;
+    const bool res_vec = ((p.N & 7) == 0) && (((uintptr_t)p.residual | (uintptr_t)p.res_scale | (uintptr_t)p.res_shift) & 15) == 0;
     const int b_per_tile = 9 * p.cin_blocks;
     for (int s = wg; tile_begin + s * tile_step < num_tiles; s += 2) {
         const int tile = tile_begin + s * tile_step;
@@ -209,6 +242,23 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         // every MMA of this tile is issued: the other warpgroup may start its main loop while these drain
         if (has_next) named_bar_arrive(kCzBarOrder + (wg ^ 1), 256);
+
+        // ---- epilogue.  Full chunks of 32 columns move their global data through the warp's staging block: once every lane holds
+        // its row's fp32 chunk in registers the block is free, so the residual comes in (bytes 0..63 of a row) and the bf16 result
+        // goes out (bytes 64..127) as 64-byte row segments, four lanes per row, instead of one 16-byte piece per row and lane.
+        // The residual is loaded into registers a chunk ahead, chunk 0's here while the MMAs drain.
+        const int q0 = m_tile * kBlockM;
+        const auto chunk_full = [&](int c) { return p.N - (n0 + c * 32) >= 32 && res_vec; };  // the same for every lane
+        uint4 res_next[4];
+        const auto res_load = [&](int c) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                res_next[k] = q0 + seg_trow(k) < p.Q
+                                  ? __ldg(reinterpret_cast<const uint4*>(p.residual + (size_t)(q0 + seg_trow(k)) * p.N + n0 + c * 32) + seg)
+                                  : make_uint4(0u, 0u, 0u, 0u);
+        };
+        if (p.residual != nullptr && p.dbg != 2 && chunk_full(0)) res_load(0);
+
         wgmma_wait<0>();
 #pragma unroll
         for (int h = 0; h < 2; ++h) wgmma_reg_fence(frag[h]);
@@ -216,18 +266,9 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
             if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
         }
-        if (!ok) {
-            if (has_next) named_bar_arrive(kCzBarStg + (wg ^ 1), 256);
-            break;
-        }
+        if (!ok) break;
 
-        // ---- accumulators -> staging tile, once the other warpgroup's epilogue has finished reading it
-        if (s > 0) named_bar_sync(kCzBarStg + wg, 256);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) wgmma_frag_store(frag[h], stg + (size_t)h * 64 * kStgPitch, kStgPitch, 0);
-        named_bar_sync(kCzBarWg + wg, 128);
-
-        const int q = m_tile * kBlockM + wwarp * 32 + lane;
+        const int q = q0 + my_trow;
         const bool row_ok = q < p.Q;
         // decode the ZP row: frame, y, x
         const int f = q / p.FS;
@@ -253,111 +294,105 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const float* rbrow = (p.res_scale && interior) ? p.res_shift + (size_t)f * p.N : nullptr;
         float st_s0 = 0.f, st_ss0 = 0.f, st_s1 = 0.f, st_ss1 = 0.f;  // statistics partials of the two column groups
 
-        // Chunks of 32 columns.  Full chunks move their global data through the warp's own staging rows: once every lane holds its
-        // row's fp32 chunk in registers, that chunk's 128 bytes of each row are free, so the residual comes in (bytes 0..63) and the
-        // bf16 result goes out (bytes 64..127) as 64-byte row segments, four lanes per row, instead of one 16-byte piece per row and
-        // lane.  The arithmetic per element is the same on both paths.
-        const int qw = m_tile * kBlockM + wwarp * 32;  // this warp's first row
-        float* wrows = stg + (size_t)(wwarp * 32) * kStgPitch;
-        const int seg = lane & 3;  // 16-byte piece of a 64-byte row segment in the coalesced loads / stores
+        // Chunks of 32 columns.  The arithmetic per element is the same on the full and the partial path.
 #pragma unroll 1
         for (int c = 0; c < (p.dbg == 2 ? 0 : nchunks); ++c) {
             const int g = c < c_half ? 0 : 1;
             const int nb = n0 + c * 32;
-            const int lim = min(32, min(BN - c * 32, p.N - nb));
+            const int lim = min(32, p.N - nb);
             if (lim <= 0) break;
-            const bool full = (lim == 32) && ((p.N & 7) == 0) && res_vec;  // the same for every lane
+            const bool full = chunk_full(c);
             uint32_t acc[32];
-            float v[32];
-            uint32_t pk[16];
+            __syncwarp();  // the previous chunk has left the block
+            cz_stage_chunk<BN>(frag, c, wrows);
+            __syncwarp();
+            stg_ld_32(my_row, acc);
             if (full) {
-                stg_ld_32(my_row + c * 32, acc);
                 __syncwarp();
                 if (p.residual != nullptr) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const int rr = 8 * k + (lane >> 2);
-                        if (qw + rr < p.Q)
-                            reinterpret_cast<uint4*>(wrows + (size_t)rr * kStgPitch + c * 32)[seg] =
-                                __ldg(reinterpret_cast<const uint4*>(p.residual + (size_t)(qw + rr) * p.N + nb) + seg);
-                    }
+                    for (int k = 0; k < 4; ++k)
+                        if (q0 + seg_trow(k) < p.Q) reinterpret_cast<uint4*>(wrows + (size_t)seg_row(k) * kCzStgPitch)[seg] = res_next[k];
+                    if (c + 1 < nchunks && chunk_full(c + 1)) res_load(c + 1);
                     __syncwarp();
                 }
                 if (row_ok) {
+                    uint4* dst = reinterpret_cast<uint4*>(my_row + 16);
                     if (!interior) {  // zero row / column of the ZP layout
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) pk[j] = 0u;
+                        for (int o = 0; o < 4; ++o) dst[o] = make_uint4(0u, 0u, 0u, 0u);
                     } else {
+                        float s_ = g ? st_s1 : st_s0, ss_ = g ? st_ss1 : st_ss0;
+                        // eight columns at a time, from the table loads to the packed result: the other chunks' accumulators are
+                        // live, so only a few loads can be in flight
 #pragma unroll
-                        for (int qq = 0; qq < 8; ++qq) {  // N % 8 == 0: the fold tables' rows are float4-aligned
-                            float4 a1 = s1row ? __ldg(reinterpret_cast<const float4*>(s1row + nb) + qq) : make_float4(0, 0, 0, 0);
-                            float4 a2 = s2row ? __ldg(reinterpret_cast<const float4*>(s2row + nb) + qq) : make_float4(0, 0, 0, 0);
-                            v[4 * qq + 0] = fmaf(ga, __uint_as_float(acc[4 * qq + 0]), fmaf(-gb, a1.x, a2.x));
-                            v[4 * qq + 1] = fmaf(ga, __uint_as_float(acc[4 * qq + 1]), fmaf(-gb, a1.y, a2.y));
-                            v[4 * qq + 2] = fmaf(ga, __uint_as_float(acc[4 * qq + 2]), fmaf(-gb, a1.z, a2.z));
-                            v[4 * qq + 3] = fmaf(ga, __uint_as_float(acc[4 * qq + 3]), fmaf(-gb, a1.w, a2.w));
-                        }
-                        if (p.relu == 1) {
+                        for (int o = 0; o < 4; ++o) {
+                            float v[8];
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                        }
-                        if (p.residual != nullptr) {
-                            const uint4* rp = reinterpret_cast<const uint4*>(my_row + c * 32);  // this row's residual, staged above
+                            for (int h = 0; h < 2; ++h) {  // N % 8 == 0: the fold tables' rows are float4-aligned
+                                const int qq = 2 * o + h;
+                                float4 a1 = s1row ? __ldg(reinterpret_cast<const float4*>(s1row + nb) + qq) : make_float4(0, 0, 0, 0);
+                                float4 a2 = s2row ? __ldg(reinterpret_cast<const float4*>(s2row + nb) + qq) : make_float4(0, 0, 0, 0);
+                                v[4 * h + 0] = fmaf(ga, __uint_as_float(acc[4 * qq + 0]), fmaf(-gb, a1.x, a2.x));
+                                v[4 * h + 1] = fmaf(ga, __uint_as_float(acc[4 * qq + 1]), fmaf(-gb, a1.y, a2.y));
+                                v[4 * h + 2] = fmaf(ga, __uint_as_float(acc[4 * qq + 2]), fmaf(-gb, a1.z, a2.z));
+                                v[4 * h + 3] = fmaf(ga, __uint_as_float(acc[4 * qq + 3]), fmaf(-gb, a1.w, a2.w));
+                            }
+                            if (p.relu == 1) {
 #pragma unroll
-                            for (int qq = 0; qq < 4; ++qq) {
-                                const uint4 rr = rp[qq];
+                                for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
+                            }
+                            if (p.residual != nullptr) {
+                                const uint4 rr = reinterpret_cast<const uint4*>(my_row)[o];  // this row's residual, staged above
                                 const float r8[8] = {bf16_lo(rr.x), bf16_hi(rr.x), bf16_lo(rr.y), bf16_hi(rr.y),
                                                      bf16_lo(rr.z), bf16_hi(rr.z), bf16_lo(rr.w), bf16_hi(rr.w)};
                                 if (rarow) {
-                                    const float4* ra4 = reinterpret_cast<const float4*>(rarow + nb) + 2 * qq;
-                                    const float4* rb4 = reinterpret_cast<const float4*>(rbrow + nb) + 2 * qq;
+                                    const float4* ra4 = reinterpret_cast<const float4*>(rarow + nb) + 2 * o;
+                                    const float4* rb4 = reinterpret_cast<const float4*>(rbrow + nb) + 2 * o;
                                     const float4 a0 = __ldg(ra4), a1 = __ldg(ra4 + 1), b0 = __ldg(rb4), b1 = __ldg(rb4 + 1);
                                     const float ra[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
                                     const float rb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
-                                    for (int j = 0; j < 8; ++j) v[8 * qq + j] += fmaf(ra[j], r8[j], rb[j]);
+                                    for (int j = 0; j < 8; ++j) v[j] += fmaf(ra[j], r8[j], rb[j]);
                                 } else {
 #pragma unroll
-                                    for (int j = 0; j < 8; ++j) v[8 * qq + j] += r8[j];
+                                    for (int j = 0; j < 8; ++j) v[j] += r8[j];
                                 }
                             }
-                        }
-                        if (p.relu == 2) {
+                            if (p.relu == 2) {
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) pk[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
-                        if (p.stat_part) {
-                            float s_ = g ? st_s1 : st_s0, ss_ = g ? st_ss1 : st_ss0;
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                const float lo = bf16_lo(pk[j]), hi = bf16_hi(pk[j]);
-                                s_ += lo; ss_ = fmaf(lo, lo, ss_);
-                                s_ += hi; ss_ = fmaf(hi, hi, ss_);
+                                for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
                             }
-                            if (g) { st_s1 = s_; st_ss1 = ss_; } else { st_s0 = s_; st_ss0 = ss_; }
-                        }
-                    }
+                            uint32_t pk[4];
 #pragma unroll
-                    for (int qq = 0; qq < 4; ++qq)
-                        reinterpret_cast<uint4*>(my_row + c * 32 + 16)[qq] = make_uint4(pk[4 * qq], pk[4 * qq + 1], pk[4 * qq + 2], pk[4 * qq + 3]);
+                            for (int j = 0; j < 4; ++j) pk[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
+                            if (p.stat_part) {
+#pragma unroll
+                                for (int j = 0; j < 4; ++j) {
+                                    const float lo = bf16_lo(pk[j]), hi = bf16_hi(pk[j]);
+                                    s_ += lo; ss_ = fmaf(lo, lo, ss_);
+                                    s_ += hi; ss_ = fmaf(hi, hi, ss_);
+                                }
+                            }
+                            dst[o] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                        }
+                        if (g) { st_s1 = s_; st_ss1 = ss_; } else { st_s0 = s_; st_ss0 = ss_; }
+                    }
                 }
                 __syncwarp();
                 if (p.dbg != 1) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const int rr = 8 * k + (lane >> 2);
-                        if (qw + rr < p.Q)
-                            reinterpret_cast<uint4*>(p.out + (size_t)(qw + rr) * p.N + nb)[seg] =
-                                reinterpret_cast<const uint4*>(wrows + (size_t)rr * kStgPitch + c * 32 + 16)[seg];
-                    }
+                    for (int k = 0; k < 4; ++k)
+                        if (q0 + seg_trow(k) < p.Q)
+                            reinterpret_cast<uint4*>(p.out + (size_t)(q0 + seg_trow(k)) * p.N + nb)[seg] =
+                                reinterpret_cast<const uint4*>(wrows + (size_t)seg_row(k) * kCzStgPitch + 16)[seg];
                 }
                 continue;
             }
             // ---- partial chunk (Cout not a multiple of the tile width / of 8): element by element, straight to global memory
             if (!row_ok) continue;
-            stg_ld_32(my_row + c * 32, acc);
+            float v[32];
+            uint32_t pk[16];
             __nv_bfloat16* op = p.out + (size_t)q * p.N + nb;
             if (!interior) {
                 for (int j = 0; j < lim; ++j) op[j] = __float2bfloat16_rn(0.f);
@@ -404,8 +439,6 @@ conv3x3_zp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     if (j < lim) op[j] = __float2bfloat16_rn(v[j]);
             }
         }
-        // the staging tile is free for the other warpgroup's next tile
-        if (has_next) named_bar_arrive(kCzBarStg + (wg ^ 1), 256);
         if (p.stat_part && row_ok)
             reinterpret_cast<float4*>(p.stat_part)[((size_t)q * P + n_tile * 2) >> 1] = make_float4(st_s0, st_ss0, st_s1, st_ss1);
     }
@@ -431,7 +464,8 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     const int H = a->H, W = a->W, C = a->Cin, N = a->Cout;
     VPT_CHECK(a->F > 0 && H >= 2 && W >= 2 && C > 0 && C % 64 == 0 && N > 0 && N % 16 == 0,
               "vpt_conv3x3_zp: need F>0, H,W>=2, Cin %% 64 == 0, Cout %% 16 == 0 (F=%d H=%d W=%d Cin=%d Cout=%d)", a->F, H, W, C, N);
-    // two stages of the 128 + 2*(W+2)-row input span, the fp32 staging tiles and two weight stages must fit in shared memory
+    // two stages of the 128 + 2*(W+2)-row input span, the warps' staging blocks and the weight stages share shared memory: up to
+    // this width at least four 128-column weight stages fit
     VPT_CHECK(W <= 182, "vpt_conv3x3_zp: W=%d too wide (at most 182: two input spans of 128 + 2*(W+2) rows must fit in shared memory)", W);
     VPT_CHECK(((uintptr_t)a->x & 15) == 0 && ((uintptr_t)a->w & 15) == 0 && ((uintptr_t)a->out & 15) == 0, "vpt_conv3x3_zp: pointers must be 16-byte aligned");
     ConvZpParams p;
@@ -448,7 +482,7 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     VPT_CHECK(p.a_box_rows <= 256, "vpt_conv3x3_zp: span does not fit the TMA box limit");
     p.a_stage_bytes = p.a_boxes * p.a_box_rows * 128;
     const uint32_t b_stage_bytes = (uint32_t)p.block_n * kBlockK * 2;
-    const size_t fixed_bytes = 1024 + 2 * (size_t)p.a_stage_bytes + kStgBytes + (4 + 2 * kCzMaxBStages) * 8;
+    const size_t fixed_bytes = 1024 + 2 * (size_t)p.a_stage_bytes + kCzStgBytes + (4 + 2 * kCzMaxBStages) * 8;
     int bst = (int)((227 * 1024 - (long long)fixed_bytes) / b_stage_bytes);
     if (bst > kCzMaxBStages) bst = kCzMaxBStages;
     VPT_CHECK(bst >= 2, "vpt_conv3x3_zp: not enough shared memory for the weight pipeline (W=%d Cout=%d)", W, N);
