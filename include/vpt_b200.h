@@ -430,6 +430,17 @@ int vpt_value_bwd(const float* vpred, const float* returns, const double* sums, 
                   float* debiasing_term, float w, float one_minus_w, float scale, void* out, int64_t ld_out, int32_t col, float* sq_err,
                   int64_t rows, void* stream);
 
+/* ----------------------------------------------------------------------------------------------------------
+ * Differentiable forward (training.py, set_autograd): the categorical heads' backward for any upstream gradient
+ * ---------------------------------------------------------------------------------------------------------- */
+/* Backward of logp = log_softmax(logits * scale) over each of `groups` groups of n columns, for the upstream gradient g = d loss / d logp
+ * (logp, g fp32 [rows][ld]; mask NULL or uint8 [rows][groups*n] dense, 0 = the logit was masked out, lib/action_head.py:170-171):
+ *   out[r][col0 + k*n + j] = scale * (g[r][k*n+j] - exp(logp[r][k*n+j]) * S[r][k]),  S[r][k] = sum_j g[r][k*n+j]   (bf16)
+ *                          = 0 where mask[r][k*n+j] == 0   (S still sums over the masked entries).
+ * Fixed-order sums, no atomics: bit-reproducible. */
+int vpt_log_softmax_bwd(const float* logp, int64_t ld_logp, const float* g, int64_t ld_g, const uint8_t* mask, int32_t groups, int32_t n, float scale,
+                        void* out, int64_t ld_out, int32_t col0, int64_t rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -148,6 +148,8 @@ SIGNATURES = {
     "vpt_rl_head_bwd": (_I, [_P, _L, _P, _L, _P, _P, _F, _F, _I, _P, _L, _I, _P, _I, _L, _P]),
     "vpt_ewma_sums": (_I, [_P, _L, _P, _P]),
     "vpt_value_bwd": (_I, [_P, _P, _P, _D, _P, _P, _P, _F, _F, _F, _P, _L, _I, _P, _L, _P]),
+    # differentiable forward (training.py, set_autograd)
+    "vpt_log_softmax_bwd": (_I, [_P, _L, _P, _L, _P, _I, _I, _F, _P, _L, _I, _L, _P]),
 }
 
 _lib = None

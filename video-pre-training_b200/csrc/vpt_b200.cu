@@ -32,6 +32,7 @@ void set_error(const char* fmt, ...) {
 #include "attention_full_bwd.cuh"
 #include "idm_bwd.cuh"
 #include "rl_bwd.cuh"
+#include "log_softmax_bwd.cuh"
 #include "firstconv_bwd.cuh"
 #include "precise.cuh"
 #include "codec.cuh"

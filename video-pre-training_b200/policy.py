@@ -13,8 +13,9 @@ parameter changes) they are re-laid-out for the kernels (`_Prepared`): conv weig
 the input GroupNorm gamma folded in plus the 9 border-class fold tables, linear weights with LayerNorm folded, the
 `dense` columns permuted from C,H,W to H,W,C order.
 
-`forward` runs under no_grad and returns detached tensors; the BC step has its own hand-written backward (training.py).
-There is no CPU path: CPU tensors raise.
+`forward` runs under no_grad and returns detached tensors; the trainers have their own hand-written backward (training.py).
+After `set_autograd(True)` a forward in grad mode (with a parameter that requires grad) is instead an autograd `Function` on that
+same backward, so that `loss.backward()` trains the model (training._AutogradRunner).  There is no CPU path: CPU tensors raise.
 """
 import math
 from collections import OrderedDict
@@ -344,6 +345,22 @@ def _fingerprint(module: nn.Module):
     return tuple((p.data_ptr(), p._version) for p in module.parameters())
 
 
+def _differentiable(module: nn.Module) -> bool:
+    """The forward builds an autograd graph only when asked to (`set_autograd`), in grad mode outside inference mode, and when at least
+    one parameter requires grad; otherwise the inference path runs, bit for bit."""
+    return module._autograd and torch.is_grad_enabled() and not torch.is_inference_mode_enabled() and \
+        any(p.requires_grad for p in module.parameters())
+
+
+def _autograd_runner(module: nn.Module):
+    """The module's differentiable-forward machinery (training._AutogradRunner), made on first use.  Tests read the tape of the last
+    differentiable call from it (`keep_tape` / `last_tape`, as with the trainers)."""
+    if module._ag_runner is None:
+        from .training import _AutogradRunner
+        module._ag_runner = _AutogradRunner(module)
+    return module._ag_runner
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # MinecraftPolicy
 # ---------------------------------------------------------------------------------------------------------------
@@ -368,9 +385,17 @@ class MinecraftPolicy(nn.Module):
         self._pprep_fp = None
         self.debug_taps = None  # set to a dict to capture intermediate activations (tests)
         self._tape = None       # set to a dict by training.BCTrainer: the forward then records what the backward needs
+        self._autograd = False  # set_autograd
+        self._ag_runner = None
 
     def output_latent_size(self):
         return self.hidsize
+
+    def set_autograd(self, on: bool = True):
+        """Opt in to the differentiable forward: in grad mode, with a parameter that requires grad, `forward` returns a latent attached
+        to the autograd graph (see `_PolicyBase.set_autograd`)."""
+        self._autograd = bool(on)
+        return self
 
     def initial_state(self, batchsize):
         """lib/policy.py:220-224 -> lib/xf.py:393-397: zeros on the module's device; state_mask None."""
@@ -580,7 +605,7 @@ class MinecraftPolicy(nn.Module):
         if tape is not None:
             if len(mrs) != 1:
                 raise NotImplementedError(f"training forward: at most {step} frames per call (got {N})")
-            tape.update(frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d)
+            tape.update(prep=prep, frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d)
         del cnn_out
         self._tap("img_process.cnn.dense", xd)
         x, mr_x = self._linear(xd, prep.linear, cfg.hidsize, mr=mr_d, relu=1, want_stats=True)
@@ -604,7 +629,10 @@ class MinecraftPolicy(nn.Module):
     def forward(self, ob, state_in, context):
         """lib/policy.py:193-218."""
         first = context["first"]
-        _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
+        if _differentiable(self):
+            (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
+        else:
+            _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
         if self.single_output:
             return latent, state_out
         return (latent, latent), state_out
@@ -621,7 +649,10 @@ class InverseActionNet(MinecraftPolicy):
     def forward(self, ob, state_in, context):
         """lib/policy.py:374-392 -> ((pi_latent, None), state_out)."""
         first = context["first"]
-        _, latent, state_out = self._forward_impl(ob["img"], first, state_in, use_lastlayer=False)
+        if _differentiable(self):
+            (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
+        else:
+            _, latent, state_out = self._forward_impl(ob["img"], first, state_in, use_lastlayer=False)
         return (latent, None), state_out
 
 
@@ -658,9 +689,23 @@ class _PolicyBase(nn.Module):
             self.head_specs[name] = (shape, n)
         self._hprep = None
         self._hprep_fp = None
+        self._autograd = False  # set_autograd
+        self._ag_runner = None
 
     def initial_state(self, batch_size: int):
         return self.net.initial_state(batch_size)
+
+    def set_autograd(self, on: bool = True):
+        """Opt in to the differentiable forward (also for `self.net` called on its own).  When on, a forward in grad mode (not inference
+        mode) with at least one parameter that requires grad runs the training forward (no stack-norm fold; within the 1e-2 tolerance of
+        the inference path, not bit-identical to it) as an autograd `Function` whose backward is the trainers' hand-written one, so that
+        `loss.backward()` accumulates into `.grad`.  pd and vpred are attached to the graph; `state_out` is detached and a `state_in`
+        that requires grad raises (no gradient through the KV memory, behavioural_cloning.py:109-111).  At most `net.cnn_chunk_frames`
+        (2048) frames per call (the IDM: `net.idm_chunk_frames` (512) and T <= 128), bf16 mode only.  A parameter that only feeds outputs
+        the loss does not use gets None, as in the reference.  `act`, `predict`, `v` and `GraphedAct` stay inference-only."""
+        self._autograd = bool(on)
+        self.net.set_autograd(on)
+        return self
 
     def set_precision(self, precision: str):
         """"bf16" (default, production: bf16 operands, 1e-2 tolerance) or "fp32" (fp32-parity mode, precise.py: 1e-3 tolerance)."""
@@ -758,12 +803,33 @@ class _PolicyBase(nn.Module):
         tot = None
         for name, (shape, n) in self.head_specs.items():
             lg = pd[name].contiguous()
-            lp = ops.gather_logprob(lg, ac[name].to(torch.int64))
+            idx = ac[name].to(torch.int64)
+            if lg.requires_grad and torch.is_grad_enabled():
+                lp = _GatherLogprob.apply(lg, idx)  # pd from the differentiable forward
+            else:
+                lp = ops.gather_logprob(lg, idx)
             for _ in shape:
                 lp = lp.sum(dim=-1)
             tot = lp if tot is None else tot + lp
         return tot
 
+
+
+class _GatherLogprob(torch.autograd.Function):
+    """`ops.gather_logprob` on log-probs attached to the graph: the same values; the backward scatters the gradient to the chosen class."""
+
+    @staticmethod
+    def forward(ctx, logits, idx):
+        ctx.save_for_backward(idx)
+        ctx.shape = logits.shape
+        return ops.gather_logprob(logits, idx)
+
+    @staticmethod
+    def backward(ctx, g):
+        (idx,) = ctx.saved_tensors
+        d = torch.zeros(ctx.shape, dtype=F32, device=g.device)
+        d.scatter_(-1, idx.reshape(*ctx.shape[:-1], 1), g.reshape(*ctx.shape[:-1], 1).to(F32))
+        return d, None
 
 
 class MinecraftAgentPolicy(_PolicyBase):
@@ -781,6 +847,10 @@ class MinecraftAgentPolicy(_PolicyBase):
             mask = obs.pop("mask", None)
         else:
             mask = None
+        if _differentiable(self):
+            outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
+            pi_logits = OrderedDict(zip(self.head_specs, outs[:-1]))
+            return (pi_logits, outs[-1], None), state_out
         lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in)
         B, t = obs["img"].shape[:2]
         pi_logits, vpred = self._heads(lat_bf16, B, t, mask)
@@ -875,6 +945,9 @@ class InverseActionPolicy(_PolicyBase):
             mask = obs.pop("mask", None)
         else:
             mask = None
+        if _differentiable(self):
+            outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
+            return (OrderedDict(zip(self.head_specs, outs)), None, None), state_out
         lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in, use_lastlayer=False)
         B, t = obs["img"].shape[:2]
         pi_logits, _ = self._heads(lat_bf16, B, t, mask)

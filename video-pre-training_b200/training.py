@@ -10,8 +10,12 @@ The three trainers share one path and differ only in the loss:
                             BCTrainer   -mean log p(demonstrated action)                        (behavioural_cloning.py:101-123)
                             RLTrainer   clipped policy gradient + value-head MSE + KL penalty    (the value head is one more column)
                             IDMTrainer  -mean sum over sub-actions log p(action)                  (factored heads)
-    _backward_from_dlog   the head weights, final_ln [-> lastlayer], the transformer, img_process.linear, dense and the ImpalaCNN;
-                          the IDM then adds its conv3d pre-stage
+    _backward_from_dlog   `_heads_bwd` (the head weights, dlog -> d latent), then `_backward_from_dlat`: final_ln [-> lastlayer],
+                          the transformer, img_process.linear, dense, the ImpalaCNN and, for the IDM, its conv3d pre-stage
+
+The differentiable forward (`set_autograd`, `_AutogradRunner` at the end of this file) runs the same taped forward and enters the same
+backward at dlog (any loss over pd / vpred, through `ops.log_softmax_bwd`) or at d latent (a bare network); its gradients go to a sink
+that hands them back to autograd instead of `param.grad`.
 
 What each layer type needs (u = gamma * n + beta is the normalised layer input, n = (x - mean) * rstd):
 
@@ -60,8 +64,11 @@ class _Trainer:
 
     use_lastlayer = True  # the model's forward runs `lastlayer` between the transformer and final_ln
 
-    def __init__(self, policy):
+    def __init__(self, policy, net=None):
+        """`policy` may be None with `net` given: a bare MinecraftPolicy / InverseActionNet (no heads; the differentiable forward)."""
         self.policy = policy
+        self.net = policy.net if net is None else net
+        self._sink = None  # None: gradients accumulate into `param.grad`; a dict: id(param) -> gradient (the differentiable forward)
         self._wprep = None
         self._wprep_fp = None
         self.keep_tape = False   # tests: keep the last forward's tape in `self.last_tape` (tests/forced_replica.py)
@@ -69,23 +76,34 @@ class _Trainer:
         self.graph_relayout = True  # re-layout of the kernel-side weights after an optimizer step as one CUDA graph replay
         self._rl_graph = None
         self._rl_seen = 0
-        cfg = policy.net.cfg
+        cfg = self.net.cfg
         h = cfg.hidsize
         # columns of the attention's input gradient: q | k | v, and R (10 basis rows per head) with the clipped_causal mask, padded to 8
         self.kcat = (3 * h + 10 * cfg.heads + 7) // 8 * 8 if cfg.mask_style == "clipped_causal" else 3 * h
-        self.ntot = sum(getattr(policy.pi_head, name).linear_layer.weight.shape[0] for name in policy.head_specs)  # action logits
+        pol = policy
+        self.ntot = 0 if pol is None else sum(getattr(pol.pi_head, name).linear_layer.weight.shape[0] for name in pol.head_specs)  # action logits
         self.ld_logits = (sum(lin.weight.shape[0] for lin in self._head_layers()) + 7) // 8 * 8  # columns of the logits gradient
 
     def _head_layers(self):
         """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order."""
         pol = self.policy
-        return [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
+        return [] if pol is None else [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
+
+    def _grad(self, p, g):
+        """Hands the gradient g of parameter p to the sink: `p.grad` (accumulated, `_acc`) or the dict of the differentiable forward."""
+        if self._sink is None:
+            _acc(p, g)
+            return
+        g = g.reshape(p.shape).to(F32)
+        prev = self._sink.get(id(p))
+        self._sink[id(p)] = g if prev is None else prev + g
 
     # -- backward-side weight layouts (re-made whenever a parameter changes, like policy._Prepared) -------------------
     def _weights_fp(self):
         """Versions of the parameters the kernel-layout copies are made from: all but the EWMA normaliser, which an RL step updates on
         every call and which no copy holds (`denormalize` keys it itself)."""
-        return tuple((p.data_ptr(), p._version) for n, p in self.policy.named_parameters() if not n.startswith("value_head.normalizer."))
+        mod = self.net if self.policy is None else self.policy
+        return tuple((p.data_ptr(), p._version) for n, p in mod.named_parameters() if not n.startswith("value_head.normalizer."))
 
     def _weights(self):
         fp = self._weights_fp()
@@ -101,7 +119,9 @@ class _Trainer:
         `_build_weights`) after an optimizer step.  Eagerly this is ~500 small torch launches;
         the parameters live at fixed addresses (FlatAdamDP's flat bucket), so from the second refresh on the whole re-layout is ONE captured
         CUDA graph replay writing the same kernel-layout tensors in place.  Called by `loss_and_grad`; a no-op when nothing changed."""
-        pol, net = self.policy, self.policy.net
+        pol, net = self.policy, self.net
+        if pol is None:
+            return  # a bare network: the lazy eager paths rebuild on use
         from .policy import _Prepared, _fingerprint
         fp_net, fp_heads = _fingerprint(net), pol._heads_fp()
         fp_all = self._weights_fp()
@@ -132,7 +152,7 @@ class _Trainer:
 
     def _build_weights(self):
         """The dgrad weights of every layer the backward runs through (builds weights only: it also runs inside the graph capture)."""
-        net = self.policy.net
+        net = self.net
         cfg = net.cfg
         P = dict(net.named_parameters())
         w = dict(stacks=[], layers=[])
@@ -157,7 +177,8 @@ class _Trainer:
                                     mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
         if self.use_lastlayer:
             w["last_t"] = _tr(P["lastlayer.layer.weight"])
-        w["heads_t"] = _tr(torch.cat([lin.weight for lin in self._head_layers()], 0), self.ld_logits)
+        if self._head_layers():
+            w["heads_t"] = _tr(torch.cat([lin.weight for lin in self._head_layers()], 0), self.ld_logits)
         return w
 
     # -- generic pieces -------------------------------------------------------------------------------------------------
@@ -169,16 +190,14 @@ class _Trainer:
         ops.gemm(A, Bt, out, M, N, K, residual=residual)
         return out
 
-    @staticmethod
-    def _wgrad_linear(dz, u, weight_param=None):
+    def _wgrad_linear(self, dz, u, weight_param=None):
         """dW [out][in] = dz^T u (wgmma GEMM over the token dimension); accumulated into `weight_param.grad` when given."""
         dW = ops.wgrad(dz, u)
         if weight_param is not None:
-            _acc(weight_param, dW)
+            self._grad(weight_param, dW)
         return dW
 
-    @staticmethod
-    def _norm_bwd(du, x, mr, gamma, rows_per_group, count, g_param, b_param, grad_map=None, zp=None, add=None, relu_x=False):
+    def _norm_bwd(self, du, x, mr, gamma, rows_per_group, count, g_param, b_param, grad_map=None, zp=None, add=None, relu_x=False):
         """Backward of n = (x - mean) * rstd, u = gamma * n + beta given du: accumulates dgamma / dbeta into `g_param` / `b_param`
         (through `grad_map` when the kernel-side gamma has another layout), returns dx (+ add).
         relu_x: x is the output of a ReLU whose backward is applied to the result in the same pass."""
@@ -187,8 +206,8 @@ class _Trainer:
         else:
             cs = ops.col_sums(du, x, mr, rows_per_group)
             ms = ops.group_sums(du, x, mr, gamma, rows_per_group, count)
-        _acc(g_param, cs[0] if grad_map is None else grad_map(cs[0]))
-        _acc(b_param, cs[1] if grad_map is None else grad_map(cs[1]))
+        self._grad(g_param, cs[0] if grad_map is None else grad_map(cs[0]))
+        self._grad(b_param, cs[1] if grad_map is None else grad_map(cs[1]))
         return ops.norm_bwd_apply(du, x, mr, gamma, ms, rows_per_group, zp=zp, add=add, relu_x=relu_x)
 
     def _normconv_bwd(self, dz, x, mr, H, W, W_rot, names, P, add=None, relu_x=False):
@@ -203,7 +222,7 @@ class _Trainer:
         shifts = [(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)]
         dWk = ops.wgrad(dz.view(R, Cout), u.view(R, Cin), shifts)  # [Cout][tap][Cin]
         del u
-        _acc(P[names + ".layer.weight"], dWk.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
+        self._grad(P[names + ".layer.weight"], dWk.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
         return self._norm_bwd(du.view(R, Cin), x.view(R, Cin), mr, g32, (H + 1) * (W + 1), H * W * Cin, gam, bet,
                               zp=(H, W, Cin), add=None if add is None else add.view(R, Cin), relu_x=relu_x).view(x.shape)
 
@@ -218,42 +237,56 @@ class _Trainer:
         return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], gam, bet, add=add, relu_x=relu_x)
 
     # -- the step ---------------------------------------------------------------------------------------------------------
-    def _taped_forward(self, img, first, state_in):
-        """The inference kernels, recording what the backward needs -> (latent bf16, pd, vpred, tape, state_out)."""
-        pol, net = self.policy, self.policy.net
+    def _taped_latent(self, img, first, state_in):
+        """The network's inference kernels, recording what the backward needs -> (latent bf16 [N][h], latent fp32 (B,t,h), tape, state_out).
+        The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`)."""
+        net = self.net
         self.refresh_weights()
-        self._weights()
-        B, t = img.shape[:2]
+        wts = self._weights()
         state_in = [(m, (k.detach(), v.detach())) for (m, (k, v)) in state_in]  # behavioural_cloning.py:111
-        tape = dict(stacks=[], blocks=[])
+        tape = dict(stacks=[], blocks=[], wts=wts)
         net._tape = tape
         try:
-            lat_bf16, _, state_out = net._forward_impl(img, first, state_in, use_lastlayer=self.use_lastlayer)
+            lat_bf16, lat_f32, state_out = net._forward_impl(img, first, state_in, use_lastlayer=self.use_lastlayer)
         finally:
             net._tape = None
         if self.keep_tape:
             self.last_tape = tape
-        pd, vpred = pol._heads(lat_bf16, B, t)
+        return lat_bf16, lat_f32, tape, state_out
+
+    def _taped_forward(self, img, first, state_in, mask=None):
+        """The inference kernels, recording what the backward needs -> (latent bf16, pd, vpred, tape, state_out)."""
+        B, t = img.shape[:2]
+        lat_bf16, _, tape, state_out = self._taped_latent(img, first, state_in)
+        pd, vpred = self.policy._heads(lat_bf16, B, t, mask)
         return lat_bf16, pd, vpred, tape, state_out
 
     def _backward_from_dlog(self, dlog, lat_bf16, tape, B, t, upper_grads_ready):
-        """Everything below the logits: the head weights, then final_ln [, lastlayer], the transformer, the dense layer and the ImpalaCNN.
-        Returns the gradient wrt the CNN input when stack 0's first conv is a normalised one (the IDM: the conv3d output), else None."""
-        cfg = self.policy.net.cfg
-        wts = self._weights()
-        P = dict(self.policy.net.named_parameters())
-        h = cfg.hidsize
-        # ---------------- heads ----------------
+        """Everything below the logits: the head weights (`_heads_bwd`), then `_backward_from_dlat`."""
+        dlat = self._heads_bwd(dlog, lat_bf16, tape)
+        del dlog
+        self._backward_from_dlat(dlat, tape, B, t, upper_grads_ready)
+
+    def _heads_bwd(self, dlog, lat_bf16, tape):
+        """The head weights' gradients from dlog bf16 [N][ld_logits] (one column block per `_head_layers()` entry) -> d latent bf16 [N][h]."""
         dWh = ops.wgrad(dlog, lat_bf16)
         dbh = ops.col_sums(dlog)[1]
         c0 = 0
         for lin in self._head_layers():
             m = lin.weight.shape[0]
-            _acc(lin.weight, dWh[c0:c0 + m])
-            _acc(lin.bias, dbh[c0:c0 + m])
+            self._grad(lin.weight, dWh[c0:c0 + m])
+            self._grad(lin.bias, dbh[c0:c0 + m])
             c0 += m
-        dlat = self._gemm(dlog, wts["heads_t"], h)
-        del dlog
+        return self._gemm(dlog, tape["wts"]["heads_t"], self.net.cfg.hidsize)
+
+    def _backward_from_dlat(self, dlat, tape, B, t, upper_grads_ready):
+        """Everything below the latent (the output of final_ln): final_ln [, lastlayer], the transformer, img_process.linear, dense, the
+        ImpalaCNN and, for the IDM, the conv3d pre-stage."""
+        net = self.net
+        cfg = net.cfg
+        wts = tape["wts"]
+        P = dict(net.named_parameters())
+        h = cfg.hidsize
         # ---------------- final_ln (plain norm) on lastlayer's output, or on relu(recurrent output) without lastlayer ----------------
         # (xl, z_last, x0, xd and the convs' h are ReLU outputs that feed a norm: their ReLU backward rides on that norm's apply pass)
         if self.use_lastlayer:
@@ -273,10 +306,19 @@ class _Trainer:
         if upper_grads_ready is not None:
             upper_grads_ready()
         # ---------------- ImpalaCNN, last stack to first ----------------
-        return self._cnn_bwd(dcnn, tape, wts, P)
+        dx3 = self._cnn_bwd(dcnn, tape, wts, P)
+        del dcnn
+        if cfg.conv3d_out is not None:
+            # the IDM's conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
+            C3 = cfg.conv3d_out
+            frames = tape["frames"]
+            dW3, db3 = ops.conv3d_t5_bwd(frames.view(B, t, *frames.shape[1:]), dx3, C3)
+            del dx3
+            self._grad(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
+            self._grad(net.conv3d_layer.layer.bias, db3)
 
     def _dense_bwd(self, dz, tape, wts, P):
-        cfg = self.policy.net.cfg
+        cfg = self.net.cfg
         Hf, Wf = cfg.final_hw
         C2 = cfg.chans[-1]
         N = dz.shape[0]
@@ -288,14 +330,14 @@ class _Trainer:
         dWz = self._wgrad_linear(dz, u)  # [out][Kd] in ZP column order
         del u
         unperm = lambda v: _dense_from_zp(v, cfg)
-        _acc(P[pfx + ".layer.weight"], unperm(dWz))
+        self._grad(P[pfx + ".layer.weight"], unperm(dWz))
         del dWz
         return self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, P[pfx + ".norm.weight"], P[pfx + ".norm.bias"],
                               grad_map=unperm, zp=(Hf, Wf, C2)).view(N, Hf + 1, Wf + 1, C2)
 
     def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t):
         """Backward of lib/util.py:193-211 (see policy.MinecraftPolicy._block for the forward in the same notation)."""
-        cfg = self.policy.net.cfg
+        cfg = self.net.cfg
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
         b = f"recurrent_layer.blocks.{l}"
         o = f"{b}.r.orc_block"
@@ -305,7 +347,7 @@ class _Trainer:
         # mlp1: z = y + hmid W1^T + b1
         dh = self._gemm(dz, W["mlp1_t"], h * cfg.pointwise_ratio)
         self._wgrad_linear(dz, S["hmid"], P[f"{b}.mlp1.layer.weight"])
-        _acc(P[f"{b}.mlp1.layer.bias"], ops.col_sums(dz)[1])
+        self._grad(P[f"{b}.mlp1.layer.bias"], ops.col_sums(dz)[1])
         # mlp0: hmid = relu(LN(y) W0^T)
         dzh = ops.relu_mask(dh, S["hmid"])
         del dh
@@ -314,7 +356,7 @@ class _Trainer:
         # proj: y = xhat + a Wp^T + bp
         da = self._gemm(dy, W["proj_t"], h)
         self._wgrad_linear(dy, S["a"], P[f"{o}.proj_layer.weight"])
-        _acc(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
+        self._grad(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
         # attention: gradients wrt q | k | v | R side by side (one buffer = one dgrad GEMM + one wgrad GEMM for all four)
         causal = cfg.mask_style == "clipped_causal"
         dqkvr = torch.zeros((N, self.kcat), dtype=BF16, device=dy.device)
@@ -324,20 +366,20 @@ class _Trainer:
         else:  # mask "none" (IDM): q | k | v only; R meets an empty band (b_nd is (10, 0)), so its parameters get exact zeros
             ops.attention_bwd(S["q"], S["full_k"], S["full_v"], None, None, None, None, da, dqkvr, B, t, 0, heads, causal=False)
             db_nd = torch.zeros_like(P[f"{o}.b_nd"], dtype=F32)
-        _acc(P[f"{o}.b_nd"], db_nd)
+        self._grad(P[f"{o}.b_nd"], db_nd)
         dxhat = self._gemm(dqkvr, W["qkvr_t"], h, residual=dy)
         dWc = self._wgrad_linear(dqkvr, S["xhat"])
         dbc = ops.col_sums(dqkvr)[1]
-        _acc(P[f"{o}.q_layer.weight"], dWc[0:h])
-        _acc(P[f"{o}.k_layer.weight"], dWc[h:2 * h])
-        _acc(P[f"{o}.v_layer.weight"], dWc[2 * h:3 * h])
-        _acc(P[f"{o}.q_layer.bias"], dbc[0:h])
+        self._grad(P[f"{o}.q_layer.weight"], dWc[0:h])
+        self._grad(P[f"{o}.k_layer.weight"], dWc[h:2 * h])
+        self._grad(P[f"{o}.v_layer.weight"], dWc[2 * h:3 * h])
+        self._grad(P[f"{o}.q_layer.bias"], dbc[0:h])
         if causal:
-            _acc(P[f"{o}.r_layer.weight"], dWc[3 * h:3 * h + nr])
-            _acc(P[f"{o}.r_layer.bias"], dbc[3 * h:3 * h + nr])
+            self._grad(P[f"{o}.r_layer.weight"], dWc[3 * h:3 * h + nr])
+            self._grad(P[f"{o}.r_layer.bias"], dbc[3 * h:3 * h + nr])
         else:
-            _acc(P[f"{o}.r_layer.weight"], torch.zeros_like(P[f"{o}.r_layer.weight"], dtype=F32))
-            _acc(P[f"{o}.r_layer.bias"], torch.zeros_like(P[f"{o}.r_layer.bias"], dtype=F32))
+            self._grad(P[f"{o}.r_layer.weight"], torch.zeros_like(P[f"{o}.r_layer.weight"], dtype=F32))
+            self._grad(P[f"{o}.r_layer.bias"], torch.zeros_like(P[f"{o}.r_layer.bias"], dtype=F32))
         # pre_r_ln (plain norm of the block input)
         g = P[f"{b}.pre_r_ln.weight"]
         return self._norm_bwd(dxhat, S["x"], S["mr_x"], g.detach().float().contiguous(), 1, h, g, P[f"{b}.pre_r_ln.bias"],
@@ -346,7 +388,7 @@ class _Trainer:
     def _cnn_bwd(self, dout, tape, wts, P):
         """Backward of lib/impala_cnn.py:187-195; `dout` is the gradient wrt the last stack's output (ZP).  Returns the gradient wrt the
         CNN input when stack 0's first conv is a normalised one (the IDM: the conv3d output, ReLU backward applied), else None."""
-        cfg = self.policy.net.cfg
+        cfg = self.net.cfg
         pfx = "img_process.cnn"
         dx = dout
         for i in reversed(range(len(cfg.chans))):
@@ -371,11 +413,11 @@ class _Trainer:
             dy1 = self._norm_bwd(dx.view(R, C), rec["y1"].view(R, C), rec["mr1"], g.detach().float().contiguous(), (H + 1) * (W + 1), H * W * C,
                                  g, P[f"{s}.n.bias"], zp=(H, W, C)).view(rec["y1"].shape)
             if i == 0 and not cfg.first_conv_norm:
-                st = self.policy.net.prepared().stacks[0]
+                st = tape["prep"].stacks[0]  # (the weights the forward used)
                 dWk, db = ops.firstconv_bwd(tape["frames"], st["fc_w"], st["fc_b"], dy1, C)
                 # kernel weights are W[c0][ky][kx][c] / 255 (lib/policy.py:44 folded in)
-                _acc(P[f"{s}.firstconv.layer.weight"], (dWk / 255.0).view(C, 3, 3, 3).permute(0, 3, 1, 2))
-                _acc(P[f"{s}.firstconv.layer.bias"], db)
+                self._grad(P[f"{s}.firstconv.layer.weight"], (dWk / 255.0).view(C, 3, 3, 3).permute(0, 3, 1, 2))
+                self._grad(P[f"{s}.firstconv.layer.bias"], db)
                 return None
             dfull = ops.maxpool3s2_bwd(dy1, rec["full"])  # includes the ReLU in front of the pool
             del dy1
@@ -565,13 +607,7 @@ class IDMTrainer(_Trainer):
             raise NotImplementedError(f"IDMTrainer: at most {self.max_t} frames per sequence (got T = {t})")
         lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
         loss, dlog = self._idm_dlog(pd, actions, N)
-        dx3 = self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
-        # the conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
-        C3 = net.cfg.conv3d_out
-        dW3, db3 = ops.conv3d_t5_bwd(img.contiguous(), dx3, C3)
-        del dx3
-        _acc(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
-        _acc(net.conv3d_layer.layer.bias, db3)
+        self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
         return loss, state_out
 
     def _idm_dlog(self, pd, actions, N):
@@ -588,3 +624,151 @@ class IDMTrainer(_Trainer):
             idx = actions[name].reshape(N, groups).to(torch.int64)
             logp = ops.softmax_nll_bwd_grouped(pd[name].reshape(N, groups, n), idx, scale, dlog, c0, lp=logp)
         return -logp.sum() / N, dlog
+
+
+# -- the differentiable forward (`set_autograd`) ------------------------------------------------------------------------------
+class _AutogradRunner(_Trainer):
+    """The shared taped forward and backward behind `loss.backward()`: `_PolicyBase.set_autograd(True)` (or `MinecraftPolicy.set_autograd`)
+    makes the forward an autograd `Function` whose backward turns the upstream gradients of its outputs into one gradient per parameter.
+
+        agent policy   outputs pd (one fp32 tensor per head) and vpred;  d pd -> `ops.log_softmax_bwd` -> dlog columns, d vpred -> the
+                       value head's column; then `_heads_bwd` and `_backward_from_dlat`
+        IDM policy     outputs pd
+        bare network   outputs the latent;  d latent -> `_backward_from_dlat`
+
+    Gradients go to a dict (`_Trainer._grad` with a sink) and are returned to autograd, which accumulates them into `.grad`.  A parameter
+    that only feeds outputs the loss does not touch gets None, as in the reference's autograd."""
+
+    def __init__(self, module):
+        from .policy import InverseActionNet, _PolicyBase
+
+        pol = module if isinstance(module, _PolicyBase) else None
+        super().__init__(pol, None if pol is not None else module)
+        self.use_lastlayer = not isinstance(self.net, InverseActionNet)  # the IDM's forward discards lastlayer's output
+        self.module = module
+
+    def _head_layers(self):
+        """The value head's output is one more column of the logits gradient, as in RLTrainer."""
+        pol = self.policy
+        if pol is None:
+            return []
+        return super()._head_layers() + ([pol.value_head.linear] if pol.has_value_head else [])
+
+    def check(self, img, state_in):
+        """The limits of one differentiable call, checked before any work."""
+        net = self.net
+        if net.precision != "bf16":
+            raise NotImplementedError("the differentiable forward runs in the bf16 mode only (set_precision('bf16'))")
+        B, t = img.shape[:2]
+        N = B * t
+        if net.cfg.conv3d_out is None:
+            if N > net.cnn_chunk_frames:
+                raise NotImplementedError(f"differentiable forward: at most {net.cnn_chunk_frames} frames per call (got B*T = {N}); "
+                                          "accumulate over calls")
+        else:
+            if N > net.idm_chunk_frames:
+                raise NotImplementedError(f"differentiable forward: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); "
+                                          "accumulate over calls")
+            if t > IDMTrainer.max_t:
+                raise NotImplementedError(f"differentiable forward: at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
+        for _, (k, v) in state_in:
+            if k.requires_grad or v.requires_grad:
+                raise ValueError("differentiable forward: state_in must not require grad -- gradients do not flow through the KV memory "
+                                 "across calls; detach the state (behavioural_cloning.py:109-111)")
+
+    def run(self, img, first, state_in, mask=None):
+        """-> (outputs, state_out): outputs attached to the graph (pd per head [+ vpred], or the latent), state_out detached."""
+        self.check(img, state_in)
+        params = [p for p in self.module.parameters()]
+        box = dict(img=img, first=first, state_in=state_in, mask=mask)
+        outs = _TapedForward.apply(self, box, *params)
+        return (outs,) if isinstance(outs, torch.Tensor) else outs, box["state_out"]
+
+    def forward_outputs(self, box):
+        """Runs the taped forward -> (output tensors, tape)."""
+        img = box["img"]
+        B, t = img.shape[:2]
+        if self.policy is None:
+            lat_bf16, lat_f32, tape, state_out = self._taped_latent(img, box["first"], box["state_in"])
+            outs = (lat_f32,)
+        else:
+            mask = box["mask"]
+            lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, box["first"], box["state_in"], mask)
+            outs = tuple(pd.values()) + ((vpred,) if vpred is not None else ())
+            masks = {}
+            for name, (shape, n) in self.policy.head_specs.items():
+                if mask is not None and mask.get(name) is not None:
+                    m = mask[name].to(device=img.device, dtype=torch.bool).expand(pd[name].shape)
+                    masks[name] = m.reshape(B * t, -1).contiguous()
+            tape["head_masks"] = masks
+        tape.update(lat=lat_bf16, B=B, t=t)
+        box["state_out"] = state_out
+        return outs, tape
+
+    def backward_grads(self, tape, outs, grads):
+        """The upstream gradients of the outputs -> {id(param): gradient} (parameters absent from it get None)."""
+        B, t = tape["B"], tape["t"]
+        N = B * t
+        sink = {}
+        self._sink = sink
+        try:
+            if self.policy is None:
+                dlat = grads[0].reshape(N, -1).to(BF16).contiguous()
+                self._backward_from_dlat(dlat, tape, B, t, None)
+                return sink
+            pol = self.policy
+            hp_cols = pol._heads_prepared()["cols"]
+            dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=tape["lat"].device)
+            unused = []
+            for i, (name, (shape, n)) in enumerate(pol.head_specs.items()):
+                lin = getattr(pol.pi_head, name).linear_layer
+                if grads[i] is None:
+                    unused.append(lin)
+                    continue
+                c0, width = hp_cols[name]
+                g = grads[i].reshape(N, width).to(F32).contiguous()
+                ops.log_softmax_bwd(outs[i].reshape(N, width), g, 1.0 / pol.temperature, dlog, c0, width // n, tape["head_masks"].get(name))
+            if pol.has_value_head:
+                gv = grads[len(pol.head_specs)]
+                if gv is None:
+                    unused.append(pol.value_head.linear)
+                else:
+                    dlog[:, self.ntot] = gv.reshape(N).to(BF16)  # d vpred: the value head's column (a strided copy of N values)
+            dlat = self._heads_bwd(dlog, tape["lat"], tape)
+            del dlog
+            self._backward_from_dlat(dlat, tape, B, t, None)
+            for lin in unused:
+                sink.pop(id(lin.weight), None)
+                sink.pop(id(lin.bias), None)
+            return sink
+        finally:
+            self._sink = None
+
+
+class _TapedForward(torch.autograd.Function):
+    """forward(runner, box, *params): the taped forward; the tape lives in ctx until the backward frees it.  The parameters are inputs
+    (saved, so that an in-place change before the backward raises torch's version-check error); the kernel-layout weights the forward
+    used are in the tape, so the backward never re-lays out newer parameters."""
+
+    @staticmethod
+    def forward(ctx, runner, box, *params):
+        ctx.set_materialize_grads(False)
+        outs, tape = runner.forward_outputs(box)
+        ctx.runner, ctx.tape, ctx.n_params = runner, tape, len(params)
+        ctx.save_for_backward(*params, *outs)
+        return outs if len(outs) > 1 else outs[0]
+
+    @staticmethod
+    def backward(ctx, *grads):
+        if torch.is_grad_enabled():
+            raise NotImplementedError("the differentiable forward has no double backward (create_graph=True)")
+        saved = ctx.saved_tensors  # (raises if a parameter or an output was modified in place since the forward)
+        if ctx.tape is None:
+            raise RuntimeError("the differentiable forward's tape was freed by an earlier backward: a graph can be back-propagated once")
+        tape, ctx.tape = ctx.tape, None
+        params, outs = saved[:ctx.n_params], saved[ctx.n_params:]
+        sink = ctx.runner.backward_grads(tape, outs, grads)
+        del tape
+        mods = list(ctx.runner.module.parameters())
+        res = [sink.get(id(p)) if ctx.needs_input_grad[2 + i] else None for i, p in enumerate(mods)]
+        return (None, None) + tuple(res)
