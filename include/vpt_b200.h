@@ -378,6 +378,17 @@ int vpt_firstconv_bwd_parts(int64_t F, int32_t H, int32_t W);
 int vpt_attention_bwd(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
                       int64_t first_stride, const uint8_t* smask, const void* dO, void* out, int64_t ld_out, float* db_nd, float* workspace,
                       int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream);
+/* vpt_attention_bwd with gradients through the KV memory (truncated BPTT across calls).  state_out = full[t : t+maxlen] of [memory|chunk].
+ * dstate_k / dstate_v fp32 [B][maxlen][h] (each nullable): the upstream gradient wrt this call's state_out K / V; row r is added in fp32
+ * to the d k / d v of chunk row r + t - maxlen before the bf16 rounding (nothing is added where it is null: the chunk columns are then
+ * bit-identical to vpt_attention_bwd).  dmem_k / dmem_v fp32 [B][maxlen][h] (null together, or both given): written in full with the
+ * gradient wrt state_in K / V: memory row j gets (1/128) sum_i dS[i][d] Q[i] and sum_i P[i][d] dO[i] over the queries i < min(j, t)
+ * (d = maxlen + i - j) where it is visible (state_mask[b][j] and not first[b][0]), plus state_out row j - t when j >= t.  All four
+ * 16-byte aligned.  Fixed-order sums, no atomics: bit-reproducible.  vpt_attention_bwd is this with four nulls. */
+int vpt_attention_bwd_state(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
+                            int64_t first_stride, const uint8_t* smask, const void* dO, void* out, int64_t ld_out, float* db_nd, float* workspace,
+                            int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis, const float* dstate_k, const float* dstate_v,
+                            float* dmem_k, float* dmem_v, void* stream);
 /* d loss / d logits of a categorical NLL head: out[r][col0 + j] = (exp(logp[r][j]) - [j == idx[r]]) * scale  (bf16)
  *                                                                                          lib/action_head.py:176-184 */
 int vpt_softmax_bwd(const float* logp, const int64_t* idx, float scale, void* out, int64_t ld_out, int32_t col0, int64_t rows, int32_t n,

@@ -136,6 +136,7 @@ SIGNATURES = {
     "vpt_firstconv_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _P]),
     "vpt_firstconv_bwd_parts": (_I, [_L, _I, _I]),
     "vpt_attention_bwd": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _L, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vpt_attention_bwd_state": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _L, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     "vpt_softmax_bwd": (_I, [_P, _P, _F, _P, _L, _I, _L, _I, _P]),
     # IDM backward (training.py, IDMTrainer)
     "vpt_conv3d_t5_bwd_workspace": (_L, [_L, _I, _I, _I]),

@@ -5,10 +5,13 @@
 //       recomputes the logits + softmax P, dP = dO V^T, dS = P * (dP - sum(P dP)); writes P and dS (indexed by the
 //       relative distance d) to a workspace, and dQ = dS K / D, dR = dS b_nd^T to the gradient buffer
 //   keys kernel  (16 chunk keys per CTA, one warp per key; Q / dO band staged in shared memory)
-//       dK = dS^T Q / D, dV = P^T dO        (chunk rows only: the KV memory is detached state)
+//       dK = dS^T Q / D, dV = P^T dO        (chunk rows; + the state_out gradient of the row, when given, before the bf16 rounding)
 //   b_nd kernel  (one CTA per distance d)  d b_nd[n][d] = sum_{b,head,i} R[b,i,head,n] * dS[b,head,i,d]
+//   memory kernel (16 memory rows per CTA, one warp per row; only when the state_in gradient is asked for)
+//       dmem_K = dS^T Q / D, dmem_V = P^T dO over the queries that see the row (+ the state_out gradient of the row when t < maxlen)
 //
 // Query i (chunk-local) sees the keys j = i+1 .. i+maxlen in [memory|chunk] coordinates, d = maxlen + i - j in [0, maxlen).
+// state_out = full[t : t + maxlen]: its row r is memory row t + r (r < maxlen - t) or chunk row r + t - maxlen.
 #pragma once
 #include "common.cuh"
 #include "backward.cuh"
@@ -173,6 +176,7 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_rows_kernel(
 
 __global__ void __launch_bounds__(kAbThreads) attn_bwd_keys_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __restrict__ dO,
                                                                     const float* __restrict__ wsP, const float* __restrict__ wsS,
+                                                                    const float* __restrict__ dsk, const float* __restrict__ dsv,
                                                                     __nv_bfloat16* __restrict__ out, long long ld_out, int t, int maxlen, int heads) {
     extern __shared__ __align__(16) uint8_t ab_smem[];
     const int nq = maxlen + kAbRows - 1;
@@ -209,14 +213,92 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_keys_kernel(const __nv_bf
         }
     }
     const float sc = 1.0f / (float)kAbD;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) dk[c] *= sc;
+    const int r = jc + maxlen - t;  // this key's row of state_out (when >= 0)
+    if (r >= 0) {  // no addend at all without a state gradient: the bits stay those of the plain backward
+        const long long so = ((long long)b * maxlen + r) * h + head * kAbD + lane * 4;
+        if (dsk != nullptr) {
+            const float4 g = __ldg(reinterpret_cast<const float4*>(dsk + so));
+            dk[0] += g.x; dk[1] += g.y; dk[2] += g.z; dk[3] += g.w;
+        }
+        if (dsv != nullptr) {
+            const float4 g = __ldg(reinterpret_cast<const float4*>(dsv + so));
+            dv[0] += g.x; dv[1] += g.y; dv[2] += g.z; dv[3] += g.w;
+        }
+    }
     const long long row = (long long)b * t + jc;
     uint2 o2;
-    o2.x = pack_bf16(dk[0] * sc, dk[1] * sc);
-    o2.y = pack_bf16(dk[2] * sc, dk[3] * sc);
+    o2.x = pack_bf16(dk[0], dk[1]);
+    o2.y = pack_bf16(dk[2], dk[3]);
     *reinterpret_cast<uint2*>(out + row * ld_out + h + head * kAbD + lane * 4) = o2;
     o2.x = pack_bf16(dv[0], dv[1]);
     o2.y = pack_bf16(dv[2], dv[3]);
     *reinterpret_cast<uint2*>(out + row * ld_out + 2 * h + head * kAbD + lane * 4) = o2;
+}
+
+// Memory row j < maxlen is seen by the queries i in [0, min(j, t)) at d = maxlen + i - j, where the row is visible (state_mask[b, j] and
+// not first[b, 0]); the P / dS the rows kernel wrote for those (i, d) are all this needs.  Writes dmem_k / dmem_v fp32 [B][maxlen][h] in
+// full (+ the state_out gradient of the row when j >= t).  Fixed-order sums over i, no atomics.
+__global__ void __launch_bounds__(kAbThreads) attn_bwd_mem_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __restrict__ dO,
+                                                                   const float* __restrict__ wsP, const float* __restrict__ wsS,
+                                                                   const uint8_t* __restrict__ first, long long first_stride,
+                                                                   const uint8_t* __restrict__ smask, const float* __restrict__ dsk,
+                                                                   const float* __restrict__ dsv, float* __restrict__ dmem_k,
+                                                                   float* __restrict__ dmem_v, int t, int maxlen, int heads) {
+    extern __shared__ __align__(16) uint8_t ab_smem[];
+    const int j0 = blockIdx.x * kAbRows, head = blockIdx.y, b = blockIdx.z;
+    const int h = heads * kAbD;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const bool mem_ok = (first[(long long)b * first_stride] == 0) && (smask != nullptr);
+    const int nq = mem_ok ? min(t, min(j0 + kAbRows, maxlen) - 1) : 0;  // queries any row of this CTA is seen by: i < j < min(j0 + 16, maxlen)
+    __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(ab_smem);
+    __nv_bfloat16* Os = Qs + (size_t)max(nq, 1) * kAbPitch;
+    stage_rows(Qs, Q + (long long)b * t * h, h, 0, nq, t, head * kAbD);
+    stage_rows(Os, dO + (long long)b * t * h, h, 0, nq, t, head * kAbD);
+    __syncthreads();
+    const int j = j0 + warp;
+    if (j >= maxlen) return;
+    const long long bh = (long long)b * heads + head;
+    float dk[4] = {0.f, 0.f, 0.f, 0.f}, dv[4] = {0.f, 0.f, 0.f, 0.f};
+    const int ni = (mem_ok && smask[(long long)b * maxlen + j] != 0) ? min(j, t) : 0;
+    for (int i0 = 0; i0 < ni; i0 += 32) {
+        const int il = i0 + lane;
+        float p = 0.f, ds = 0.f;
+        if (il < ni) {
+            const long long w = (bh * t + il) * maxlen + (maxlen + il - j);
+            p = __ldg(wsP + w);
+            ds = __ldg(wsS + w);
+        }
+        const int n = min(32, ni - i0);
+        for (int ii = 0; ii < n; ++ii) {
+            const float pp = __shfl_sync(0xffffffffu, p, ii), ss = __shfl_sync(0xffffffffu, ds, ii);
+            const int r = i0 + ii;  // staged row of query i
+            const uint2 qv = *reinterpret_cast<const uint2*>(Qs + (size_t)r * kAbPitch + lane * 4);
+            const uint2 ov = *reinterpret_cast<const uint2*>(Os + (size_t)r * kAbPitch + lane * 4);
+            dk[0] = fmaf(ss, bf16_lo(qv.x), dk[0]); dk[1] = fmaf(ss, bf16_hi(qv.x), dk[1]);
+            dk[2] = fmaf(ss, bf16_lo(qv.y), dk[2]); dk[3] = fmaf(ss, bf16_hi(qv.y), dk[3]);
+            dv[0] = fmaf(pp, bf16_lo(ov.x), dv[0]); dv[1] = fmaf(pp, bf16_hi(ov.x), dv[1]);
+            dv[2] = fmaf(pp, bf16_lo(ov.y), dv[2]); dv[3] = fmaf(pp, bf16_hi(ov.y), dv[3]);
+        }
+    }
+    const float sc = 1.0f / (float)kAbD;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) dk[c] *= sc;
+    if (j >= t) {  // memory row j is row j - t of state_out (t < maxlen)
+        const long long so = ((long long)b * maxlen + (j - t)) * h + head * kAbD + lane * 4;
+        if (dsk != nullptr) {
+            const float4 g = __ldg(reinterpret_cast<const float4*>(dsk + so));
+            dk[0] += g.x; dk[1] += g.y; dk[2] += g.z; dk[3] += g.w;
+        }
+        if (dsv != nullptr) {
+            const float4 g = __ldg(reinterpret_cast<const float4*>(dsv + so));
+            dv[0] += g.x; dv[1] += g.y; dv[2] += g.z; dv[3] += g.w;
+        }
+    }
+    const long long o = ((long long)b * maxlen + j) * h + head * kAbD + lane * 4;
+    *reinterpret_cast<float4*>(dmem_k + o) = make_float4(dk[0], dk[1], dk[2], dk[3]);
+    *reinterpret_cast<float4*>(dmem_v + o) = make_float4(dv[0], dv[1], dv[2], dv[3]);
 }
 
 // one CTA per distance d: db_nd[n][d] = sum over (b, head, i) of R[b,i,head,n] * dS[b,head,i,d]; fixed-order reduction
@@ -254,24 +336,30 @@ __global__ void __launch_bounds__(256) attn_bwd_bnd_kernel(const float* __restri
 
 }  // namespace vpt
 
-extern "C" int vpt_attention_bwd(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
-                                 int64_t first_stride, const uint8_t* smask, const void* dO, void* out, int64_t ld_out, float* db_nd, float* workspace,
-                                 int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
+extern "C" int vpt_attention_bwd_state(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
+                                       const uint8_t* first, int64_t first_stride, const uint8_t* smask, const void* dO, void* out, int64_t ld_out,
+                                       float* db_nd, float* workspace, int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis,
+                                       const float* dstate_k, const float* dstate_v, float* dmem_k, float* dmem_v, void* stream) {
     using namespace vpt;
     VPT_CHECK(Q && Kf && Vf && R && b_nd && first && dO && out && db_nd && workspace, "vpt_attention_bwd: null argument");
     VPT_CHECK(B > 0 && B <= 65535 && t > 0 && heads > 0 && maxlen > 0 && maxlen <= 32 * kAbMaxPerLane && nbasis > 0 && nbasis <= 10,
               "vpt_attention_bwd: unsupported shape (B=%d t=%d maxlen=%d heads=%d nbasis=%d)", B, t, maxlen, heads, nbasis);
     VPT_CHECK(ld_out % 4 == 0 && ld_out >= 3 * (int64_t)heads * kAbD + heads * nbasis, "vpt_attention_bwd: gradient buffer too narrow");
+    VPT_CHECK((dmem_k == nullptr) == (dmem_v == nullptr), "vpt_attention_bwd_state: dmem_k and dmem_v are given together or not at all");
+    for (const float* p : {dstate_k, dstate_v, (const float*)dmem_k, (const float*)dmem_v})
+        VPT_CHECK(reinterpret_cast<uintptr_t>(p) % 16 == 0, "vpt_attention_bwd_state: state gradients must be 16-byte aligned");
     const size_t ws_half = (size_t)B * heads * t * maxlen;
     float* wsP = workspace;
     float* wsS = workspace + ws_half;
     const int nk = maxlen + kAbRows - 1;
     const size_t smem_rows = (size_t)(2 * nk + 2 * kAbRows) * kAbPitch * 2 + ((size_t)nbasis * maxlen + (size_t)kAbRows * maxlen) * 4 + maxlen + 16;
     const size_t smem_keys = (size_t)(2 * nk) * kAbPitch * 2;
+    const size_t smem_mem = (size_t)(2 * max(min(t, maxlen - 1), 1)) * kAbPitch * 2;
     static bool attr_set = false;
     if (!attr_set) {
         VPT_CUDA(cudaFuncSetAttribute(attn_bwd_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         VPT_CUDA(cudaFuncSetAttribute(attn_bwd_keys_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VPT_CUDA(cudaFuncSetAttribute(attn_bwd_mem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr_set = true;
     }
     dim3 grid((t + kAbRows - 1) / kAbRows, heads, B);
@@ -281,10 +369,25 @@ extern "C" int vpt_attention_bwd(const void* Q, const void* Kf, const void* Vf, 
         heads, nbasis);
     VPT_LAUNCH_CHECK();
     attn_bwd_keys_kernel<<<grid, kAbThreads, smem_keys, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(Q),
-                                                                               reinterpret_cast<const __nv_bfloat16*>(dO), wsP, wsS,
-                                                                               reinterpret_cast<__nv_bfloat16*>(out), ld_out, t, maxlen, heads);
+                                                                               reinterpret_cast<const __nv_bfloat16*>(dO), wsP, wsS, dstate_k,
+                                                                               dstate_v, reinterpret_cast<__nv_bfloat16*>(out), ld_out, t, maxlen,
+                                                                               heads);
     VPT_LAUNCH_CHECK();
     attn_bwd_bnd_kernel<<<maxlen, 256, 0, (cudaStream_t)stream>>>(R, ld_r, wsS, db_nd, B, t, maxlen, heads, nbasis);
     VPT_LAUNCH_CHECK();
+    if (dmem_k != nullptr) {
+        dim3 mgrid((maxlen + kAbRows - 1) / kAbRows, heads, B);
+        attn_bwd_mem_kernel<<<mgrid, kAbThreads, smem_mem, (cudaStream_t)stream>>>(
+            reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(dO), wsP, wsS, first, first_stride, smask, dstate_k,
+            dstate_v, dmem_k, dmem_v, t, maxlen, heads);
+        VPT_LAUNCH_CHECK();
+    }
     return VPT_OK;
+}
+
+extern "C" int vpt_attention_bwd(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
+                                 int64_t first_stride, const uint8_t* smask, const void* dO, void* out, int64_t ld_out, float* db_nd, float* workspace,
+                                 int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
+    return vpt_attention_bwd_state(Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, dO, out, ld_out, db_nd, workspace, B, t, maxlen, heads,
+                                   nbasis, nullptr, nullptr, nullptr, nullptr, stream);
 }

@@ -534,6 +534,7 @@ def softmax_bwd(logp, idx, scale, out, col0):
 from .ops_idm import conv3d_t5_bwd, softmax_nll_bwd_grouped  # noqa: E402,F401  (IDM backward ops, csrc/idm_bwd.cuh)
 from .ops_rl import ewma_sums, ppo_coef, rl_head_bwd, value_bwd  # noqa: E402,F401  (RL fine-tuning ops, csrc/rl_bwd.cuh)
 from .ops_autograd import log_softmax_bwd  # noqa: E402,F401  (differentiable forward, csrc/log_softmax_bwd.cuh)
+from .ops_bptt import attention_bwd_state  # noqa: E402,F401  (gradients through the KV memory, csrc/attention_bwd.cuh)
 
 
 # ---- on-device action codec (csrc/codec.cuh) -----------------------------------------------------------------------------

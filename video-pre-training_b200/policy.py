@@ -386,15 +386,17 @@ class MinecraftPolicy(nn.Module):
         self.debug_taps = None  # set to a dict to capture intermediate activations (tests)
         self._tape = None       # set to a dict by training.BCTrainer: the forward then records what the backward needs
         self._autograd = False  # set_autograd
+        self._state_grad = False
         self._ag_runner = None
 
     def output_latent_size(self):
         return self.hidsize
 
-    def set_autograd(self, on: bool = True):
+    def set_autograd(self, on: bool = True, state_grad: bool = False):
         """Opt in to the differentiable forward: in grad mode, with a parameter that requires grad, `forward` returns a latent attached
-        to the autograd graph (see `_PolicyBase.set_autograd`)."""
+        to the autograd graph; `state_grad` also attaches the state's K / V (see `_PolicyBase.set_autograd`)."""
         self._autograd = bool(on)
+        self._state_grad = bool(on) and bool(state_grad)
         return self
 
     def initial_state(self, batchsize):
@@ -690,21 +692,28 @@ class _PolicyBase(nn.Module):
         self._hprep = None
         self._hprep_fp = None
         self._autograd = False  # set_autograd
+        self._state_grad = False
         self._ag_runner = None
 
     def initial_state(self, batch_size: int):
         return self.net.initial_state(batch_size)
 
-    def set_autograd(self, on: bool = True):
+    def set_autograd(self, on: bool = True, state_grad: bool = False):
         """Opt in to the differentiable forward (also for `self.net` called on its own).  When on, a forward in grad mode (not inference
         mode) with at least one parameter that requires grad runs the training forward (no stack-norm fold; within the 1e-2 tolerance of
         the inference path, not bit-identical to it) as an autograd `Function` whose backward is the trainers' hand-written one, so that
         `loss.backward()` accumulates into `.grad`.  pd and vpred are attached to the graph; `state_out` is detached and a `state_in`
         that requires grad raises (no gradient through the KV memory, behavioural_cloning.py:109-111).  At most `net.cnn_chunk_frames`
         (2048) frames per call (the IDM: `net.idm_chunk_frames` (512) and T <= 128), bf16 mode only.  A parameter that only feeds outputs
-        the loss does not use gets None, as in the reference.  `act`, `predict`, `v` and `GraphedAct` stay inference-only."""
+        the loss does not use gets None, as in the reference.  `act`, `predict`, `v` and `GraphedAct` stay inference-only.
+
+        state_grad=True (truncated backpropagation through time across calls): `state_out`'s K / V are attached to the graph too and a
+        `state_in` whose K / V require grad is accepted, so a loss on a later call trains this one through the KV memory.  Truncate with
+        `state = tree_map(detach)` every k calls and call `backward()` once per window: every call of the window keeps its tape (its
+        activations) until then.  Each call keeps its own limits.  No effect on a model without memory (the IDM)."""
         self._autograd = bool(on)
-        self.net.set_autograd(on)
+        self._state_grad = bool(on) and bool(state_grad)
+        self.net.set_autograd(on, state_grad=state_grad)
         return self
 
     def set_precision(self, precision: str):

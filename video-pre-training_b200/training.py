@@ -27,7 +27,9 @@ What each layer type needs (u = gamma * n + beta is the normalised layer input, 
     max-pool, first conv, attention, softmax heads: their own backward kernels (see include/vpt_b200.h).
 
 The KV memory carried in `state_in` is detached exactly like behavioural_cloning.py:111 (`tree_map(lambda x: x.detach())`),
-and `value_head.*` receives no gradient from the BC loss (None in the reference: the BC loss never touches it).
+and `value_head.*` receives no gradient from the BC loss (None in the reference: the BC loss never touches it).  Only the differentiable
+forward with `state_grad` (`set_autograd(True, state_grad=True)`) carries gradients through it: `_backward_from_dlat` then takes the
+gradient wrt each layer's state_out K / V and returns the one wrt its state_in K / V (`ops.attention_bwd_state`).
 """
 import torch
 import torch.distributed as dist
@@ -279,9 +281,10 @@ class _Trainer:
             c0 += m
         return self._gemm(dlog, tape["wts"]["heads_t"], self.net.cfg.hidsize)
 
-    def _backward_from_dlat(self, dlat, tape, B, t, upper_grads_ready):
+    def _backward_from_dlat(self, dlat, tape, B, t, upper_grads_ready, dstate=None, want_dmem=None):
         """Everything below the latent (the output of final_ln): final_ln [, lastlayer], the transformer, img_process.linear, dense, the
-        ImpalaCNN and, for the IDM, the conv3d pre-stage."""
+        ImpalaCNN and, for the IDM, the conv3d pre-stage.  dstate: None or per layer None / (dk, dv), the gradient wrt that layer's
+        state_out K / V; want_dmem: None or per layer whether its state_in gradient is wanted.  Returns per layer (dmem_k, dmem_v) or None."""
         net = self.net
         cfg = net.cfg
         wts = tape["wts"]
@@ -298,8 +301,10 @@ class _Trainer:
         if self.use_lastlayer:
             dx = self._normlinear_bwd(dx, tape["z_last"], tape["mr_zl"], wts["last_t"], "lastlayer", P, relu_x=True)
         # ---------------- transformer blocks, last to first ----------------
+        dmem = [None] * cfg.n_layers
         for l in reversed(range(cfg.n_layers)):
-            dx = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t)
+            dx, dmem[l] = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t,
+                                          dstate=None if dstate is None else dstate[l], want_dmem=bool(want_dmem and want_dmem[l]))
         # ---------------- img_process.linear, dense ----------------
         dz = self._normlinear_bwd(dx, tape["xd"], tape["mr_d"], wts["linear_t"], "img_process.linear", P, relu_x=True)
         dcnn = self._dense_bwd(dz, tape, wts, P)
@@ -316,6 +321,7 @@ class _Trainer:
             del dx3
             self._grad(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
             self._grad(net.conv3d_layer.layer.bias, db3)
+        return dmem
 
     def _dense_bwd(self, dz, tape, wts, P):
         cfg = self.net.cfg
@@ -335,8 +341,10 @@ class _Trainer:
         return self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, P[pfx + ".norm.weight"], P[pfx + ".norm.bias"],
                               grad_map=unperm, zp=(Hf, Wf, C2)).view(N, Hf + 1, Wf + 1, C2)
 
-    def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t):
-        """Backward of lib/util.py:193-211 (see policy.MinecraftPolicy._block for the forward in the same notation)."""
+    def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t, dstate=None, want_dmem=False):
+        """Backward of lib/util.py:193-211 (see policy.MinecraftPolicy._block for the forward in the same notation) -> (d block input,
+        (dmem_k, dmem_v) or None).  dstate: None or (dk, dv), the gradient wrt the layer's state_out K / V (either None); want_dmem: return
+        the gradient wrt its state_in K / V (lib/xf.py:366-391 builds the memory with cat and slicing, so autograd reaches it)."""
         cfg = self.net.cfg
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
         b = f"recurrent_layer.blocks.{l}"
@@ -360,7 +368,11 @@ class _Trainer:
         # attention: gradients wrt q | k | v | R side by side (one buffer = one dgrad GEMM + one wgrad GEMM for all four)
         causal = cfg.mask_style == "clipped_causal"
         dqkvr = torch.zeros((N, self.kcat), dtype=BF16, device=dy.device)
-        if causal:
+        dmem = None
+        if causal and (dstate is not None or want_dmem):  # the KV memory is in the graph (the differentiable forward's state_grad)
+            db_nd, dmem = ops.attention_bwd_state(S["q"], S["full_k"], S["full_v"], S["R"], P[f"{o}.b_nd"].detach().float().contiguous(), first_u8,
+                                                  S["smask"], da, dqkvr, B, t, maxlen, heads, dstate=dstate, want_dmem=want_dmem)
+        elif causal:
             db_nd = ops.attention_bwd(S["q"], S["full_k"], S["full_v"], S["R"], P[f"{o}.b_nd"].detach().float().contiguous(), first_u8, S["smask"],
                                       da, dqkvr, B, t, maxlen, heads)
         else:  # mask "none" (IDM): q | k | v only; R meets an empty band (b_nd is (10, 0)), so its parameters get exact zeros
@@ -382,8 +394,9 @@ class _Trainer:
             self._grad(P[f"{o}.r_layer.bias"], torch.zeros_like(P[f"{o}.r_layer.bias"], dtype=F32))
         # pre_r_ln (plain norm of the block input)
         g = P[f"{b}.pre_r_ln.weight"]
-        return self._norm_bwd(dxhat, S["x"], S["mr_x"], g.detach().float().contiguous(), 1, h, g, P[f"{b}.pre_r_ln.bias"],
-                              relu_x=(l == 0))  # block 0's input is relu(img_process.linear)
+        dx = self._norm_bwd(dxhat, S["x"], S["mr_x"], g.detach().float().contiguous(), 1, h, g, P[f"{b}.pre_r_ln.bias"],
+                            relu_x=(l == 0))  # block 0's input is relu(img_process.linear)
+        return dx, dmem
 
     def _cnn_bwd(self, dout, tape, wts, P):
         """Backward of lib/impala_cnn.py:187-195; `dout` is the gradient wrt the last stack's output (ZP).  Returns the gradient wrt the
@@ -637,7 +650,13 @@ class _AutogradRunner(_Trainer):
         bare network   outputs the latent;  d latent -> `_backward_from_dlat`
 
     Gradients go to a dict (`_Trainer._grad` with a sink) and are returned to autograd, which accumulates them into `.grad`.  A parameter
-    that only feeds outputs the loss does not touch gets None, as in the reference's autograd."""
+    that only feeds outputs the loss does not touch gets None, as in the reference's autograd.
+
+    With `state_grad` (`set_autograd(True, state_grad=True)`, models with a KV memory) the state_in K / V of every layer are inputs of the
+    `Function` too and the state_out K / V extra outputs, so a loss on a later call reaches this one through the memory (truncated BPTT:
+    the caller detaches the state every k calls).  The backward then also takes d state_out and returns d state_in
+    (`ops.attention_bwd_state`); a call whose own outputs get no gradient but whose state_out does runs the same backward from a zero d
+    latent."""
 
     def __init__(self, module):
         from .policy import InverseActionNet, _PolicyBase
@@ -653,6 +672,11 @@ class _AutogradRunner(_Trainer):
         if pol is None:
             return []
         return super()._head_layers() + ([pol.value_head.linear] if pol.has_value_head else [])
+
+    def state_grad(self):
+        """Whether this module's differentiable forward carries gradients through the KV memory (`set_autograd(.., state_grad=True)`;
+        nothing changes for a model without memory, maxlen = 0: the IDM)."""
+        return bool(getattr(self.module, "_state_grad", False)) and self.net.cfg.maxlen > 0
 
     def check(self, img, state_in):
         """The limits of one differentiable call, checked before any work."""
@@ -671,18 +695,29 @@ class _AutogradRunner(_Trainer):
                                           "accumulate over calls")
             if t > IDMTrainer.max_t:
                 raise NotImplementedError(f"differentiable forward: at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
+        if self.state_grad():
+            return
         for _, (k, v) in state_in:
             if k.requires_grad or v.requires_grad:
                 raise ValueError("differentiable forward: state_in must not require grad -- gradients do not flow through the KV memory "
-                                 "across calls; detach the state (behavioural_cloning.py:109-111)")
+                                 "across calls; detach the state (behavioural_cloning.py:109-111) or opt in with "
+                                 "set_autograd(True, state_grad=True)")
 
     def run(self, img, first, state_in, mask=None):
-        """-> (outputs, state_out): outputs attached to the graph (pd per head [+ vpred], or the latent), state_out detached."""
+        """-> (outputs, state_out): outputs attached to the graph (pd per head [+ vpred], or the latent); state_out detached, or with
+        `state_grad` its K / V attached (state_mask is a plain bool tensor either way)."""
         self.check(img, state_in)
         params = [p for p in self.module.parameters()]
-        box = dict(img=img, first=first, state_in=state_in, mask=mask)
-        outs = _TapedForward.apply(self, box, *params)
-        return (outs,) if isinstance(outs, torch.Tensor) else outs, box["state_out"]
+        sg = self.state_grad()
+        kv = [x for _, (k, v) in state_in for x in (k, v)] if sg else []
+        box = dict(img=img, first=first, state_in=state_in, mask=mask, state_grad=sg)
+        outs = _TapedForward.apply(self, box, *params, *kv)
+        outs = (outs,) if isinstance(outs, torch.Tensor) else outs
+        if not sg:
+            return outs, box["state_out"]
+        n = len(outs) - len(kv)
+        kvo = outs[n:]
+        return outs[:n], [(m, (kvo[2 * l], kvo[2 * l + 1])) for l, (m, _) in enumerate(box["state_out"])]
 
     def forward_outputs(self, box):
         """Runs the taped forward -> (output tensors, tape)."""
@@ -705,18 +740,25 @@ class _AutogradRunner(_Trainer):
         box["state_out"] = state_out
         return outs, tape
 
-    def backward_grads(self, tape, outs, grads):
-        """The upstream gradients of the outputs -> {id(param): gradient} (parameters absent from it get None)."""
+    def backward_grads(self, tape, outs, grads, dstate=None, want_dmem=None):
+        """The upstream gradients of the outputs -> ({id(param): gradient} (parameters absent from it get None), per layer d state_in
+        (dmem_k, dmem_v) or None).  dstate / want_dmem as in `_backward_from_dlat` (the `state_grad` case)."""
         B, t = tape["B"], tape["t"]
         N = B * t
         sink = {}
         self._sink = sink
+        h = self.net.cfg.hidsize
         try:
             if self.policy is None:
-                dlat = grads[0].reshape(N, -1).to(BF16).contiguous()
-                self._backward_from_dlat(dlat, tape, B, t, None)
-                return sink
+                if grads[0] is None:  # only the state_out feeds the loss
+                    dlat = torch.zeros((N, h), dtype=BF16, device=tape["lat"].device)
+                else:
+                    dlat = grads[0].reshape(N, -1).to(BF16).contiguous()
+                return sink, self._backward_from_dlat(dlat, tape, B, t, None, dstate, want_dmem)
             pol = self.policy
+            if all(g is None for g in grads):  # only the state_out feeds the loss: no head gradient, a zero d latent
+                return sink, self._backward_from_dlat(torch.zeros((N, h), dtype=BF16, device=tape["lat"].device), tape, B, t, None, dstate,
+                                                      want_dmem)
             hp_cols = pol._heads_prepared()["cols"]
             dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=tape["lat"].device)
             unused = []
@@ -736,39 +778,61 @@ class _AutogradRunner(_Trainer):
                     dlog[:, self.ntot] = gv.reshape(N).to(BF16)  # d vpred: the value head's column (a strided copy of N values)
             dlat = self._heads_bwd(dlog, tape["lat"], tape)
             del dlog
-            self._backward_from_dlat(dlat, tape, B, t, None)
+            dmem = self._backward_from_dlat(dlat, tape, B, t, None, dstate, want_dmem)
             for lin in unused:
                 sink.pop(id(lin.weight), None)
                 sink.pop(id(lin.bias), None)
-            return sink
+            return sink, dmem
         finally:
             self._sink = None
 
 
+def _aligned_f32(x):
+    """x as a contiguous, 16-byte aligned fp32 tensor (the layout the state-gradient kernel reads)."""
+    x = x.to(F32).contiguous()
+    return x if x.data_ptr() % 16 == 0 else x.clone()
+
+
 class _TapedForward(torch.autograd.Function):
-    """forward(runner, box, *params): the taped forward; the tape lives in ctx until the backward frees it.  The parameters are inputs
-    (saved, so that an in-place change before the backward raises torch's version-check error); the kernel-layout weights the forward
-    used are in the tape, so the backward never re-lays out newer parameters."""
+    """forward(runner, box, *params[, *state K / V]): the taped forward; the tape lives in ctx until the backward frees it.  The parameters
+    are inputs (saved, so that an in-place change before the backward raises torch's version-check error); the kernel-layout weights the
+    forward used are in the tape, so the backward never re-lays out newer parameters.  With `box["state_grad"]` the state_in K / V of
+    every layer follow the parameters as inputs, and the state_out K / V follow the outputs."""
 
     @staticmethod
-    def forward(ctx, runner, box, *params):
+    def forward(ctx, runner, box, *inputs):
         ctx.set_materialize_grads(False)
         outs, tape = runner.forward_outputs(box)
-        ctx.runner, ctx.tape, ctx.n_params = runner, tape, len(params)
-        ctx.save_for_backward(*params, *outs)
+        n_params = len(inputs) - (2 * len(box["state_in"]) if box["state_grad"] else 0)
+        ctx.runner, ctx.tape, ctx.n_params, ctx.n_outs = runner, tape, n_params, len(outs)
+        ctx.save_for_backward(*inputs[:n_params], *outs)
+        if box["state_grad"]:
+            outs = outs + tuple(x for _, (k, v) in box["state_out"] for x in (k, v))
         return outs if len(outs) > 1 else outs[0]
 
     @staticmethod
     def backward(ctx, *grads):
         if torch.is_grad_enabled():
             raise NotImplementedError("the differentiable forward has no double backward (create_graph=True)")
+        if ctx.tape is None:  # (checked first: torch has freed the saved tensors too)
+            raise RuntimeError("the differentiable forward's tape was freed by an earlier backward: a graph can be back-propagated once "
+                               "(with state_grad, detach the state or call backward once per window)")
         saved = ctx.saved_tensors  # (raises if a parameter or an output was modified in place since the forward)
-        if ctx.tape is None:
-            raise RuntimeError("the differentiable forward's tape was freed by an earlier backward: a graph can be back-propagated once")
         tape, ctx.tape = ctx.tape, None
         params, outs = saved[:ctx.n_params], saved[ctx.n_params:]
-        sink = ctx.runner.backward_grads(tape, outs, grads)
+        dstate = want_dmem = None
+        if len(grads) > ctx.n_outs:  # state_grad: per layer d state_out K / V, and whether d state_in K / V is wanted
+            gs, need = grads[ctx.n_outs:], ctx.needs_input_grad[2 + ctx.n_params:]
+            L = len(gs) // 2
+            dstate = [None if gs[2 * l] is None and gs[2 * l + 1] is None else (gs[2 * l], gs[2 * l + 1]) for l in range(L)]
+            dstate = [None if d is None else tuple(None if x is None else _aligned_f32(x) for x in d) for d in dstate]
+            want_dmem = [need[2 * l] or need[2 * l + 1] for l in range(L)]
+        sink, dmem = ctx.runner.backward_grads(tape, outs, grads[:ctx.n_outs], dstate, want_dmem)
         del tape
         mods = list(ctx.runner.module.parameters())
         res = [sink.get(id(p)) if ctx.needs_input_grad[2 + i] else None for i, p in enumerate(mods)]
+        if want_dmem is not None:
+            need = ctx.needs_input_grad[2 + ctx.n_params:]
+            for l, d in enumerate(dmem):
+                res += [d[0] if d is not None and need[2 * l] else None, d[1] if d is not None and need[2 * l + 1] else None]
         return (None, None) + tuple(res)
