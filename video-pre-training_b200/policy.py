@@ -352,6 +352,13 @@ def _differentiable(module: nn.Module) -> bool:
         any(p.requires_grad for p in module.parameters())
 
 
+def check_recompute_frames(v):
+    """`recompute_frames` of the trainers and `set_autograd`: None (keep the CNN's activations for the backward) or a positive int."""
+    if v is not None and (isinstance(v, bool) or not isinstance(v, int) or v <= 0):
+        raise ValueError(f"recompute_frames must be None or a positive int (got {v!r})")
+    return v
+
+
 def _autograd_runner(module: nn.Module):
     """The module's differentiable-forward machinery (training._AutogradRunner), made on first use.  Tests read the tape of the last
     differentiable call from it (`keep_tape` / `last_tape`, as with the trainers)."""
@@ -387,16 +394,20 @@ class MinecraftPolicy(nn.Module):
         self._tape = None       # set to a dict by training.BCTrainer: the forward then records what the backward needs
         self._autograd = False  # set_autograd
         self._state_grad = False
+        self._recompute_frames = None
         self._ag_runner = None
 
     def output_latent_size(self):
         return self.hidsize
 
-    def set_autograd(self, on: bool = True, state_grad: bool = False):
+    def set_autograd(self, on: bool = True, state_grad: bool = False, recompute_frames: Optional[int] = None):
         """Opt in to the differentiable forward: in grad mode, with a parameter that requires grad, `forward` returns a latent attached
-        to the autograd graph; `state_grad` also attaches the state's K / V (see `_PolicyBase.set_autograd`)."""
+        to the autograd graph; `state_grad` also attaches the state's K / V, `recompute_frames` re-runs the CNN in the backward instead of
+        keeping its activations (see `_PolicyBase.set_autograd`)."""
+        recompute_frames = check_recompute_frames(recompute_frames)
         self._autograd = bool(on)
         self._state_grad = bool(on) and bool(state_grad)
+        self._recompute_frames = recompute_frames if on else None
         return self
 
     def initial_state(self, batchsize):
@@ -430,20 +441,23 @@ class MinecraftPolicy(nn.Module):
     # -- CNN -----------------------------------------------------------------------------------------------
     # Activations are kept in the "ZP" layout [F][H+1][W+1][C] (zero last row / column; include/vpt_b200.h): it lets the
     # conv kernel address every 3x3 neighbour linearly and reuse one shared-memory input span for all nine taps.
-    def _cnn_chunk(self, img, prep: _Prepared, out, pfx="img_process.cnn"):
+    def _cnn_chunk(self, img, prep: _Prepared, out, pfx="img_process.cnn", train=False, stacks=None):
         """lib/impala_cnn.py:187-195 for a chunk of frames; writes the last stack's output (ZP [F, Hf+1, Wf+1, C2] bf16) into
-        `out` and returns (out, per-frame stats)."""
+        `out` and returns (out, per-frame stats).
+        train: the training layout (no stack-norm fold; each residual branch's output `r` kept apart, then `add_zp`), which the
+        backward's recompute of a chunk reproduces bit for bit.  stacks: a list that receives, per stack, what the backward needs
+        (training layout only; None records nothing)."""
         cfg = self.cfg
         H, W = cfg.img_shape[0], cfg.img_shape[1]
         x, mr = None, None
-        tape = self._tape
+        assert train or stacks is None
         if prep.conv3d is not None:  # IDM: img is (b, T, H, W, 3), whole sequences (the temporal conv needs its neighbours)
             x, mr = ops.conv3d_t5(img, prep.conv3d[0], prep.conv3d[1], cfg.conv3d_out)
             self._tap("conv3d", x)
         for i, c in enumerate(cfg.chans):
             st = prep.stacks[i]
-            rec = dict(x_in=x, mr_in=mr, H_in=H, W_in=W, full=None, blocks=[]) if tape is not None else None
-            fold = self.fold_stack_norm and rec is None  # inference: the post-pool GroupNorm is folded into its two consumers
+            rec = dict(x_in=x, mr_in=mr, H_in=H, W_in=W, full=None, blocks=[]) if stacks is not None else None
+            fold = self.fold_stack_norm and not train  # inference: the post-pool GroupNorm is folded into its two consumers
             if i == 0 and "fc_w" in st:
                 y1, mr1, chan = ops.firstconv_pool(img, st["fc_w"], st["fc_b"], c, zp=True, want_chan=True)
             else:
@@ -482,17 +496,19 @@ class MinecraftPolicy(nn.Module):
                 self._tap(f"{pfx}.stacks.{i}.blocks.{j}.conv0", hmid)
                 Wb, S1, S2 = st["convs"][2 * j + 1]
                 last = (i == len(cfg.chans) - 1) and j == 1
-                if rec is None:
+                if not train:
                     x, mr = ops.conv3x3_zp(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, residual=x, out=out if last else None)
                 else:
                     # training: the branch output r = relu(conv1(..)) is kept on its own (its sign pattern IS the ReLU mask the
                     # backward needs; x + r rounded to bf16 no longer shows which small r were positive), then added
                     r, _ = ops.conv3x3_zp(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, want_stats=False)
                     x, mr = ops.add_zp(x, r, H, W, out=out if last else None)
-                    rec["blocks"].append(dict(h=hmid, mrh=mrh, r=r, x=x, mr=mr))
+                    if rec is not None:
+                        rec["blocks"].append(dict(h=hmid, mrh=mrh, r=r, x=x, mr=mr))
+                    del r
                 self._tap(f"{pfx}.stacks.{i}.blocks.{j}", x)
             if rec is not None:
-                tape["stacks"].append(rec)
+                stacks.append(rec)
         return x, mr
 
     # -- transformer -----------------------------------------------------------------------------------------
@@ -591,23 +607,28 @@ class MinecraftPolicy(nn.Module):
         # ---- ImpalaCNN in frame chunks (bounds the activation workspace), then ONE dense GEMM over all frames
         cnn_out = torch.empty((N, Hf + 1, Wf + 1, C2), dtype=BF16, device=img.device)
         mrs = []
+        tape = self._tape
+        # training forward: tape["recompute"] None keeps every stack's activations for the backward (one CNN pass per call); an integer
+        # runs the CNN in chunks of that many frames, records nothing per stack, and the backward re-runs each chunk (training.py)
+        recompute = None if tape is None else tape.get("recompute")
+        stacks = tape["stacks"] if tape is not None and recompute is None else None
         if cfg.conv3d_out is None:
-            step = self.cnn_chunk_frames
+            step = self.cnn_chunk_frames if recompute is None else min(recompute, self.cnn_chunk_frames)
         else:  # chunks of whole sequences; the IDM's 128-channel full-resolution stage is ~13 MiB/frame
-            step = max(1, self.idm_chunk_frames // t) * t
+            step = max(1, (self.idm_chunk_frames if recompute is None else min(recompute, self.idm_chunk_frames)) // t) * t
         for f0 in range(0, N, step):
             F_ = min(step, N - f0)
             chunk = frames[f0:f0 + F_] if cfg.conv3d_out is None else frames[f0:f0 + F_].view(F_ // t, t, *frame_shape)
-            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_])
+            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_], train=tape is not None, stacks=stacks)
             mrs.append(mr)
         mr_c = mrs[0] if len(mrs) == 1 else torch.cat(mrs, 0)
         Kd = (Hf + 1) * (Wf + 1) * C2  # ZP rows flattened; the zero row / column meets zero weight columns
         xd, mr_d = self._linear(cnn_out.view(N, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
-        tape = self._tape
         if tape is not None:
-            if len(mrs) != 1:
+            if recompute is None and len(mrs) != 1:
                 raise NotImplementedError(f"training forward: at most {step} frames per call (got {N})")
-            tape.update(prep=prep, frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d)
+            tape.update(prep=prep, frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d,
+                        cnn_chunks=[(f0, min(f0 + step, N)) for f0 in range(0, N, step)])
         del cnn_out
         self._tap("img_process.cnn.dense", xd)
         x, mr_x = self._linear(xd, prep.linear, cfg.hidsize, mr=mr_d, relu=1, want_stats=True)
@@ -693,27 +714,38 @@ class _PolicyBase(nn.Module):
         self._hprep_fp = None
         self._autograd = False  # set_autograd
         self._state_grad = False
+        self._recompute_frames = None
         self._ag_runner = None
 
     def initial_state(self, batch_size: int):
         return self.net.initial_state(batch_size)
 
-    def set_autograd(self, on: bool = True, state_grad: bool = False):
+    def set_autograd(self, on: bool = True, state_grad: bool = False, recompute_frames: Optional[int] = None):
         """Opt in to the differentiable forward (also for `self.net` called on its own).  When on, a forward in grad mode (not inference
         mode) with at least one parameter that requires grad runs the training forward (no stack-norm fold; within the 1e-2 tolerance of
         the inference path, not bit-identical to it) as an autograd `Function` whose backward is the trainers' hand-written one, so that
         `loss.backward()` accumulates into `.grad`.  pd and vpred are attached to the graph; `state_out` is detached and a `state_in`
-        that requires grad raises (no gradient through the KV memory, behavioural_cloning.py:109-111).  At most `net.cnn_chunk_frames`
-        (2048) frames per call (the IDM: `net.idm_chunk_frames` (512) and T <= 128), bf16 mode only.  A parameter that only feeds outputs
-        the loss does not use gets None, as in the reference.  `act`, `predict`, `v` and `GraphedAct` stay inference-only.
+        that requires grad raises (no gradient through the KV memory, behavioural_cloning.py:109-111).  With recompute_frames=None at
+        most `net.cnn_chunk_frames` (2048) frames per call (the IDM: `net.idm_chunk_frames` (512)); always T <= 128 for the IDM and bf16
+        mode only.  A parameter that only feeds outputs the loss does not use gets None, as in the reference.  `act`, `predict`, `v` and
+        `GraphedAct` stay inference-only.
 
         state_grad=True (truncated backpropagation through time across calls): `state_out`'s K / V are attached to the graph too and a
         `state_in` whose K / V require grad is accepted, so a loss on a later call trains this one through the KV memory.  Truncate with
         `state = tree_map(detach)` every k calls and call `backward()` once per window: every call of the window keeps its tape (its
-        activations) until then.  Each call keeps its own limits.  No effect on a model without memory (the IDM)."""
+        activations) until then.  Each call keeps its own limits.  No effect on a model without memory (the IDM).
+
+        recompute_frames=F (a positive int): the forward runs the ImpalaCNN in chunks of F frames (at most `net.cnn_chunk_frames`; the
+        IDM rounds F down to whole sequences, at least one) and keeps only its output, and the backward re-runs each chunk's forward
+        before back-propagating through it.  That costs one more CNN forward per call and frees the CNN activations, nearly all of a
+        call's tape (20.7 MiB per frame at 2x width with its backward workspace, measured on an H100: README), so a call or a BPTT window can hold many more frames:
+        up to `training._Trainer.max_call_frames` per call.  The gradients are those of the stored tape (bit-identical when one chunk
+        holds the call).  None keeps the activations (faster when they fit)."""
+        recompute_frames = check_recompute_frames(recompute_frames)
         self._autograd = bool(on)
         self._state_grad = bool(on) and bool(state_grad)
-        self.net.set_autograd(on, state_grad=state_grad)
+        self._recompute_frames = recompute_frames if on else None
+        self.net.set_autograd(on, state_grad=state_grad, recompute_frames=recompute_frames)
         return self
 
     def set_precision(self, precision: str):

@@ -13,6 +13,10 @@ The three trainers share one path and differ only in the loss:
     _backward_from_dlog   `_heads_bwd` (the head weights, dlog -> d latent), then `_backward_from_dlat`: final_ln [-> lastlayer],
                           the transformer, img_process.linear, dense, the ImpalaCNN and, for the IDM, its conv3d pre-stage
 
+The ImpalaCNN's activations are nearly all of a call's tape.  With `recompute_frames` (the trainers' constructors, `set_autograd`) the
+forward keeps only the CNN's output and the backward re-runs the CNN chunk by chunk (`_recompute_cnn`), back-propagating through each
+chunk before making the next; without it the forward's tape is the one chunk.
+
 The differentiable forward (`set_autograd`, `_AutogradRunner` at the end of this file) runs the same taped forward and enters the same
 backward at dlog (any loss over pd / vpred, through `ops.log_softmax_bwd`) or at d latent (a bare network); its gradients go to a sink
 that hands them back to autograd instead of `param.grad`.
@@ -65,16 +69,29 @@ class _Trainer:
     and the backward from d logits.  A subclass checks its policy before calling `_Trainer.__init__` and supplies the loss."""
 
     use_lastlayer = True  # the model's forward runs `lastlayer` between the transformer and final_ln
+    # Frames per call with `recompute_frames` (without it the stored CNN tape bounds a call first: net.cnn_chunk_frames /
+    # net.idm_chunk_frames).  The CNN launches then see one chunk (at most net.cnn_chunk_frames frames, as in the inference forward);
+    # every launch above the CNN takes the call's N = B*T frames as rows: the GEMMs (the dense layer over [N, (Hf+1)(Wf+1)C2], the heads
+    # over [N, 8641 + ...]) as the 32-bit `vpt_gemm_args.M`, walked in 128-row tiles by a signed 32-bit TMA row coordinate; the norm,
+    # elementwise, softmax and head-gradient kernels as 64-bit row / element counts; the attention and the KV-memory copies put B on a
+    # grid's y axis.  So N <= 2^31 - 128 and B <= 65535; device memory (about 1 MB per frame above the CNN at 2x width) binds first.
+    max_call_frames = 2 ** 31 - 128
+    max_call_batch = 65535
 
-    def __init__(self, policy, net=None):
-        """`policy` may be None with `net` given: a bare MinecraftPolicy / InverseActionNet (no heads; the differentiable forward)."""
+    def __init__(self, policy, net=None, recompute_frames=None):
+        """`policy` may be None with `net` given: a bare MinecraftPolicy / InverseActionNet (no heads; the differentiable forward).
+        `recompute_frames`: see `BCTrainer`."""
+        from .policy import check_recompute_frames
+
         self.policy = policy
         self.net = policy.net if net is None else net
+        self.recompute_frames = check_recompute_frames(recompute_frames)
         self._sink = None  # None: gradients accumulate into `param.grad`; a dict: id(param) -> gradient (the differentiable forward)
         self._wprep = None
         self._wprep_fp = None
         self.keep_tape = False   # tests: keep the last forward's tape in `self.last_tape` (tests/forced_replica.py)
         self.last_tape = None
+        self.on_recompute = None  # tests: called as on_recompute(f0, f1, out, mr) with every chunk's recomputed CNN output and statistics
         self.graph_relayout = True  # re-layout of the kernel-side weights after an optimizer step as one CUDA graph replay
         self._rl_graph = None
         self._rl_seen = 0
@@ -239,14 +256,25 @@ class _Trainer:
         return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], gam, bet, add=add, relu_x=relu_x)
 
     # -- the step ---------------------------------------------------------------------------------------------------------
+    def check_call_frames(self, img):
+        """With `recompute_frames`: the per-call limits (`max_call_frames`, `max_call_batch`), checked before any work so that a call that
+        cannot finish accumulates nothing.  (The stored tape's limits are checked by the trainers and the differentiable forward.)"""
+        if self.recompute_frames is None:
+            return
+        B, t = img.shape[:2]
+        if B * t > self.max_call_frames or B > self.max_call_batch:
+            raise NotImplementedError(f"{type(self).__name__}: at most {self.max_call_frames} frames and B <= {self.max_call_batch} per call "
+                                      f"(got B = {B}, T = {t})")
+
     def _taped_latent(self, img, first, state_in):
         """The network's inference kernels, recording what the backward needs -> (latent bf16 [N][h], latent fp32 (B,t,h), tape, state_out).
         The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`)."""
         net = self.net
+        self.check_call_frames(img)
         self.refresh_weights()
         wts = self._weights()
         state_in = [(m, (k.detach(), v.detach())) for (m, (k, v)) in state_in]  # behavioural_cloning.py:111
-        tape = dict(stacks=[], blocks=[], wts=wts)
+        tape = dict(stacks=[], blocks=[], wts=wts, recompute=self.recompute_frames)
         net._tape = tape
         try:
             lat_bf16, lat_f32, state_out = net._forward_impl(img, first, state_in, use_lastlayer=self.use_lastlayer)
@@ -310,18 +338,39 @@ class _Trainer:
         dcnn = self._dense_bwd(dz, tape, wts, P)
         if upper_grads_ready is not None:
             upper_grads_ready()
-        # ---------------- ImpalaCNN, last stack to first ----------------
-        dx3 = self._cnn_bwd(dcnn, tape, wts, P)
-        del dcnn
-        if cfg.conv3d_out is not None:
-            # the IDM's conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
-            C3 = cfg.conv3d_out
-            frames = tape["frames"]
-            dW3, db3 = ops.conv3d_t5_bwd(frames.view(B, t, *frames.shape[1:]), dx3, C3)
+        # ---------------- ImpalaCNN, last stack to first, chunk by chunk (last chunk first) ----------------
+        # The stored tape is the one-chunk case: its per-stack activations come from the forward.  With `recompute` every chunk's are made
+        # again from the frames and the forward's weights, used, and dropped before the next chunk.
+        frames = tape["frames"]
+        for f0, f1 in reversed(tape["cnn_chunks"]):
+            ct = tape if tape["recompute"] is None else self._recompute_cnn(tape, f0, f1, t)
+            dx3 = self._cnn_bwd(dcnn[f0:f1], ct, wts, P)
+            del ct
+            if cfg.conv3d_out is not None:
+                # the IDM's conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
+                C3 = cfg.conv3d_out
+                dW3, db3 = ops.conv3d_t5_bwd(frames[f0:f1].view((f1 - f0) // t, t, *frames.shape[1:]), dx3, C3)
+                self._grad(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
+                self._grad(net.conv3d_layer.layer.bias, db3)
             del dx3
-            self._grad(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
-            self._grad(net.conv3d_layer.layer.bias, db3)
+        del dcnn
         return dmem
+
+    def _recompute_cnn(self, tape, f0, f1, t):
+        """The forward of CNN chunk [f0, f1) again, in the training layout with the kernel-layout weights the forward used (tape["prep"]),
+        recording what `_cnn_bwd` needs -> that chunk's tape.  The kernels are deterministic, so this is the forward's chunk bit for bit."""
+        net = self.net
+        cfg = net.cfg
+        frames = tape["frames"][f0:f1]
+        img = frames if cfg.conv3d_out is None else frames.view((f1 - f0) // t, t, *frames.shape[1:])
+        Hf, Wf = cfg.final_hw
+        out = torch.empty((f1 - f0, Hf + 1, Wf + 1, cfg.chans[-1]), dtype=BF16, device=frames.device)
+        stacks = []
+        with torch.no_grad():
+            _, mr = net._cnn_chunk(img, tape["prep"], out, train=True, stacks=stacks)
+        if self.on_recompute is not None:
+            self.on_recompute(f0, f1, out, mr)
+        return dict(stacks=stacks, prep=tape["prep"], frames=frames)
 
     def _dense_bwd(self, dz, tape, wts, P):
         cfg = self.net.cfg
@@ -446,15 +495,21 @@ class BCTrainer(_Trainer):
     `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions)` accumulates d loss / d param into `.grad`.
 
         loss = -(1 / (B*T)) * sum_{b,t} sum_heads log_softmax(logits_head / temperature)[action]      (lib/action_head.py:176-184)
+
+    recompute_frames=None keeps the ImpalaCNN's activations from the forward for the backward: at most `net.cnn_chunk_frames` (2048)
+    frames per call, and at 2x width 20.7 MiB per frame with its backward workspace (H100, README).  recompute_frames=F (a positive int) keeps only the CNN's output: the forward
+    runs the CNN in chunks of F frames (at most `net.cnn_chunk_frames`) and the backward re-runs each chunk's forward before
+    back-propagating through it.  That costs one more CNN forward per call and allows `max_call_frames` frames per call (e.g. B = 128,
+    T = 128 in one call at 2x width); the gradients are those of the stored tape.
     """
 
-    def __init__(self, policy: MinecraftAgentPolicy):
+    def __init__(self, policy: MinecraftAgentPolicy, recompute_frames=None):
         if not isinstance(policy, MinecraftAgentPolicy):
             raise TypeError(f"{type(self).__name__} trains a MinecraftAgentPolicy (behavioural_cloning.py:54-62)")
         cfg = policy.net.cfg
         if cfg.conv3d_out is not None or cfg.first_conv_norm or cfg.mask_style != "clipped_causal":
             raise NotImplementedError(f"{type(self).__name__}: only the causal policy models are trained by the reference")
-        super().__init__(policy)
+        super().__init__(policy, recompute_frames=recompute_frames)
 
     def _check_heads(self):
         """Every head must have a single sub-action.  Checked before the forward: nothing is accumulated into .grad by a call that
@@ -505,12 +560,12 @@ class RLTrainer(BCTrainer):
     `old_logprob`, `advantages` and `returns` are fp32 (B, T), `returns` in the denormalised space; `pd_ref` is what the frozen
     reference policy's forward returns for the same frames (None only with kl_coef == 0).  `trainer.stats` holds 0-d device tensors
     pi_loss, vf_loss, kl_ref and clipfrac of the last call.  Hand every parameter with `requires_grad` to the optimizer (the three
-    normaliser tensors have none)."""
+    normaliser tensors have none).  `recompute_frames` as in `BCTrainer`."""
 
     ewma_beta = 0.99999  # NormalizeEwma's default (lib/normalize_ewma.py:9; per_element_update=False, norm over (B, T))
 
-    def __init__(self, policy: MinecraftAgentPolicy):
-        super().__init__(policy)
+    def __init__(self, policy: MinecraftAgentPolicy, recompute_frames=None):
+        super().__init__(policy, recompute_frames=recompute_frames)
         self.stats = None
 
     def _head_layers(self):
@@ -579,15 +634,17 @@ class IDMTrainer(_Trainer):
     the conv3d pre-stage.  Which parameters get which gradient follows the reference's autograd: `lastlayer.*` gets None (its
     output is discarded, lib/policy.py:390-391); `r_layer.*` gets zeros and `b_nd` an empty (10, 0) gradient (R meets an empty band).
 
-    One call holds whole sequences (the temporal conv needs the neighbouring frames) and at most `net.idm_chunk_frames` (512) frames,
-    i.e. B = 4 at T = 128: the training forward keeps the whole CNN tape of one call.  Larger batches accumulate over calls
-    (`.grad` accumulates, as with BCTrainer).  bf16 only.  `first` and the state do nothing with mask "none": the state stays
+    One call holds whole sequences (the temporal conv needs the neighbouring frames).  With recompute_frames=None it holds at most
+    `net.idm_chunk_frames` (512) frames, i.e. B = 4 at T = 128: the training forward keeps the whole CNN tape of one call.  With
+    recompute_frames=F the CNN runs, and is re-run in the backward, in chunks of F frames rounded down to whole sequences (at least one,
+    at most `net.idm_chunk_frames`), and a call may hold `max_call_frames` frames (as in `BCTrainer`).  Batches also accumulate over calls
+    (`.grad` accumulates, as with BCTrainer).  T <= 128, bf16 only.  `first` and the state do nothing with mask "none": the state stays
     (None, (B,0,h), (B,0,h))."""
 
     max_t = 128  # frames per sequence the unmasked attention backward supports
     use_lastlayer = False  # the IDM's forward discards lastlayer's output (lib/policy.py:390-391)
 
-    def __init__(self, policy: InverseActionPolicy):
+    def __init__(self, policy: InverseActionPolicy, recompute_frames=None):
         if not isinstance(policy, InverseActionPolicy):
             raise TypeError("IDMTrainer trains an InverseActionPolicy (lib/policy.py:406-467)")
         cfg = policy.net.cfg
@@ -595,7 +652,7 @@ class IDMTrainer(_Trainer):
             raise NotImplementedError("IDMTrainer: needs the IDM configuration (conv3d pre-stage, attention mask 'none', no KV memory)")
         if cfg.timesteps is not None and cfg.timesteps > self.max_t:
             raise NotImplementedError(f"IDMTrainer: the unmasked attention backward supports chunks of at most {self.max_t} frames")
-        super().__init__(policy)
+        super().__init__(policy, recompute_frames=recompute_frames)
 
     @staticmethod
     def optimizer_params(policy):
@@ -614,8 +671,9 @@ class IDMTrainer(_Trainer):
         B, t = img.shape[:2]
         N = B * t
         # checked before the forward: nothing is accumulated into .grad by a call that cannot finish
-        if N > net.idm_chunk_frames:
-            raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls")
+        if self.recompute_frames is None and N > net.idm_chunk_frames:
+            raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls "
+                                      "or pass recompute_frames")
         if t > self.max_t:
             raise NotImplementedError(f"IDMTrainer: at most {self.max_t} frames per sequence (got T = {t})")
         lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
@@ -685,16 +743,19 @@ class _AutogradRunner(_Trainer):
             raise NotImplementedError("the differentiable forward runs in the bf16 mode only (set_precision('bf16'))")
         B, t = img.shape[:2]
         N = B * t
+        self.recompute_frames = self.module._recompute_frames  # set_autograd(.., recompute_frames=..)
+        stored = self.recompute_frames is None
         if net.cfg.conv3d_out is None:
-            if N > net.cnn_chunk_frames:
+            if stored and N > net.cnn_chunk_frames:
                 raise NotImplementedError(f"differentiable forward: at most {net.cnn_chunk_frames} frames per call (got B*T = {N}); "
-                                          "accumulate over calls")
+                                          "accumulate over calls or set_autograd(True, recompute_frames=...)")
         else:
-            if N > net.idm_chunk_frames:
+            if stored and N > net.idm_chunk_frames:
                 raise NotImplementedError(f"differentiable forward: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); "
-                                          "accumulate over calls")
+                                          "accumulate over calls or set_autograd(True, recompute_frames=...)")
             if t > IDMTrainer.max_t:
                 raise NotImplementedError(f"differentiable forward: at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
+        self.check_call_frames(img)
         if self.state_grad():
             return
         for _, (k, v) in state_in:
