@@ -1,6 +1,7 @@
 """The differentiable forward (`set_autograd`, training._AutogradRunner) on the CPU: `loss.backward()` through the test-only torch emulation
 of the ops (tests/emu_ops.py, tests/emu_idm_ops.py, tests/emu_autograd_ops.py) against autograd through the oracle and against the
 trainers.  tests/test_gpu_autograd.py repeats it through the CUDA kernels."""
+import copy
 import inspect
 
 import pytest
@@ -9,11 +10,13 @@ import torch
 import emu_autograd_ops
 import emu_idm_ops
 import emu_ops
+import emu_rl_ops
 import vpt_oracle as O
 from common import make_policy, small_kwargs
 from test_idm_training import check_pattern, kind, make_batch, make_idm
 from video_pre_training_b200 import ops, ops_autograd
-from video_pre_training_b200.training import BCTrainer, IDMTrainer
+from video_pre_training_b200.policy import _autograd_runner
+from video_pre_training_b200.training import BCTrainer, IDMTrainer, RLTrainer
 
 
 def _with_grad(fn):
@@ -205,6 +208,52 @@ def test_bc_and_idm_losses_match_the_trainers(emulated):
     (pd, _, _), _ = idm.set_autograd(True)({"img": img}, first, idm.initial_state(2))
     (-idm.logprob(actions, pd).mean()).backward()
     assert _worst(_grads(idm), ref) < 1e-2
+
+
+def test_trainers_and_differentiable_forward_share_the_layouts(emulated, monkeypatch):
+    """BCTrainer, RLTrainer and `loss.backward()` on one policy read the policy's one forward fold and net backward copy, rebuilt once for
+    all three after an in-place parameter update, and get the same gradients as each of them on a copy of the policy of its own."""
+    for name in dir(emu_rl_ops):
+        if not name.startswith("_") and callable(getattr(emu_rl_ops, name)) and hasattr(ops, name):
+            monkeypatch.setattr(ops, name, getattr(emu_rl_ops, name))
+    pol0, _, _ = make_policy(small_kwargs())
+    g = torch.Generator().manual_seed(9)
+    B, T = 2, 8
+    img, first, actions = batch(g, B, T)
+    rl_args = (0.1 * torch.randn(B, T, generator=g) - 14.0, torch.randn(B, T, generator=g), 3.0 + torch.randn(B, T, generator=g))
+    runs = []
+    for pols in ([pol0] * 3, [copy.deepcopy(pol0) for _ in range(3)]):
+        bc, rl, ag = BCTrainer(pols[0]), RLTrainer(pols[1]), _autograd_runner(pols[2].set_autograd(True))
+        for tr in (bc, rl, ag):
+            tr.keep_tape = True
+        rounds = []
+        for _ in range(2):
+            grads = []
+            for i, pol in enumerate(pols):
+                pol.zero_grad(set_to_none=True)
+                if i == 0:
+                    bc.loss_and_grad(img, first, pol.initial_state(B), actions)
+                elif i == 1:
+                    rl.loss_and_grad(img, first, pol.initial_state(B), actions, *rl_args, vf_coef=0.5, kl_coef=0.0)
+                else:
+                    (pd, _, _), _ = pol({"img": img}, first, pol.initial_state(B))
+                    bc_loss(pol, pd, actions).backward()
+                grads.append(_grads(pol))
+            rounds.append((grads, [(tr.last_tape["prep"], tr.last_tape["wts"]) for tr in (bc, rl, ag)]))
+            with torch.no_grad():
+                for pol in {id(p): p for p in pols}.values():
+                    for p in pol.parameters():
+                        if p.requires_grad:
+                            p.mul_(0.99)
+        runs.append(rounds)
+    for (grads, layouts), (grads_apart, _) in zip(*runs):
+        assert all(a is b for lay in layouts[1:] for a, b in zip(lay, layouts[0]))
+        for gs, ga in zip(grads, grads_apart):
+            assert gs.keys() == ga.keys()
+            for n in gs:
+                assert (gs[n] is None and ga[n] is None) or torch.equal(gs[n], ga[n]), n
+    (_, first_layouts), (_, second_layouts) = runs[0]
+    assert all(a is not b for a, b in zip(first_layouts[0], second_layouts[0]))
 
 
 def test_bare_network_latent_is_differentiable(emulated, exact):

@@ -10,7 +10,7 @@ from common import emulation, make_policy, small_kwargs
 from video_pre_training_b200 import _native as nat
 from video_pre_training_b200 import ops
 from video_pre_training_b200.parallel import FlatAdamDP
-from video_pre_training_b200.training import BCTrainer
+from video_pre_training_b200.training import BCTrainer, RLTrainer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -292,8 +292,8 @@ def test_bc_training_reduces_the_loss():
     assert all(l == l for l in losses) and losses[-1] < losses[0] - 0.5, losses
 
 
-def test_graphed_weight_relayout_equals_eager():
-    """BCTrainer.refresh_weights: from the second optimizer step on the kernel-side weight re-layout is one CUDA-graph replay; the
+def test_graphed_policy_relayout_equals_eager():
+    """The policy's refresh_weights: from the second optimizer step on the kernel-side weight re-layout is one CUDA-graph replay; the
     training trajectory must be bit-identical to the eager re-layout."""
     img, first, actions = _case(seed=2, B=2)
     img, first = img.to(DEV), first.to(DEV)
@@ -303,7 +303,7 @@ def test_graphed_weight_relayout_equals_eager():
         pol, _, _ = make_policy(small_kwargs(), seed=4)
         pol = pol.to(DEV)
         tr = BCTrainer(pol)
-        tr.graph_relayout = graphed
+        pol.graph_relayout = graphed
         opt = FlatAdamDP([p for n, p in pol.named_parameters() if not n.startswith("value_head")], lr=2e-4)
         losses = []
         for _ in range(5):
@@ -311,11 +311,45 @@ def test_graphed_weight_relayout_equals_eager():
             loss, _ = tr.loss_and_grad(img, first, pol.initial_state(2), actions)
             opt.step()
             losses.append(loss.item())
-        assert (tr._rl_graph is not None) == graphed
+        assert (pol._relayout is not None) == graphed
         finals.append((losses, opt.flat_p.clone()))
     nat.device_check()
     assert finals[0][0] == finals[1][0], (finals[0][0], finals[1][0])
     assert torch.equal(finals[0][1], finals[1][1])
+
+
+def test_bc_and_rl_steps_share_one_relayout_graph():
+    """BC and RL steps alternating on one policy with FlatAdamDP: the policy holds one re-layout graph, which rewrites both trainers'
+    heads_t as well, and the trajectory (losses, parameters, EWMA normaliser) is bit-identical to the eager re-layout."""
+    B, T = 2, 8
+    img, first, actions = _case(seed=3, B=B, T=T)
+    img, first = img.to(DEV), first.to(DEV)
+    actions = {k: v.to(DEV) for k, v in actions.items()}
+    g = torch.Generator().manual_seed(5)
+    old = (0.1 * torch.randn(B, T, generator=g) - 14.0).to(DEV)  # ~ log(1/121) + log(1/8641): ratios near 1
+    adv, returns = torch.randn(B, T, generator=g).to(DEV), (3.0 + torch.randn(B, T, generator=g)).to(DEV)
+    finals = []
+    for graphed in (False, True):
+        pol, _, _ = make_policy(small_kwargs(), seed=4)
+        pol = pol.to(DEV)
+        pol.graph_relayout = graphed
+        bc, rl = BCTrainer(pol), RLTrainer(pol)
+        opt = FlatAdamDP(pol.parameters(), lr=2e-4)  # (the normaliser does not require grad: not in the bucket)
+        losses = []
+        for i in range(6):
+            opt.zero_grad()
+            if i % 2 == 0:
+                loss, _ = bc.loss_and_grad(img, first, pol.initial_state(B), actions)
+            else:
+                loss, _ = rl.loss_and_grad(img, first, pol.initial_state(B), actions, old, adv, returns, vf_coef=0.5, kl_coef=0.0)
+            opt.step()
+            losses.append(loss.item())
+        # one graph: the net's forward folds and backward transposes, the head folds, BC's and RL's heads_t
+        assert (pol._relayout is not None and len(pol._relayout[1]) == 5) if graphed else pol._relayout is None
+        finals.append((losses, opt.flat_p.clone(), pol.value_head.normalizer.running_mean.clone()))
+    nat.device_check()
+    assert finals[0][0] == finals[1][0], (finals[0][0], finals[1][0])
+    assert torch.equal(finals[0][1], finals[1][1]) and torch.equal(finals[0][2], finals[1][2])
 
 
 def test_bc_step_at_3x_width_shapes():

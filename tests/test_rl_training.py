@@ -188,7 +188,7 @@ def test_rl_with_unit_ratio_and_advantage_is_the_bc_step(emulated, exact):
             assert ((p.grad - bc[n]).norm() / bc[n].norm()).item() < 1e-5, n
 
 
-def test_rl_second_call_keeps_the_weight_layouts(emulated):
+def test_rl_second_call_keeps_the_policy_weight_layouts(emulated):
     """The normaliser update of a call does not invalidate the kernel-layout weight caches, but `denormalize` sees it."""
     pol, _, _, _ = make_pair()
     tr = RLTrainer(pol)
@@ -199,10 +199,11 @@ def test_rl_second_call_keeps_the_weight_layouts(emulated):
     actions = {"camera": torch.randint(0, 121, (B, T, 1), generator=g), "buttons": torch.randint(0, 8641, (B, T, 1), generator=g)}
     args = (torch.zeros(B, T), torch.ones(B, T), 5.0 + torch.randn(B, T, generator=g))
     tr.loss_and_grad(img, first, pol.initial_state(B), actions, *args, vf_coef=1.0, kl_coef=0.0)
-    held = (pol.net._prep, pol._hprep, tr._wprep)
+    layouts = lambda: (pol.net.prepared(), pol._heads_prepared(), pol.net.prepared_backward(), pol._heads_prepared_backward(tr._head_layers()))
+    held = layouts()
     v0 = pol.denormalize(torch.zeros(1, 1, 1)).clone()
     tr.loss_and_grad(img, first, pol.initial_state(B), actions, *args[:2], args[2] + 3.0, vf_coef=1.0, kl_coef=0.0)
-    assert pol.net._prep is held[0] and pol._hprep is held[1] and tr._wprep is held[2]
+    assert all(a is b for a, b in zip(layouts(), held))
     assert not torch.equal(pol.denormalize(torch.zeros(1, 1, 1)), v0)
 
 

@@ -133,7 +133,7 @@ if a.ops and rank == 0:
     p0.record()
     pol.net.prepared(); pol._heads_prepared()
     p1.record()
-    tr._weights()
+    pol.net.prepared_backward(); pol._heads_prepared_backward(tr._head_layers())
     p2.record()
     torch.cuda.synchronize()
     print(f"instrumented step: fwd+bwd {s0.elapsed_time(s1):.1f} ms, adam {s1.elapsed_time(s2):.1f} ms; sum of ops {sum(tot.values()):.1f} ms; "

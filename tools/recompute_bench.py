@@ -107,8 +107,6 @@ def bc_step(pol, opt, trainers, batches, B):
 def bc_stored_vs_recompute(width, rfs):
     pol, opt = policy(width)
     batch = [frames(torch.Generator(device="cuda").manual_seed(0), 16)]
-    # one trainer for every variant: a second one would hold a second copy of the kernel-layout weights, for which the 3x stored tape
-    # leaves no room on an 80 GB card
     tr = vpt_b200.BCTrainer(pol)
 
     def with_recompute(rf):

@@ -184,8 +184,8 @@ class FlatAdamDP:
                                               self.exp_avg_sq.data_ptr(), self.n, self.lr, self.betas[0], self.betas[1], self.eps,
                                               self.weight_decay, 1.0 / world, self.t, torch.cuda.current_stream().cuda_stream),
                       "vpt_adam_step")
-            # the kernel wrote the parameters through raw pointers: bump their version counters so that the kernel-layout weight
-            # copies (policy._Prepared, training.BCTrainer._weights) are rebuilt before the next forward
+            # the kernel wrote the parameters through raw pointers: bump their version counters so that the model's kernel-layout
+            # weight copies (policy._Versioned) are rebuilt before the next forward
             for p in self.params:
                 torch.autograd.graph.increment_version(p)
         else:

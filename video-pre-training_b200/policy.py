@@ -17,6 +17,7 @@ the input GroupNorm gamma folded in plus the 9 border-class fold tables, linear 
 After `set_autograd(True)` a forward in grad mode (with a parameter that requires grad) is instead an autograd `Function` on that
 same backward, so that `loss.backward()` trains the model (training._AutogradRunner).  There is no CPU path: CPU tensors raise.
 """
+import functools
 import math
 from collections import OrderedDict
 from typing import Dict, Optional
@@ -123,6 +124,8 @@ class NetConfig:
         if self.first_conv_norm and self.conv3d_out is None:
             raise NotImplementedError("vpt_b200: first_conv_norm without the conv3d pre-stage is not implemented")
         self.final_hw = (H // 8, W // 8)
+        # columns of the attention's input gradient in the backward: q | k | v [| R, 10 rows per head, clipped_causal], padded to 8
+        self.kcat = (3 * hidsize + NBASIS * attention_heads + 7) // 8 * 8 if self.mask_style == "clipped_causal" else 3 * hidsize
 
     def forward_flops_per_frame(self, head_outputs: int = 121 + 8641 + 1) -> float:
         """Algorithmic work of one frame through the forward path (SURVEY.md section 8d): 2 x MAC; clipped-causal attention counts
@@ -341,8 +344,31 @@ class _Prepared:
         self.fin_g, self.fin_b = g("final_ln.weight").float().contiguous(), g("final_ln.bias").float().contiguous()
 
 
-def _fingerprint(module: nn.Module):
-    return tuple((p.data_ptr(), p._version) for p in module.parameters())
+def _fingerprint(params):
+    return tuple((p.data_ptr(), p._version) for p in params)
+
+
+class _Versioned:
+    """One kernel-layout copy of some parameters and the versions it was made from: `get()` rebuilds it when a parameter has new storage
+    (a load, `.to()`) or was updated in place (an optimizer step; FlatAdamDP bumps `_version` after its kernel writes).  `params` and
+    `build` are bound methods of the owning module, so that a deep copy of the module owns its own copy; `build` makes weights only,
+    since `_PolicyBase.refresh_weights` also runs it inside a CUDA graph capture."""
+
+    def __init__(self, params, build):
+        self.params, self.build = params, build
+        self.fp = self.value = None
+
+    def stale(self):
+        return self.value is None or _fingerprint(self.params()) != self.fp
+
+    def get(self):
+        if self.stale():
+            with torch.no_grad():
+                self.set(self.build())
+        return self.value
+
+    def set(self, value):
+        self.value, self.fp = value, _fingerprint(self.params())
 
 
 def _differentiable(module: nn.Module) -> bool:
@@ -377,6 +403,7 @@ class MinecraftPolicy(nn.Module):
     cnn_chunk_frames = 2048  # frames per CNN pass (bounds the activation workspace: ~5 MiB/frame at 2x width)
     fold_stack_norm = True   # inference: fold the post-pool GroupNorm of every stack into block 0 (no `affine_norm_zp` pass)
     idm_chunk_frames = 512   # IDM: ~13 MiB/frame at 4x width (conv3d output + full-resolution first conv)
+    use_lastlayer = True     # the forward runs `lastlayer` between the transformer and final_ln
 
     def __init__(self, **policy_kwargs):
         super().__init__()
@@ -385,11 +412,10 @@ class MinecraftPolicy(nn.Module):
         self.single_output = self.cfg.single_output
         for name, t in _net_schema(self.cfg).items():
             _set(self, name, t)
-        self._prep = None
-        self._prep_fp = None
+        self._fold = _Versioned(self.parameters, self._build_prepared)
+        self._fold_fp32 = _Versioned(self.parameters, self._build_prepared_precise)
+        self._bwd = _Versioned(self.parameters, self._build_backward)
         self.precision = "bf16"  # "fp32": the fp32-parity mode (precise.py): bf16 hi/lo split operands, fp32 activations
-        self._pprep = None
-        self._pprep_fp = None
         self.debug_taps = None  # set to a dict to capture intermediate activations (tests)
         self._tape = None       # set to a dict by training.BCTrainer: the forward then records what the backward needs
         self._autograd = False  # set_autograd
@@ -418,21 +444,49 @@ class MinecraftPolicy(nn.Module):
 
     # -- weights -------------------------------------------------------------------------------------------
     def prepared(self) -> _Prepared:
-        fp = _fingerprint(self)
-        if self._prep is None or fp != self._prep_fp:
-            with torch.no_grad():
-                self._prep = _Prepared(self.cfg, dict(self.named_parameters()))
-            self._prep_fp = fp
-        return self._prep
+        return self._fold.get()
 
     def prepared_precise(self):
+        return self._fold_fp32.get()
+
+    def prepared_backward(self):
+        """The dgrad weights of every layer the trainers' backward runs through (training.py)."""
+        return self._bwd.get()
+
+    def _build_prepared(self):
+        return _Prepared(self.cfg, dict(self.named_parameters()))
+
+    def _build_prepared_precise(self):
         from .precise import PreparedPrecise
-        fp = _fingerprint(self)
-        if self._pprep is None or fp != self._pprep_fp:
-            with torch.no_grad():
-                self._pprep = PreparedPrecise(self.cfg, dict(self.named_parameters()))
-            self._pprep_fp = fp
-        return self._pprep
+        return PreparedPrecise(self.cfg, dict(self.named_parameters()))
+
+    def _build_backward(self):
+        from .training import _rot, _tr
+        cfg = self.cfg
+        P = dict(self.named_parameters())
+        w = dict(stacks=[], layers=[])
+        pfx = "img_process.cnn"
+        for i in range(len(cfg.chans)):
+            s = f"{pfx}.stacks.{i}"
+            st = dict(convs=[_rot(P[f"{s}.blocks.{j}.conv{k}.layer.weight"]) for j in range(2) for k in range(2)])
+            if i > 0 or cfg.first_conv_norm:  # (stack 0's plain first conv has its own backward kernel, ops.firstconv_bwd)
+                st["first"] = _rot(P[f"{s}.firstconv.layer.weight"])
+            w["stacks"].append(st)
+        perm = lambda v: _dense_to_zp(v.detach(), cfg)
+        w["dense_t"] = _tr(perm(P[f"{pfx}.dense.layer.weight"]))
+        w["dense_g"] = perm(P[f"{pfx}.dense.norm.weight"]).float().contiguous()
+        w["dense_b"] = perm(P[f"{pfx}.dense.norm.bias"]).float().contiguous()
+        w["linear_t"] = _tr(P["img_process.linear.layer.weight"])
+        qkvr = ("q", "k", "v", "r") if cfg.mask_style == "clipped_causal" else ("q", "k", "v")  # R only where the mask has a band
+        for l in range(cfg.n_layers):
+            o = f"recurrent_layer.blocks.{l}.r.orc_block"
+            b = f"recurrent_layer.blocks.{l}"
+            cat = torch.cat([P[f"{o}.{c}_layer.weight"] for c in qkvr], 0)
+            w["layers"].append(dict(qkvr_t=_tr(cat, cfg.kcat), proj_t=_tr(P[f"{o}.proj_layer.weight"]), mlp0_t=_tr(P[f"{b}.mlp0.layer.weight"]),
+                                    mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
+        if self.use_lastlayer:
+            w["last_t"] = _tr(P["lastlayer.layer.weight"])
+        return w
 
     def _tap(self, name, t):
         if self.debug_taps is not None:
@@ -581,7 +635,7 @@ class MinecraftPolicy(nn.Module):
 
     # -- whole net -------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def _forward_impl(self, img, first, state_in, use_lastlayer=True):
+    def _forward_impl(self, img, first, state_in):
         cfg = self.cfg
         ops.require_cuda(img)
         if img.dtype != torch.uint8:
@@ -595,7 +649,7 @@ class MinecraftPolicy(nn.Module):
             if self._tape is not None:
                 raise NotImplementedError("the BC step runs in the bf16 mode only")
             from . import precise
-            return precise.forward(self, img, first, state_in, use_lastlayer)
+            return precise.forward(self, img, first, state_in)
         if self.precision != "bf16":
             raise ValueError(f"unknown precision {self.precision!r} (use 'bf16' or 'fp32')")
         prep = self.prepared()
@@ -641,7 +695,7 @@ class MinecraftPolicy(nn.Module):
             x, mr_x, s = self._block(l, x, mr_x, first_u8, state_in[l], B, t, prep, last=(l == cfg.n_layers - 1))
             state_out.append(s)
         # x is relu(recurrent output) here
-        if use_lastlayer:
+        if self.use_lastlayer:
             z_last, mr_zl = x, mr_x
             x, mr_x = self._linear(x, prep.last, cfg.hidsize, mr=mr_x, relu=1, want_stats=True)
             if tape is not None:
@@ -666,6 +720,8 @@ class InverseActionNet(MinecraftPolicy):
     relu -> final_ln.  `lastlayer` keeps its parameters (state_dict schema) but its output is discarded by the reference
     (lib/policy.py:390-391), so it is not computed."""
 
+    use_lastlayer = False
+
     def __init__(self, hidsize=512, conv3d_params=None, **MCPoliy_kwargs):
         super().__init__(hidsize=hidsize, conv3d_params=conv3d_params, **MCPoliy_kwargs)
 
@@ -675,7 +731,7 @@ class InverseActionNet(MinecraftPolicy):
         if _differentiable(self):
             (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
         else:
-            _, latent, state_out = self._forward_impl(ob["img"], first, state_in, use_lastlayer=False)
+            _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
         return (latent, None), state_out
 
 
@@ -686,6 +742,7 @@ class _PolicyBase(nn.Module):
     """Shared head plumbing of MinecraftAgentPolicy and InverseActionPolicy (lib/action_head.py:136-260)."""
 
     has_value_head = True
+    graph_relayout = True  # `refresh_weights` as one CUDA graph replay (False: the copies are rebuilt eagerly on use)
 
     def _init_heads(self, action_space, pi_head_kwargs):
         self.action_space = action_space
@@ -710,8 +767,11 @@ class _PolicyBase(nn.Module):
             _set(self, f"pi_head.{name}.linear_layer.weight", w)
             _set(self, f"pi_head.{name}.linear_layer.bias", b)
             self.head_specs[name] = (shape, n)
-        self._hprep = None
-        self._hprep_fp = None
+        self._heads_fold = _Versioned(self._head_params, self._build_heads_prepared)
+        self._heads_fold_fp32 = _Versioned(self._head_params, self._build_heads_prepared_precise)
+        self._heads_bwd = {}       # tuple of head layers -> _Versioned heads_t (`_heads_prepared_backward`)
+        self._relayout = None      # (parameter pointers, copies, CUDA graph, graph-owned layouts) of `refresh_weights`
+        self._relayout_seen = 0
         self._autograd = False  # set_autograd
         self._state_grad = False
         self._recompute_frames = None
@@ -755,49 +815,88 @@ class _PolicyBase(nn.Module):
         self.net.precision = precision
         return self
 
+    # -- kernel-layout copies of the head weights, and their re-layout after an optimizer step ------------------
+    def _head_params(self):
+        """The parameters of the heads' kernel-layout copies.  The EWMA normaliser is in none of them: an RL step updates it on every call,
+        and `denormalize` caches its own scalars."""
+        return [*self.pi_head.parameters(), *(self.value_head.linear.parameters() if self.has_value_head else ())]
+
+    def _heads_prepared(self):
+        return self._heads_fold.get()
+
     def _heads_prepared_precise(self):
-        from .precise import _f, _split_w
-        params = [p for n, p in self.named_parameters() if not n.startswith("net.")]
-        fp = tuple((p.data_ptr(), p._version) for p in params)
-        if getattr(self, "_hpprep", None) is None or fp != self._hpprep_fp:
-            with torch.no_grad():
-                ws, bs, cols, c0 = [], [], OrderedDict(), 0
-                for name in self.head_specs:
-                    lin = getattr(self.pi_head, name).linear_layer
-                    ws.append(lin.weight.detach())
-                    bs.append(lin.bias.detach())
-                    cols[name] = (c0, lin.weight.shape[0])
-                    c0 += lin.weight.shape[0]
-                self._hpprep = dict(pi=(_split_w(torch.cat(ws, 0)), _f(torch.cat(bs, 0))), cols=cols, ntot=c0)
-                if self.has_value_head:
-                    self._hpprep["v"] = (_split_w(self.value_head.linear.weight), _f(self.value_head.linear.bias))
-            self._hpprep_fp = fp
-        return self._hpprep
+        return self._heads_fold_fp32.get()
 
-    def _heads_fp(self):
-        """Versions of the head weights (the EWMA normaliser is not folded into any kernel-layout copy: `denormalize` keys it itself)."""
-        return tuple((p.data_ptr(), p._version) for n, p in self.named_parameters() if not n.startswith(("net.", "value_head.normalizer.")))
+    def _heads_prepared_backward(self, layers):
+        """heads_t, the dgrad weight bf16 [h][ld] of the given head layers (the column blocks of the trainers' logits gradient, in order),
+        zero-padded to a multiple of 8 columns.  One copy per list of layers: the BC and IDM steps use the action heads, the RL step and
+        the differentiable forward the value head as well."""
+        key = tuple(layers)
+        if key not in self._heads_bwd:
+            self._heads_bwd[key] = _Versioned(self._head_params, functools.partial(self._build_heads_backward, key))
+        return self._heads_bwd[key].get()
 
-    def _build_heads_prepared(self):
+    def _pi_matrix(self):
+        """The action heads as one linear layer: (weight [ntot][h], bias [ntot], {name: (first column, width)}, ntot)."""
         ws, bs, cols, c0 = [], [], OrderedDict(), 0
-        for name, (shape, n) in self.head_specs.items():
+        for name in self.head_specs:
             lin = getattr(self.pi_head, name).linear_layer
             ws.append(lin.weight.detach())
             bs.append(lin.bias.detach())
             cols[name] = (c0, lin.weight.shape[0])
             c0 += lin.weight.shape[0]
-        hp = dict(pi=_fold_linear(torch.cat(ws, 0), bias=torch.cat(bs, 0)), cols=cols, ntot=c0)
+        return torch.cat(ws, 0), torch.cat(bs, 0), cols, c0
+
+    def _build_heads_prepared(self):
+        W, b, cols, ntot = self._pi_matrix()
+        hp = dict(pi=_fold_linear(W, bias=b), cols=cols, ntot=ntot)
         if self.has_value_head:
             hp["v"] = _fold_linear(self.value_head.linear.weight.detach(), bias=self.value_head.linear.bias.detach())
         return hp
 
-    def _heads_prepared(self):
-        fp = self._heads_fp()
-        if self._hprep is None or fp != self._hprep_fp:
-            with torch.no_grad():
-                self._hprep = self._build_heads_prepared()
-            self._hprep_fp = fp
-        return self._hprep
+    def _build_heads_prepared_precise(self):
+        from .precise import _f, _split_w
+        W, b, cols, ntot = self._pi_matrix()
+        hp = dict(pi=(_split_w(W), _f(b)), cols=cols, ntot=ntot)
+        if self.has_value_head:
+            hp["v"] = (_split_w(self.value_head.linear.weight), _f(self.value_head.linear.bias))
+        return hp
+
+    def _build_heads_backward(self, layers):
+        from .training import _tr
+        rows = sum(lin.weight.shape[0] for lin in layers)
+        return _tr(torch.cat([lin.weight for lin in layers], 0), (rows + 7) // 8 * 8)
+
+    def refresh_weights(self):
+        """Re-layout after an optimizer step of the copies training uses (net forward folds and backward transposes, head folds, every
+        `heads_t` asked for); called by the trainers and the differentiable forward, a no-op when nothing changed.  Eagerly ~500 small
+        launches; the parameters live at fixed addresses (FlatAdamDP's bucket), so from the second refresh on it is ONE captured CUDA
+        graph replay writing the same tensors in place.  No parameter changes between a forward and its backward (the trainers run both
+        in one call, the differentiable forward's version check refuses it), so no tape's layouts are rewritten before its backward."""
+        caches = [self.net._fold, self._heads_fold, self.net._bwd, *self._heads_bwd.values()]
+        if not any(c.stale() for c in caches):
+            return
+        if not self.graph_relayout or not all(p.is_cuda for p in self.parameters()):
+            return  # the getters rebuild eagerly on use
+        ptrs = tuple(p.data_ptr() for p in self.parameters())
+        if self._relayout is not None and (self._relayout[0] != ptrs or self._relayout[1] != caches):
+            self._relayout = None  # the parameters moved (e.g. .to(), a new optimizer bucket) or a new heads_t was asked for: capture again
+        if self._relayout is None:
+            self._relayout_seen += 1
+            if self._relayout_seen < 2:
+                return  # first change: eager (also warms up every lazily initialised helper before capture)
+            g = torch.cuda.CUDAGraph()
+            torch.cuda.synchronize()
+            with torch.no_grad(), torch.cuda.graph(g):
+                values = [c.build() for c in caches]
+            self._relayout = (ptrs, caches, g, values)
+        _, caches, g, values = self._relayout
+        g.replay()
+        for c, v in zip(caches, values):
+            c.set(v)
+
+    def __getstate__(self):
+        return {**super().__getstate__(), "_relayout": None, "_relayout_seen": 0}  # a copy captures its own graph (a CUDA graph cannot be copied)
 
     @torch.no_grad()
     def _heads(self, lat_bf16, B, t, mask=None):
@@ -880,6 +979,7 @@ class MinecraftAgentPolicy(_PolicyBase):
         super().__init__()
         self.net = MinecraftPolicy(**policy_kwargs)
         self._init_heads(action_space, pi_head_kwargs)
+        self._denorm = _Versioned(self.value_head.normalizer.parameters, self._build_denorm)
 
     def forward(self, obs, first: torch.Tensor, state_in):
         """lib/policy.py:252-269 -> ((pi_logits, vpred, None), state_out)."""
@@ -899,17 +999,15 @@ class MinecraftAgentPolicy(_PolicyBase):
 
     def denormalize(self, v):
         """lib/normalize_ewma.py:31-35,57-60 (a 3-scalar affine map; host-side glue)."""
+        std, mean = self._denorm.get()  # the scalars only change when the normaliser is updated / reloaded:
+        return v * std + mean           # 7 of the 9 tiny launches per rollout step were their recomputation
+
+    def _build_denorm(self):
         nz = self.value_head.normalizer
-        bufs = (nz.debiasing_term, nz.running_mean, nz.running_mean_sq)
-        key = tuple((b.data_ptr(), b._version) for b in bufs)
-        if getattr(self, "_denorm_key", None) != key:  # the three scalars only change when the normaliser is updated / reloaded:
-            deb = nz.debiasing_term.clamp(min=1e-5)    # 7 of the 9 tiny launches per rollout step were this recomputation
-            mean = nz.running_mean / deb
-            var = (nz.running_mean_sq / deb - mean ** 2).clamp(min=1e-2)
-            self._denorm = (torch.sqrt(var)[None, None], mean[None, None])
-            self._denorm_key = key
-        std, mean = self._denorm
-        return v * std + mean
+        deb = nz.debiasing_term.clamp(min=1e-5)
+        mean = nz.running_mean / deb
+        var = (nz.running_mean_sq / deb - mean ** 2).clamp(min=1e-2)
+        return torch.sqrt(var)[None, None], mean[None, None]
 
     def get_logprob_of_action(self, pd, action):
         """lib/policy.py:271-279."""
@@ -989,7 +1087,7 @@ class InverseActionPolicy(_PolicyBase):
         if _differentiable(self):
             outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
             return (OrderedDict(zip(self.head_specs, outs)), None, None), state_out
-        lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in, use_lastlayer=False)
+        lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in)
         B, t = obs["img"].shape[:2]
         pi_logits, _ = self._heads(lat_bf16, B, t, mask)
         return (pi_logits, None, None), state_out
@@ -1024,8 +1122,7 @@ class GraphedAct:
         self.state = [(torch.zeros((B, 1, cfg.maxlen), dtype=torch.bool, device=dev),
                        (torch.zeros((B, cfg.maxlen, cfg.hidsize), dtype=F32, device=dev),
                         torch.zeros((B, cfg.maxlen, cfg.hidsize), dtype=F32, device=dev))) for _ in range(cfg.n_layers)]
-        policy.net.prepared()
-        policy._heads_prepared()
+        self._held = self._layouts()
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):  # warm-up outside capture (lazy function attributes, allocator pools)
@@ -1033,19 +1130,13 @@ class GraphedAct:
                 policy.act({"img": self.img}, self.first, self.state)
         torch.cuda.current_stream(dev).wait_stream(side)
         self.graphs = {}
-        self._pin()
 
-    def _weights_fp(self):
-        return _fingerprint(self.policy)
-
-    def _pin(self):
-        """The captured graph holds RAW device pointers into the kernel-layout weight copies: keep those copies alive and remember
-        which parameter versions they were made from (a later load_weights / optimizer step invalidates the graph)."""
-        self._fp = self._weights_fp()
-        self._held = (self.policy.net.prepared(), self.policy._heads_prepared())
-        if self.policy.has_value_head:  # refresh the cached de-normalisation scalars OUTSIDE the capture (they must not live in the graph's pool)
-            with torch.no_grad():
-                self.policy.denormalize(torch.zeros((1, 1, 1), device=self.img.device))
+    def _layouts(self):
+        """What a captured graph reads through RAW device pointers: the kernel-layout weight copies and the de-normalisation scalars, as
+        the policy holds them now (it rebuilds a stale one here, OUTSIDE any capture: they must not live in a graph's pool).  A copy
+        re-laid out in place by `refresh_weights` stays the same object, and the graph reads its new values."""
+        pol = self.policy
+        return pol.net.prepared(), pol._heads_prepared(), pol._denorm.get()
 
     def _capture(self, stochastic: bool):
         g = torch.cuda.CUDAGraph()
@@ -1078,9 +1169,10 @@ class GraphedAct:
                     m_in.copy_(m)
                 k_in.copy_(k)
                 v_in.copy_(v)
-        if self._weights_fp() != self._fp:  # parameters changed since capture: re-layout the weights and re-capture
+        held = self._layouts()
+        if any(a is not b for a, b in zip(held, self._held)):  # a copy was rebuilt since capture (a load, an optimizer step): re-capture
             self.graphs = {}
-            self._pin()
+            self._held = held
         g, ac, res = self.graphs.get(stochastic) or self._capture(stochastic)
         g.replay()
         out = {"log_prob": res["log_prob"], "vpred": res["vpred"]}

@@ -97,7 +97,7 @@ def _norm_gemm(x, rows, C, W, gamma, beta, N, *, conv=None, groups=None, relu=Tr
     return gemm3(xh, xl, W, rows, N, K, conv=conv, relu=relu)
 
 
-def forward(net, img, first, state_in, use_lastlayer=True):
+def forward(net, img, first, state_in):
     """policy.MinecraftPolicy._forward_impl in the fp32-parity mode -> ((latent hi, latent lo), latent fp32 (B,t,h), state_out)."""
     cfg = net.cfg
     prep = net.prepared_precise()
@@ -178,7 +178,7 @@ def forward(net, img, first, state_in, use_lastlayer=True):
         x = ops.add_f32(y, gemm3(hh, hl, L["mlp1"][0], N, h, h * cfg.pointwise_ratio, bias=L["mlp1"][1]), relu=last)  # F.relu of lib/policy.py:211
         if not last:
             net._tap(f"recurrent_layer.blocks.{l}", x)
-    if use_lastlayer:
+    if net.use_lastlayer:
         Wt, gt, bt = prep.last
         x = _norm_gemm(x, N, h, Wt, gt, bt, h)
     lh, ll, lat = ops.norm_split_f32(x, ops.group_stats_f32(x, N), prep.fin[0], prep.fin[1], groups=N, want_f32=True)

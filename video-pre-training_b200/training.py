@@ -39,7 +39,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops
-from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy, _dense_from_zp, _dense_to_zp
+from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy, _dense_from_zp
 
 
 def _rot(W):
@@ -65,10 +65,10 @@ def _acc(p, g):
 
 
 class _Trainer:
-    """The machinery the trainers share: backward-side weight layouts and their re-layout after an optimizer step, the taped forward
-    and the backward from d logits.  A subclass checks its policy before calling `_Trainer.__init__` and supplies the loss."""
+    """The machinery the trainers share: the taped forward and the backward from d logits, on the kernel-layout weights the model keeps
+    (`MinecraftPolicy.prepared_backward`, `_PolicyBase._heads_prepared_backward`).  A subclass checks its policy before calling
+    `_Trainer.__init__` and supplies the loss."""
 
-    use_lastlayer = True  # the model's forward runs `lastlayer` between the transformer and final_ln
     # Frames per call with `recompute_frames` (without it the stored CNN tape bounds a call first: net.cnn_chunk_frames /
     # net.idm_chunk_frames).  The CNN launches then see one chunk (at most net.cnn_chunk_frames frames, as in the inference forward);
     # every launch above the CNN takes the call's N = B*T frames as rows: the GEMMs (the dense layer over [N, (Hf+1)(Wf+1)C2], the heads
@@ -87,20 +87,9 @@ class _Trainer:
         self.net = policy.net if net is None else net
         self.recompute_frames = check_recompute_frames(recompute_frames)
         self._sink = None  # None: gradients accumulate into `param.grad`; a dict: id(param) -> gradient (the differentiable forward)
-        self._wprep = None
-        self._wprep_fp = None
         self.keep_tape = False   # tests: keep the last forward's tape in `self.last_tape` (tests/forced_replica.py)
         self.last_tape = None
         self.on_recompute = None  # tests: called as on_recompute(f0, f1, out, mr) with every chunk's recomputed CNN output and statistics
-        self.graph_relayout = True  # re-layout of the kernel-side weights after an optimizer step as one CUDA graph replay
-        self._rl_graph = None
-        self._rl_seen = 0
-        cfg = self.net.cfg
-        h = cfg.hidsize
-        # columns of the attention's input gradient: q | k | v, and R (10 basis rows per head) with the clipped_causal mask, padded to 8
-        self.kcat = (3 * h + 10 * cfg.heads + 7) // 8 * 8 if cfg.mask_style == "clipped_causal" else 3 * h
-        pol = policy
-        self.ntot = 0 if pol is None else sum(getattr(pol.pi_head, name).linear_layer.weight.shape[0] for name in pol.head_specs)  # action logits
         self.ld_logits = (sum(lin.weight.shape[0] for lin in self._head_layers()) + 7) // 8 * 8  # columns of the logits gradient
 
     def _head_layers(self):
@@ -116,89 +105,6 @@ class _Trainer:
         g = g.reshape(p.shape).to(F32)
         prev = self._sink.get(id(p))
         self._sink[id(p)] = g if prev is None else prev + g
-
-    # -- backward-side weight layouts (re-made whenever a parameter changes, like policy._Prepared) -------------------
-    def _weights_fp(self):
-        """Versions of the parameters the kernel-layout copies are made from: all but the EWMA normaliser, which an RL step updates on
-        every call and which no copy holds (`denormalize` keys it itself)."""
-        mod = self.net if self.policy is None else self.policy
-        return tuple((p.data_ptr(), p._version) for n, p in mod.named_parameters() if not n.startswith("value_head.normalizer."))
-
-    def _weights(self):
-        fp = self._weights_fp()
-        if self._wprep is not None and fp == self._wprep_fp:
-            return self._wprep
-        with torch.no_grad():
-            self._wprep = self._build_weights()
-        self._wprep_fp = fp
-        return self._wprep
-
-    def refresh_weights(self):
-        """Re-layout of every kernel-side weight copy (forward folds of policy._Prepared + the heads, backward transposes of
-        `_build_weights`) after an optimizer step.  Eagerly this is ~500 small torch launches;
-        the parameters live at fixed addresses (FlatAdamDP's flat bucket), so from the second refresh on the whole re-layout is ONE captured
-        CUDA graph replay writing the same kernel-layout tensors in place.  Called by `loss_and_grad`; a no-op when nothing changed."""
-        pol, net = self.policy, self.net
-        if pol is None:
-            return  # a bare network: the lazy eager paths rebuild on use
-        from .policy import _Prepared, _fingerprint
-        fp_net, fp_heads = _fingerprint(net), pol._heads_fp()
-        fp_all = self._weights_fp()
-        if net._prep is not None and net._prep_fp == fp_net and pol._hprep is not None and pol._hprep_fp == fp_heads and self._wprep is not None \
-                and self._wprep_fp == fp_all:
-            return
-        ptrs = tuple(p.data_ptr() for p in pol.parameters())
-        if not self.graph_relayout or not all(p.is_cuda for p in pol.parameters()):
-            return  # the lazy eager paths (prepared() / _heads_prepared() / _weights()) rebuild on use
-        if self._rl_graph is not None and self._rl_graph[0] != ptrs:
-            self._rl_graph = None  # the parameters moved (e.g. .to(), a new optimizer bucket): capture again
-        if self._rl_graph is None:
-            self._rl_seen += 1
-            if self._rl_seen < 2:
-                return  # first change: eager (also warms up every lazily initialised helper before capture)
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            with torch.no_grad(), torch.cuda.graph(g):
-                prep = _Prepared(net.cfg, dict(net.named_parameters()))
-                hprep = pol._build_heads_prepared()
-                wprep = self._build_weights()
-            self._rl_graph = (ptrs, g, prep, hprep, wprep)
-        _, g, prep, hprep, wprep = self._rl_graph
-        g.replay()
-        net._prep, net._prep_fp = prep, fp_net
-        pol._hprep, pol._hprep_fp = hprep, fp_heads
-        self._wprep, self._wprep_fp = wprep, fp_all
-
-    def _build_weights(self):
-        """The dgrad weights of every layer the backward runs through (builds weights only: it also runs inside the graph capture)."""
-        net = self.net
-        cfg = net.cfg
-        P = dict(net.named_parameters())
-        w = dict(stacks=[], layers=[])
-        pfx = "img_process.cnn"
-        for i in range(len(cfg.chans)):
-            s = f"{pfx}.stacks.{i}"
-            st = dict(convs=[_rot(P[f"{s}.blocks.{j}.conv{k}.layer.weight"]) for j in range(2) for k in range(2)])
-            if i > 0 or cfg.first_conv_norm:  # (stack 0's plain first conv has its own backward kernel, ops.firstconv_bwd)
-                st["first"] = _rot(P[f"{s}.firstconv.layer.weight"])
-            w["stacks"].append(st)
-        perm = lambda v: _dense_to_zp(v.detach(), cfg)
-        w["dense_t"] = _tr(perm(P[f"{pfx}.dense.layer.weight"]))
-        w["dense_g"] = perm(P[f"{pfx}.dense.norm.weight"]).float().contiguous()
-        w["dense_b"] = perm(P[f"{pfx}.dense.norm.bias"]).float().contiguous()
-        w["linear_t"] = _tr(P["img_process.linear.layer.weight"])
-        qkvr = ("q", "k", "v", "r") if cfg.mask_style == "clipped_causal" else ("q", "k", "v")  # R only where the mask has a band
-        for l in range(cfg.n_layers):
-            o = f"recurrent_layer.blocks.{l}.r.orc_block"
-            b = f"recurrent_layer.blocks.{l}"
-            cat = torch.cat([P[f"{o}.{c}_layer.weight"] for c in qkvr], 0)
-            w["layers"].append(dict(qkvr_t=_tr(cat, self.kcat), proj_t=_tr(P[f"{o}.proj_layer.weight"]), mlp0_t=_tr(P[f"{b}.mlp0.layer.weight"]),
-                                    mlp1_t=_tr(P[f"{b}.mlp1.layer.weight"])))
-        if self.use_lastlayer:
-            w["last_t"] = _tr(P["lastlayer.layer.weight"])
-        if self._head_layers():
-            w["heads_t"] = _tr(torch.cat([lin.weight for lin in self._head_layers()], 0), self.ld_logits)
-        return w
 
     # -- generic pieces -------------------------------------------------------------------------------------------------
     @staticmethod
@@ -268,16 +174,18 @@ class _Trainer:
 
     def _taped_latent(self, img, first, state_in):
         """The network's inference kernels, recording what the backward needs -> (latent bf16 [N][h], latent fp32 (B,t,h), tape, state_out).
-        The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`)."""
-        net = self.net
+        The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`, `heads_t`)."""
+        net, pol = self.net, self.policy
         self.check_call_frames(img)
-        self.refresh_weights()
-        wts = self._weights()
+        if pol is not None:
+            pol.refresh_weights()  # (a bare network: the getters rebuild eagerly on use)
+        layers = self._head_layers()
         state_in = [(m, (k.detach(), v.detach())) for (m, (k, v)) in state_in]  # behavioural_cloning.py:111
-        tape = dict(stacks=[], blocks=[], wts=wts, recompute=self.recompute_frames)
+        tape = dict(stacks=[], blocks=[], wts=net.prepared_backward(), heads_t=pol._heads_prepared_backward(layers) if layers else None,
+                    recompute=self.recompute_frames)
         net._tape = tape
         try:
-            lat_bf16, lat_f32, state_out = net._forward_impl(img, first, state_in, use_lastlayer=self.use_lastlayer)
+            lat_bf16, lat_f32, state_out = net._forward_impl(img, first, state_in)
         finally:
             net._tape = None
         if self.keep_tape:
@@ -307,7 +215,7 @@ class _Trainer:
             self._grad(lin.weight, dWh[c0:c0 + m])
             self._grad(lin.bias, dbh[c0:c0 + m])
             c0 += m
-        return self._gemm(dlog, tape["wts"]["heads_t"], self.net.cfg.hidsize)
+        return self._gemm(dlog, tape["heads_t"], self.net.cfg.hidsize)
 
     def _backward_from_dlat(self, dlat, tape, B, t, upper_grads_ready, dstate=None, want_dmem=None):
         """Everything below the latent (the output of final_ln): final_ln [, lastlayer], the transformer, img_process.linear, dense, the
@@ -320,13 +228,13 @@ class _Trainer:
         h = cfg.hidsize
         # ---------------- final_ln (plain norm) on lastlayer's output, or on relu(recurrent output) without lastlayer ----------------
         # (xl, z_last, x0, xd and the convs' h are ReLU outputs that feed a norm: their ReLU backward rides on that norm's apply pass)
-        if self.use_lastlayer:
+        if net.use_lastlayer:
             x, mr = tape["xl"], tape["mr_xl"]
         else:  # lib/policy.py:389-392: the last block's z, relu fused into its epilogue
             x, mr = tape["blocks"][-1]["z"], tape["blocks"][-1]["mr_z"]
         fg = P["final_ln.weight"]
         dx = self._norm_bwd(dlat, x, mr, fg.detach().float().contiguous(), 1, h, fg, P["final_ln.bias"], relu_x=True)
-        if self.use_lastlayer:
+        if net.use_lastlayer:
             dx = self._normlinear_bwd(dx, tape["z_last"], tape["mr_zl"], wts["last_t"], "lastlayer", P, relu_x=True)
         # ---------------- transformer blocks, last to first ----------------
         dmem = [None] * cfg.n_layers
@@ -416,7 +324,7 @@ class _Trainer:
         self._grad(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
         # attention: gradients wrt q | k | v | R side by side (one buffer = one dgrad GEMM + one wgrad GEMM for all four)
         causal = cfg.mask_style == "clipped_causal"
-        dqkvr = torch.zeros((N, self.kcat), dtype=BF16, device=dy.device)
+        dqkvr = torch.zeros((N, cfg.kcat), dtype=BF16, device=dy.device)
         dmem = None
         if causal and (dstate is not None or want_dmem):  # the KV memory is in the graph (the differentiable forward's state_grad)
             db_nd, dmem = ops.attention_bwd_state(S["q"], S["full_k"], S["full_v"], S["R"], P[f"{o}.b_nd"].detach().float().contiguous(), first_u8,
@@ -617,7 +525,7 @@ class RLTrainer(BCTrainer):
             count = N * dist.get_world_size()
         nz = pol.value_head.normalizer
         sq = ops.value_bwd(vpred.reshape(N), ret, sums, count, nz.running_mean, nz.running_mean_sq, nz.debiasing_term, self.ewma_beta,
-                           2.0 * vf_coef / N, dlog, self.ntot)
+                           2.0 * vf_coef / N, dlog, hp["ntot"])
         self.stats = dict(pi_loss=pi_loss.mean(), vf_loss=sq.mean(), kl_ref=kl.mean(), clipfrac=clipped.mean())
         loss = self.stats["pi_loss"] + vf_coef * self.stats["vf_loss"] + kl_coef * self.stats["kl_ref"]
         return loss, dlog
@@ -642,7 +550,6 @@ class IDMTrainer(_Trainer):
     (None, (B,0,h), (B,0,h))."""
 
     max_t = 128  # frames per sequence the unmasked attention backward supports
-    use_lastlayer = False  # the IDM's forward discards lastlayer's output (lib/policy.py:390-391)
 
     def __init__(self, policy: InverseActionPolicy, recompute_frames=None):
         if not isinstance(policy, InverseActionPolicy):
@@ -717,11 +624,10 @@ class _AutogradRunner(_Trainer):
     latent."""
 
     def __init__(self, module):
-        from .policy import InverseActionNet, _PolicyBase
+        from .policy import _PolicyBase
 
         pol = module if isinstance(module, _PolicyBase) else None
         super().__init__(pol, None if pol is not None else module)
-        self.use_lastlayer = not isinstance(self.net, InverseActionNet)  # the IDM's forward discards lastlayer's output
         self.module = module
 
     def _head_layers(self):
@@ -820,7 +726,7 @@ class _AutogradRunner(_Trainer):
             if all(g is None for g in grads):  # only the state_out feeds the loss: no head gradient, a zero d latent
                 return sink, self._backward_from_dlat(torch.zeros((N, h), dtype=BF16, device=tape["lat"].device), tape, B, t, None, dstate,
                                                       want_dmem)
-            hp_cols = pol._heads_prepared()["cols"]
+            hp = pol._heads_prepared()
             dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=tape["lat"].device)
             unused = []
             for i, (name, (shape, n)) in enumerate(pol.head_specs.items()):
@@ -828,7 +734,7 @@ class _AutogradRunner(_Trainer):
                 if grads[i] is None:
                     unused.append(lin)
                     continue
-                c0, width = hp_cols[name]
+                c0, width = hp["cols"][name]
                 g = grads[i].reshape(N, width).to(F32).contiguous()
                 ops.log_softmax_bwd(outs[i].reshape(N, width), g, 1.0 / pol.temperature, dlog, c0, width // n, tape["head_masks"].get(name))
             if pol.has_value_head:
@@ -836,7 +742,7 @@ class _AutogradRunner(_Trainer):
                 if gv is None:
                     unused.append(pol.value_head.linear)
                 else:
-                    dlog[:, self.ntot] = gv.reshape(N).to(BF16)  # d vpred: the value head's column (a strided copy of N values)
+                    dlog[:, hp["ntot"]] = gv.reshape(N).to(BF16)  # d vpred: the value head's column (a strided copy of N values)
             dlat = self._heads_bwd(dlog, tape["lat"], tape)
             del dlog
             dmem = self._backward_from_dlat(dlat, tape, B, t, None, dstate, want_dmem)
