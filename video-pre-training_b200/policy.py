@@ -495,12 +495,12 @@ class MinecraftPolicy(nn.Module):
     # -- CNN -----------------------------------------------------------------------------------------------
     # Activations are kept in the "ZP" layout [F][H+1][W+1][C] (zero last row / column; include/vpt_b200.h): it lets the
     # conv kernel address every 3x3 neighbour linearly and reuse one shared-memory input span for all nine taps.
-    def _cnn_chunk(self, img, prep: _Prepared, out, pfx="img_process.cnn", train=False, stacks=None):
+    def _cnn_chunk(self, img, prep: _Prepared, out, pfx="img_process.cnn", train=False, stacks=None, record_from=0):
         """lib/impala_cnn.py:187-195 for a chunk of frames; writes the last stack's output (ZP [F, Hf+1, Wf+1, C2] bf16) into
         `out` and returns (out, per-frame stats).
         train: the training layout (no stack-norm fold; each residual branch's output `r` kept apart, then `add_zp`), which the
         backward's recompute of a chunk reproduces bit for bit.  stacks: a list that receives, per stack, what the backward needs
-        (training layout only; None records nothing)."""
+        (training layout only; None records nothing), or None for the stacks below `record_from`, which the backward does not enter."""
         cfg = self.cfg
         H, W = cfg.img_shape[0], cfg.img_shape[1]
         x, mr = None, None
@@ -510,7 +510,7 @@ class MinecraftPolicy(nn.Module):
             self._tap("conv3d", x)
         for i, c in enumerate(cfg.chans):
             st = prep.stacks[i]
-            rec = dict(x_in=x, mr_in=mr, H_in=H, W_in=W, full=None, blocks=[]) if stacks is not None else None
+            rec = dict(x_in=x, mr_in=mr, H_in=H, W_in=W, full=None, blocks=[]) if stacks is not None and i >= record_from else None
             fold = self.fold_stack_norm and not train  # inference: the post-pool GroupNorm is folded into its two consumers
             if i == 0 and "fc_w" in st:
                 y1, mr1, chan = ops.firstconv_pool(img, st["fc_w"], st["fc_b"], c, zp=True, want_chan=True)
@@ -561,7 +561,7 @@ class MinecraftPolicy(nn.Module):
                         rec["blocks"].append(dict(h=hmid, mrh=mrh, r=r, x=x, mr=mr))
                     del r
                 self._tap(f"{pfx}.stacks.{i}.blocks.{j}", x)
-            if rec is not None:
+            if stacks is not None:
                 stacks.append(rec)
         return x, mr
 
@@ -628,9 +628,9 @@ class MinecraftPolicy(nn.Module):
         z, mr_z = self._linear(hmid, L["mlp1"], h, residual=y, relu=2 if last else 0, want_stats=True)
         if not last:
             self._tap(f"recurrent_layer.blocks.{l}", z)
-        if self._tape is not None:
+        if self._tape is not None:  # (None for a block below the backward's lowest unit)
             self._tape["blocks"].append(dict(x=x, mr_x=mr_x, xhat=xhat, q=q, full_k=full_k, full_v=full_v, R=R, smask=smask_u8, a=a, y=y,
-                                             mr_y=mr_y, hmid=hmid, z=z, mr_z=mr_z))
+                                             mr_y=mr_y, hmid=hmid, z=z, mr_z=mr_z) if l >= self._tape["blocks_from"] else None)
         return z, mr_z, (new_mask, (new_k, new_v))
 
     # -- whole net -------------------------------------------------------------------------------------------
@@ -663,9 +663,11 @@ class MinecraftPolicy(nn.Module):
         mrs = []
         tape = self._tape
         # training forward: tape["recompute"] None keeps every stack's activations for the backward (one CNN pass per call); an integer
-        # runs the CNN in chunks of that many frames, records nothing per stack, and the backward re-runs each chunk (training.py)
+        # runs the CNN in chunks of that many frames, records nothing per stack, and the backward re-runs each chunk (training.py).
+        # Only the stacks from tape["stacks_from"] on are recorded: with the CNN frozen none, and the call may hold several chunks.
         recompute = None if tape is None else tape.get("recompute")
-        stacks = tape["stacks"] if tape is not None and recompute is None else None
+        cnn_bwd = tape is not None and tape["stacks_from"] < len(cfg.chans)
+        stacks = tape["stacks"] if cnn_bwd and recompute is None else None
         if cfg.conv3d_out is None:
             step = self.cnn_chunk_frames if recompute is None else min(recompute, self.cnn_chunk_frames)
         else:  # chunks of whole sequences; the IDM's 128-channel full-resolution stage is ~13 MiB/frame
@@ -673,16 +675,17 @@ class MinecraftPolicy(nn.Module):
         for f0 in range(0, N, step):
             F_ = min(step, N - f0)
             chunk = frames[f0:f0 + F_] if cfg.conv3d_out is None else frames[f0:f0 + F_].view(F_ // t, t, *frame_shape)
-            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_], train=tape is not None, stacks=stacks)
+            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_], train=tape is not None, stacks=stacks,
+                                    record_from=0 if tape is None else tape["stacks_from"])
             mrs.append(mr)
         mr_c = mrs[0] if len(mrs) == 1 else torch.cat(mrs, 0)
         Kd = (Hf + 1) * (Wf + 1) * C2  # ZP rows flattened; the zero row / column meets zero weight columns
         xd, mr_d = self._linear(cnn_out.view(N, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
         if tape is not None:
-            if recompute is None and len(mrs) != 1:
+            if cnn_bwd and recompute is None and len(mrs) != 1:
                 raise NotImplementedError(f"training forward: at most {step} frames per call (got {N})")
             tape.update(prep=prep, frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d,
-                        cnn_chunks=[(f0, min(f0 + step, N)) for f0 in range(0, N, step)])
+                        cnn_chunks=[(f0, min(f0 + step, N)) for f0 in range(0, N, step)] if cnn_bwd else [])
         del cnn_out
         self._tap("img_process.cnn.dense", xd)
         x, mr_x = self._linear(xd, prep.linear, cfg.hidsize, mr=mr_d, relu=1, want_stats=True)
@@ -800,7 +803,11 @@ class _PolicyBase(nn.Module):
         before back-propagating through it.  That costs one more CNN forward per call and frees the CNN activations, nearly all of a
         call's tape (20.7 MiB per frame at 2x width with its backward workspace, measured on an H100: README), so a call or a BPTT window can hold many more frames:
         up to `training._Trainer.max_call_frames` per call.  The gradients are those of the stored tape (bit-identical when one chunk
-        holds the call).  None keeps the activations (faster when they fit)."""
+        holds the call).  None keeps the activations (faster when they fit).
+
+        Frozen parameters (requires_grad=False when the forward runs) get no gradient and the backward skips the work that only served
+        them, stopping at the lowest unit that trains; with the ImpalaCNN frozen the forward keeps none of its activations and the
+        stored-tape frame limit does not apply."""
         recompute_frames = check_recompute_frames(recompute_frames)
         self._autograd = bool(on)
         self._state_grad = bool(on) and bool(state_grad)

@@ -17,6 +17,12 @@ The ImpalaCNN's activations are nearly all of a call's tape.  With `recompute_fr
 forward keeps only the CNN's output and the backward re-runs the CNN chunk by chunk (`_recompute_cnn`), back-propagating through each
 chunk before making the next; without it the forward's tape is the one chunk.
 
+Only the parameters that require grad when the forward runs train (`_grad_plan`): a frozen parameter gets no gradient (its `.grad` is
+left as it is), its weight-side work (`wgrad`, the norms' column sums, d b_nd, the head columns) is not done, and the backward stops at
+the lowest unit of `_grad_units` that needs a gradient, without that unit's input gradient.  The forward records only what that backward
+reads: with the ImpalaCNN frozen no per-stack activation at all, so the stored tape no longer bounds a call's frames.  With every
+parameter trainable the same kernels run in the same order as without the rule.
+
 The differentiable forward (`set_autograd`, `_AutogradRunner` at the end of this file) runs the same taped forward and enters the same
 backward at dlog (any loss over pd / vpred, through `ops.log_softmax_bwd`) or at d latent (a bare network); its gradients go to a sink
 that hands them back to autograd instead of `param.grad`.
@@ -55,6 +61,26 @@ def _tr(W, pad_to=None):
     return Wt.contiguous()
 
 
+def _grad_units(net):
+    """The backward's units in forward order, each a tuple of parameter-name prefixes of `net` (the heads come after the last one).  A
+    unit's input gradient is computed only when a unit below it needs a gradient."""
+    cfg = net.cfg
+    units = [("conv3d_layer.",)] if cfg.conv3d_out is not None else []
+    for i in range(len(cfg.chans)):
+        s = f"img_process.cnn.stacks.{i}"
+        units += [(f"{s}.firstconv.",), (f"{s}.n.",)] + [(f"{s}.blocks.{j}.conv{k}.",) for j in range(2) for k in range(2)]
+    units += [("img_process.cnn.dense.",), ("img_process.linear.",)]
+    for l in range(cfg.n_layers):
+        b = f"recurrent_layer.blocks.{l}"
+        o = f"{b}.r.orc_block"
+        units += [(f"{b}.pre_r_ln.",), tuple(f"{o}.{c}_layer." for c in "qkvr"), (f"{o}.b_nd",), (f"{o}.proj_layer.",), (f"{b}.mlp0.",),
+                  (f"{b}.mlp1.",)]
+    if net.use_lastlayer:
+        units.append(("lastlayer.",))
+    units.append(("final_ln.",))
+    return units
+
+
 def _acc(p, g):
     """p.grad += g (allocating on first use), like autograd's accumulation."""
     g = g.reshape(p.shape)
@@ -91,14 +117,53 @@ class _Trainer:
         self.last_tape = None
         self.on_recompute = None  # tests: called as on_recompute(f0, f1, out, mr) with every chunk's recomputed CNN output and statistics
         self.ld_logits = (sum(lin.weight.shape[0] for lin in self._head_layers()) + 7) // 8 * 8  # columns of the logits gradient
+        self._units = _grad_units(self.net)
+        self._pos = {u[0]: i for i, u in enumerate(self._units)}  # a unit's first prefix -> its place in forward order
+        self._train, self._lowest = frozenset(), len(self._units) + 1  # the running backward's `_grad_plan` (set from its tape)
 
     def _head_layers(self):
         """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order."""
         pol = self.policy
         return [] if pol is None else [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
 
+    def _grad_plan(self, want_dmem=None):
+        """What the backward of a forward starting now does, from the parameters' `requires_grad` (and, with `state_grad`, from whether
+        each layer's state_in K / V gradient is wanted) -> dict(train: ids of the parameters that train, lowest: the place in
+        `_grad_units` order of the lowest unit that needs a gradient (the heads: len(units); nothing: len(units) + 1), stacks_from /
+        blocks_from: the first CNN stack / transformer block whose activations the backward reads (their count: none), cnn: whether
+        the backward enters the CNN)."""
+        net, cfg, units = self.net, self.net.cfg, self._units
+        train = frozenset(id(p) for p in (net if self.policy is None else self.policy).parameters() if p.requires_grad)
+        names = tuple(n for n, p in net.named_parameters() if id(p) in train)
+        lowest = next((i for i, u in enumerate(units) if any(n.startswith(u) for n in names)), len(units) + 1)
+        if lowest > len(units) and any(id(p) in train for lin in self._head_layers() for p in (lin.weight, lin.bias)):
+            lowest = len(units)
+        for l, want in enumerate(want_dmem or ()):
+            if want:  # the attention backward of layer l gives its state_in gradient
+                lowest = min(lowest, self._pos[f"recurrent_layer.blocks.{l}.r.orc_block.b_nd"])
+        nst = len(cfg.chans)
+        stacks_from = next((i for i in range(nst) if lowest <= self._pos[f"img_process.cnn.stacks.{i}.blocks.1.conv1."]), nst)
+        blocks_from = next((l for l in range(cfg.n_layers) if lowest <= self._pos[f"recurrent_layer.blocks.{l}.mlp1."]), cfg.n_layers)
+        if not net.use_lastlayer and lowest <= self._pos["final_ln."]:
+            blocks_from = min(blocks_from, cfg.n_layers - 1)  # final_ln reads the last block's output
+        return dict(train=train, lowest=lowest, stacks_from=stacks_from, blocks_from=blocks_from, cnn=stacks_from < nst)
+
+    def _use_plan(self, tape):
+        self._train, self._lowest = tape["train"], tape["lowest"]
+
+    def _trains(self, p):
+        """Whether parameter p trains in the running backward."""
+        return id(p) in self._train
+
+    def _below(self, prefix):
+        """Whether a unit below the one whose first prefix is `prefix` needs a gradient, i.e. whether that unit's input gradient is needed."""
+        return self._lowest < self._pos[prefix]
+
     def _grad(self, p, g):
-        """Hands the gradient g of parameter p to the sink: `p.grad` (accumulated, `_acc`) or the dict of the differentiable forward."""
+        """Hands the gradient g of parameter p to the sink: `p.grad` (accumulated, `_acc`) or the dict of the differentiable forward.
+        Nothing for a frozen parameter."""
+        if not self._trains(p):
+            return
         if self._sink is None:
             _acc(p, g)
             return
@@ -122,105 +187,138 @@ class _Trainer:
             self._grad(weight_param, dW)
         return dW
 
-    def _norm_bwd(self, du, x, mr, gamma, rows_per_group, count, g_param, b_param, grad_map=None, zp=None, add=None, relu_x=False):
+    def _norm_bwd(self, du, x, mr, gamma, rows_per_group, count, g_param, b_param, grad_map=None, zp=None, add=None, relu_x=False,
+                  want_dx=True):
         """Backward of n = (x - mean) * rstd, u = gamma * n + beta given du: accumulates dgamma / dbeta into `g_param` / `b_param`
-        (through `grad_map` when the kernel-side gamma has another layout), returns dx (+ add).
+        (through `grad_map` when the kernel-side gamma has another layout), returns dx (+ add), or None without `want_dx`.
         relu_x: x is the output of a ReLU whose backward is applied to the result in the same pass."""
         if rows_per_group > 1:  # GroupNorm frames: column sums and group sums share one pass over (du, x)
             cs, ms = ops.norm_sums(du, x, mr, gamma, rows_per_group, count)
         else:
-            cs = ops.col_sums(du, x, mr, rows_per_group)
-            ms = ops.group_sums(du, x, mr, gamma, rows_per_group, count)
-        self._grad(g_param, cs[0] if grad_map is None else grad_map(cs[0]))
-        self._grad(b_param, cs[1] if grad_map is None else grad_map(cs[1]))
+            cs = ops.col_sums(du, x, mr, rows_per_group) if self._trains(g_param) or self._trains(b_param) else None
+            ms = ops.group_sums(du, x, mr, gamma, rows_per_group, count) if want_dx else None
+        for p, c in ((g_param, 0), (b_param, 1)):
+            if self._trains(p):
+                self._grad(p, cs[c] if grad_map is None else grad_map(cs[c]))
+        if not want_dx:
+            return None
         return ops.norm_bwd_apply(du, x, mr, gamma, ms, rows_per_group, zp=zp, add=add, relu_x=relu_x)
 
     def _normconv_bwd(self, dz, x, mr, H, W, W_rot, names, P, add=None, relu_x=False):
         """dz: gradient wrt the conv output (ReLU already applied), ZP [F,H+1,W+1,Cout]; x: the layer input (ZP, pre-norm).
-        Accumulates the weight / norm gradients and returns the gradient wrt x (+ add)."""
+        Accumulates the weight / norm gradients and returns the gradient wrt x (+ add), or None when no unit below needs it."""
         Fn, Cin, Cout = x.shape[0], x.shape[3], dz.shape[3]
         R = Fn * (H + 1) * (W + 1)
-        gam, bet = P[names + ".norm.weight"], P[names + ".norm.bias"]
+        gam, bet, wt = P[names + ".norm.weight"], P[names + ".norm.bias"], P[names + ".layer.weight"]
+        want_dx = self._below(names + ".")
+        norm = want_dx or self._trains(gam) or self._trains(bet)
         g32 = gam.detach().float().contiguous()
-        du, _ = ops.conv3x3_zp(dz, W_rot, H, W, relu=0, want_stats=False)
-        u, _ = ops.affine_norm_zp(x, mr, g32, bet.detach().float().contiguous())
-        shifts = [(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)]
-        dWk = ops.wgrad(dz.view(R, Cout), u.view(R, Cin), shifts)  # [Cout][tap][Cin]
-        del u
-        self._grad(P[names + ".layer.weight"], dWk.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
-        return self._norm_bwd(du.view(R, Cin), x.view(R, Cin), mr, g32, (H + 1) * (W + 1), H * W * Cin, gam, bet,
-                              zp=(H, W, Cin), add=None if add is None else add.view(R, Cin), relu_x=relu_x).view(x.shape)
+        du = ops.conv3x3_zp(dz, W_rot, H, W, relu=0, want_stats=False)[0] if norm else None
+        if self._trains(wt):
+            u, _ = ops.affine_norm_zp(x, mr, g32, bet.detach().float().contiguous())
+            shifts = [(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)]
+            dWk = ops.wgrad(dz.view(R, Cout), u.view(R, Cin), shifts)  # [Cout][tap][Cin]
+            del u
+            self._grad(wt, dWk.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
+        if not norm:
+            return None
+        dx = self._norm_bwd(du.view(R, Cin), x.view(R, Cin), mr, g32, (H + 1) * (W + 1), H * W * Cin, gam, bet,
+                            zp=(H, W, Cin), add=None if add is None else add.view(R, Cin), relu_x=relu_x, want_dx=want_dx)
+        return None if dx is None else dx.view(x.shape)
 
     def _normlinear_bwd(self, dz, x, mr, Wt, names, P, add=None, relu_x=False):
-        """[LayerNorm ->] Linear backward; dz [rows][out] is the gradient wrt the GEMM output (after ReLU masking)."""
-        gam, bet = P[names + ".norm.weight"], P[names + ".norm.bias"]
+        """[LayerNorm ->] Linear backward; dz [rows][out] is the gradient wrt the GEMM output (after ReLU masking).  Returns the gradient
+        wrt x (+ add), or None when no unit below needs it."""
+        gam, bet, wt = P[names + ".norm.weight"], P[names + ".norm.bias"], P[names + ".layer.weight"]
+        want_dx = self._below(names + ".")
+        norm = want_dx or self._trains(gam) or self._trains(bet)
         g32, b32 = gam.detach().float().contiguous(), bet.detach().float().contiguous()
-        du = self._gemm(dz, Wt, Wt.shape[0])
-        u, _, _ = ops.affine_norm(x, mr, g32, b32, rows_per_group=1)
-        self._wgrad_linear(dz, u, P[names + ".layer.weight"])
-        del u
-        return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], gam, bet, add=add, relu_x=relu_x)
+        du = self._gemm(dz, Wt, Wt.shape[0]) if norm else None
+        if self._trains(wt):
+            u, _, _ = ops.affine_norm(x, mr, g32, b32, rows_per_group=1)
+            self._wgrad_linear(dz, u, wt)
+            del u
+        if not norm:
+            return None
+        return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], gam, bet, add=add, relu_x=relu_x, want_dx=want_dx)
 
     # -- the step ---------------------------------------------------------------------------------------------------------
-    def check_call_frames(self, img):
-        """With `recompute_frames`: the per-call limits (`max_call_frames`, `max_call_batch`), checked before any work so that a call that
-        cannot finish accumulates nothing.  (The stored tape's limits are checked by the trainers and the differentiable forward.)"""
-        if self.recompute_frames is None:
+    def check_call_frames(self, img, plan=None):
+        """With `recompute_frames`, or when the backward does not enter the CNN (`plan`, default `_grad_plan()`): the per-call limits
+        (`max_call_frames`, `max_call_batch`), checked before any work so that a call that cannot finish accumulates nothing.  (The stored
+        tape's limits are checked by the trainers and the differentiable forward.)"""
+        if self.recompute_frames is None and (plan or self._grad_plan())["cnn"]:
             return
         B, t = img.shape[:2]
         if B * t > self.max_call_frames or B > self.max_call_batch:
             raise NotImplementedError(f"{type(self).__name__}: at most {self.max_call_frames} frames and B <= {self.max_call_batch} per call "
                                       f"(got B = {B}, T = {t})")
 
-    def _taped_latent(self, img, first, state_in):
+    def _taped_latent(self, img, first, state_in, want_dmem=None):
         """The network's inference kernels, recording what the backward needs -> (latent bf16 [N][h], latent fp32 (B,t,h), tape, state_out).
-        The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`, `heads_t`)."""
+        The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`, `heads_t`), and
+        the backward's `_grad_plan` (want_dmem: see there)."""
         net, pol = self.net, self.policy
-        self.check_call_frames(img)
+        tape = self._grad_plan(want_dmem)
+        self.check_call_frames(img, tape)
         if pol is not None:
             pol.refresh_weights()  # (a bare network: the getters rebuild eagerly on use)
         layers = self._head_layers()
         state_in = [(m, (k.detach(), v.detach())) for (m, (k, v)) in state_in]  # behavioural_cloning.py:111
-        tape = dict(stacks=[], blocks=[], wts=net.prepared_backward(), heads_t=pol._heads_prepared_backward(layers) if layers else None,
+        tape.update(stacks=[], blocks=[], wts=net.prepared_backward(), heads_t=pol._heads_prepared_backward(layers) if layers else None,
                     recompute=self.recompute_frames)
         net._tape = tape
         try:
             lat_bf16, lat_f32, state_out = net._forward_impl(img, first, state_in)
         finally:
             net._tape = None
+        if tape["lowest"] > self._pos["img_process.cnn.dense."]:  # the backward stops above the dense layer, which alone reads cnn_out
+            tape.update(cnn_out=None, mr_c=None)
         if self.keep_tape:
             self.last_tape = tape
         return lat_bf16, lat_f32, tape, state_out
 
-    def _taped_forward(self, img, first, state_in, mask=None):
+    def _taped_forward(self, img, first, state_in, mask=None, want_dmem=None):
         """The inference kernels, recording what the backward needs -> (latent bf16, pd, vpred, tape, state_out)."""
         B, t = img.shape[:2]
-        lat_bf16, _, tape, state_out = self._taped_latent(img, first, state_in)
+        lat_bf16, _, tape, state_out = self._taped_latent(img, first, state_in, want_dmem)
         pd, vpred = self.policy._heads(lat_bf16, B, t, mask)
         return lat_bf16, pd, vpred, tape, state_out
 
     def _backward_from_dlog(self, dlog, lat_bf16, tape, B, t, upper_grads_ready):
-        """Everything below the logits: the head weights (`_heads_bwd`), then `_backward_from_dlat`."""
-        dlat = self._heads_bwd(dlog, lat_bf16, tape)
+        """Everything below the logits: the head weights (`_heads_bwd`), then `_backward_from_dlat` when a unit below the heads trains.
+        dlog may be None when nothing trains."""
+        dlat = None if dlog is None else self._heads_bwd(dlog, lat_bf16, tape)
         del dlog
-        self._backward_from_dlat(dlat, tape, B, t, upper_grads_ready)
+        if dlat is not None:
+            self._backward_from_dlat(dlat, tape, B, t, upper_grads_ready)
+        elif upper_grads_ready is not None:
+            upper_grads_ready()
 
     def _heads_bwd(self, dlog, lat_bf16, tape):
-        """The head weights' gradients from dlog bf16 [N][ld_logits] (one column block per `_head_layers()` entry) -> d latent bf16 [N][h]."""
-        dWh = ops.wgrad(dlog, lat_bf16)
-        dbh = ops.col_sums(dlog)[1]
+        """The head weights' gradients from dlog bf16 [N][ld_logits] (one column block per `_head_layers()` entry) -> d latent bf16 [N][h],
+        or None when nothing below the heads trains."""
+        self._use_plan(tape)
+        layers = self._head_layers()
+        dWh = ops.wgrad(dlog, lat_bf16) if any(self._trains(lin.weight) for lin in layers) else None
+        dbh = ops.col_sums(dlog)[1] if any(self._trains(lin.bias) for lin in layers) else None
         c0 = 0
-        for lin in self._head_layers():
+        for lin in layers:
             m = lin.weight.shape[0]
-            self._grad(lin.weight, dWh[c0:c0 + m])
-            self._grad(lin.bias, dbh[c0:c0 + m])
+            if self._trains(lin.weight):
+                self._grad(lin.weight, dWh[c0:c0 + m])
+            if self._trains(lin.bias):
+                self._grad(lin.bias, dbh[c0:c0 + m])
             c0 += m
-        return self._gemm(dlog, tape["heads_t"], self.net.cfg.hidsize)
+        return self._gemm(dlog, tape["heads_t"], self.net.cfg.hidsize) if self._lowest < len(self._units) else None
 
     def _backward_from_dlat(self, dlat, tape, B, t, upper_grads_ready, dstate=None, want_dmem=None):
         """Everything below the latent (the output of final_ln): final_ln [, lastlayer], the transformer, img_process.linear, dense, the
         ImpalaCNN and, for the IDM, the conv3d pre-stage.  dstate: None or per layer None / (dk, dv), the gradient wrt that layer's
-        state_out K / V; want_dmem: None or per layer whether its state_in gradient is wanted.  Returns per layer (dmem_k, dmem_v) or None."""
+        state_out K / V; want_dmem: None or per layer whether its state_in gradient is wanted.  Returns per layer (dmem_k, dmem_v) or None.
+        Each stage runs only while a unit at or below it needs a gradient (`_grad_plan`); `upper_grads_ready` is called once, before the
+        CNN or, when the backward does not enter it, at its end."""
+        self._use_plan(tape)
         net = self.net
         cfg = net.cfg
         wts = tape["wts"]
@@ -228,33 +326,38 @@ class _Trainer:
         h = cfg.hidsize
         # ---------------- final_ln (plain norm) on lastlayer's output, or on relu(recurrent output) without lastlayer ----------------
         # (xl, z_last, x0, xd and the convs' h are ReLU outputs that feed a norm: their ReLU backward rides on that norm's apply pass)
-        if net.use_lastlayer:
-            x, mr = tape["xl"], tape["mr_xl"]
-        else:  # lib/policy.py:389-392: the last block's z, relu fused into its epilogue
-            x, mr = tape["blocks"][-1]["z"], tape["blocks"][-1]["mr_z"]
-        fg = P["final_ln.weight"]
-        dx = self._norm_bwd(dlat, x, mr, fg.detach().float().contiguous(), 1, h, fg, P["final_ln.bias"], relu_x=True)
-        if net.use_lastlayer:
+        dx = None
+        if self._lowest <= self._pos["final_ln."]:
+            if net.use_lastlayer:
+                x, mr = tape["xl"], tape["mr_xl"]
+            else:  # lib/policy.py:389-392: the last block's z, relu fused into its epilogue
+                x, mr = tape["blocks"][-1]["z"], tape["blocks"][-1]["mr_z"]
+            fg = P["final_ln.weight"]
+            dx = self._norm_bwd(dlat, x, mr, fg.detach().float().contiguous(), 1, h, fg, P["final_ln.bias"], relu_x=True,
+                                want_dx=self._below("final_ln."))
+        if dx is not None and net.use_lastlayer:
             dx = self._normlinear_bwd(dx, tape["z_last"], tape["mr_zl"], wts["last_t"], "lastlayer", P, relu_x=True)
         # ---------------- transformer blocks, last to first ----------------
         dmem = [None] * cfg.n_layers
         for l in reversed(range(cfg.n_layers)):
+            if dx is None:
+                break
             dx, dmem[l] = self._block_bwd(l, dx, tape["blocks"][l], tape["first_u8"], wts["layers"][l], P, B, t,
                                           dstate=None if dstate is None else dstate[l], want_dmem=bool(want_dmem and want_dmem[l]))
         # ---------------- img_process.linear, dense ----------------
-        dz = self._normlinear_bwd(dx, tape["xd"], tape["mr_d"], wts["linear_t"], "img_process.linear", P, relu_x=True)
-        dcnn = self._dense_bwd(dz, tape, wts, P)
+        dz = None if dx is None else self._normlinear_bwd(dx, tape["xd"], tape["mr_d"], wts["linear_t"], "img_process.linear", P, relu_x=True)
+        dcnn = None if dz is None else self._dense_bwd(dz, tape, wts, P)
         if upper_grads_ready is not None:
             upper_grads_ready()
         # ---------------- ImpalaCNN, last stack to first, chunk by chunk (last chunk first) ----------------
         # The stored tape is the one-chunk case: its per-stack activations come from the forward.  With `recompute` every chunk's are made
-        # again from the frames and the forward's weights, used, and dropped before the next chunk.
+        # again from the frames and the forward's weights, used, and dropped before the next chunk.  (No chunk when the CNN is frozen.)
         frames = tape["frames"]
         for f0, f1 in reversed(tape["cnn_chunks"]):
             ct = tape if tape["recompute"] is None else self._recompute_cnn(tape, f0, f1, t)
             dx3 = self._cnn_bwd(dcnn[f0:f1], ct, wts, P)
             del ct
-            if cfg.conv3d_out is not None:
+            if cfg.conv3d_out is not None and dx3 is not None:
                 # the IDM's conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
                 C3 = cfg.conv3d_out
                 dW3, db3 = ops.conv3d_t5_bwd(frames[f0:f1].view((f1 - f0) // t, t, *frames.shape[1:]), dx3, C3)
@@ -266,7 +369,7 @@ class _Trainer:
 
     def _recompute_cnn(self, tape, f0, f1, t):
         """The forward of CNN chunk [f0, f1) again, in the training layout with the kernel-layout weights the forward used (tape["prep"]),
-        recording what `_cnn_bwd` needs -> that chunk's tape.  The kernels are deterministic, so this is the forward's chunk bit for bit."""
+        recording what `_cnn_bwd` needs (the stacks from tape["stacks_from"] on) -> that chunk's tape.  The kernels are deterministic, so this is the forward's chunk bit for bit."""
         net = self.net
         cfg = net.cfg
         frames = tape["frames"][f0:f1]
@@ -275,7 +378,7 @@ class _Trainer:
         out = torch.empty((f1 - f0, Hf + 1, Wf + 1, cfg.chans[-1]), dtype=BF16, device=frames.device)
         stacks = []
         with torch.no_grad():
-            _, mr = net._cnn_chunk(img, tape["prep"], out, train=True, stacks=stacks)
+            _, mr = net._cnn_chunk(img, tape["prep"], out, train=True, stacks=stacks, record_from=tape["stacks_from"])
         if self.on_recompute is not None:
             self.on_recompute(f0, f1, out, mr)
         return dict(stacks=stacks, prep=tape["prep"], frames=frames)
@@ -288,40 +391,58 @@ class _Trainer:
         Kd = (Hf + 1) * (Wf + 1) * C2
         x = tape["cnn_out"].view(N, Kd)
         pfx = "img_process.cnn.dense"
-        du = self._gemm(dz, wts["dense_t"], Kd)
-        u, _, _ = ops.affine_norm(x, tape["mr_c"], wts["dense_g"], wts["dense_b"], rows_per_group=1)
-        dWz = self._wgrad_linear(dz, u)  # [out][Kd] in ZP column order
-        del u
+        gam, bet, wt = P[pfx + ".norm.weight"], P[pfx + ".norm.bias"], P[pfx + ".layer.weight"]
+        want_dx = self._below(pfx + ".")
+        norm = want_dx or self._trains(gam) or self._trains(bet)
+        du = self._gemm(dz, wts["dense_t"], Kd) if norm else None
         unperm = lambda v: _dense_from_zp(v, cfg)
-        self._grad(P[pfx + ".layer.weight"], unperm(dWz))
-        del dWz
-        return self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, P[pfx + ".norm.weight"], P[pfx + ".norm.bias"],
-                              grad_map=unperm, zp=(Hf, Wf, C2)).view(N, Hf + 1, Wf + 1, C2)
+        if self._trains(wt):
+            u, _, _ = ops.affine_norm(x, tape["mr_c"], wts["dense_g"], wts["dense_b"], rows_per_group=1)
+            dWz = self._wgrad_linear(dz, u)  # [out][Kd] in ZP column order
+            del u
+            self._grad(wt, unperm(dWz))
+            del dWz
+        if not norm:
+            return None
+        dx = self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, gam, bet, grad_map=unperm, zp=(Hf, Wf, C2), want_dx=want_dx)
+        return None if dx is None else dx.view(N, Hf + 1, Wf + 1, C2)
 
     def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t, dstate=None, want_dmem=False):
         """Backward of lib/util.py:193-211 (see policy.MinecraftPolicy._block for the forward in the same notation) -> (d block input,
         (dmem_k, dmem_v) or None).  dstate: None or (dk, dv), the gradient wrt the layer's state_out K / V (either None); want_dmem: return
-        the gradient wrt its state_in K / V (lib/xf.py:366-391 builds the memory with cat and slicing, so autograd reaches it)."""
+        the gradient wrt its state_in K / V (lib/xf.py:366-391 builds the memory with cat and slicing, so autograd reaches it).  The d block
+        input is None when no unit below the block needs it; the backward then stops at the lowest unit of the block that needs a gradient."""
         cfg = self.net.cfg
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
         b = f"recurrent_layer.blocks.{l}"
         o = f"{b}.r.orc_block"
         N = B * t
         nr = 10 * heads
+        trains = self._trains
         dz = dzo  # (last block: z is relu(..) (lib/policy.py:211 fused into its epilogue); the norm backward above already masked dzo)
         # mlp1: z = y + hmid W1^T + b1
-        dh = self._gemm(dz, W["mlp1_t"], h * cfg.pointwise_ratio)
-        self._wgrad_linear(dz, S["hmid"], P[f"{b}.mlp1.layer.weight"])
-        self._grad(P[f"{b}.mlp1.layer.bias"], ops.col_sums(dz)[1])
+        dh = self._gemm(dz, W["mlp1_t"], h * cfg.pointwise_ratio) if self._below(f"{b}.mlp1.") else None
+        if trains(P[f"{b}.mlp1.layer.weight"]):
+            self._wgrad_linear(dz, S["hmid"], P[f"{b}.mlp1.layer.weight"])
+        if trains(P[f"{b}.mlp1.layer.bias"]):
+            self._grad(P[f"{b}.mlp1.layer.bias"], ops.col_sums(dz)[1])
+        if dh is None:
+            return None, None
         # mlp0: hmid = relu(LN(y) W0^T)
         dzh = ops.relu_mask(dh, S["hmid"])
         del dh
         dy = self._normlinear_bwd(dzh, S["y"], S["mr_y"], W["mlp0_t"], f"{b}.mlp0", P, add=dz)
         del dzh
+        if dy is None:
+            return None, None
         # proj: y = xhat + a Wp^T + bp
-        da = self._gemm(dy, W["proj_t"], h)
-        self._wgrad_linear(dy, S["a"], P[f"{o}.proj_layer.weight"])
-        self._grad(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
+        da = self._gemm(dy, W["proj_t"], h) if self._below(f"{o}.proj_layer.") else None
+        if trains(P[f"{o}.proj_layer.weight"]):
+            self._wgrad_linear(dy, S["a"], P[f"{o}.proj_layer.weight"])
+        if trains(P[f"{o}.proj_layer.bias"]):
+            self._grad(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
+        if da is None:
+            return None, None
         # attention: gradients wrt q | k | v | R side by side (one buffer = one dgrad GEMM + one wgrad GEMM for all four)
         causal = cfg.mask_style == "clipped_causal"
         dqkvr = torch.zeros((N, cfg.kcat), dtype=BF16, device=dy.device)
@@ -334,30 +455,38 @@ class _Trainer:
                                       da, dqkvr, B, t, maxlen, heads)
         else:  # mask "none" (IDM): q | k | v only; R meets an empty band (b_nd is (10, 0)), so its parameters get exact zeros
             ops.attention_bwd(S["q"], S["full_k"], S["full_v"], None, None, None, None, da, dqkvr, B, t, 0, heads, causal=False)
-            db_nd = torch.zeros_like(P[f"{o}.b_nd"], dtype=F32)
+            db_nd = torch.zeros_like(P[f"{o}.b_nd"], dtype=F32) if trains(P[f"{o}.b_nd"]) else None
         self._grad(P[f"{o}.b_nd"], db_nd)
-        dxhat = self._gemm(dqkvr, W["qkvr_t"], h, residual=dy)
-        dWc = self._wgrad_linear(dqkvr, S["xhat"])
-        dbc = ops.col_sums(dqkvr)[1]
-        self._grad(P[f"{o}.q_layer.weight"], dWc[0:h])
-        self._grad(P[f"{o}.k_layer.weight"], dWc[h:2 * h])
-        self._grad(P[f"{o}.v_layer.weight"], dWc[2 * h:3 * h])
-        self._grad(P[f"{o}.q_layer.bias"], dbc[0:h])
-        if causal:
-            self._grad(P[f"{o}.r_layer.weight"], dWc[3 * h:3 * h + nr])
-            self._grad(P[f"{o}.r_layer.bias"], dbc[3 * h:3 * h + nr])
-        else:
-            self._grad(P[f"{o}.r_layer.weight"], torch.zeros_like(P[f"{o}.r_layer.weight"], dtype=F32))
-            self._grad(P[f"{o}.r_layer.bias"], torch.zeros_like(P[f"{o}.r_layer.bias"], dtype=F32))
+        if not self._below(f"{o}.b_nd"):
+            return None, dmem
+        # q | k | v | r: one dgrad GEMM and one wgrad GEMM for the four (r only where the mask has a band)
+        ws = [P[f"{o}.{c}_layer.weight"] for c in ("q", "k", "v")] + ([P[f"{o}.r_layer.weight"]] if causal else [])
+        bs = [P[f"{o}.q_layer.bias"]] + ([P[f"{o}.r_layer.bias"]] if causal else [])
+        dxhat = self._gemm(dqkvr, W["qkvr_t"], h, residual=dy) if self._below(f"{o}.q_layer.") else None
+        dWc = self._wgrad_linear(dqkvr, S["xhat"]) if any(map(trains, ws)) else None
+        dbc = ops.col_sums(dqkvr)[1] if any(map(trains, bs)) else None
+        for p, r0, r1 in zip(ws, (0, h, 2 * h, 3 * h), (h, 2 * h, 3 * h, 3 * h + nr)):
+            if trains(p):
+                self._grad(p, dWc[r0:r1])
+        for p, r0, r1 in zip(bs, (0, 3 * h), (h, 3 * h + nr)):
+            if trains(p):
+                self._grad(p, dbc[r0:r1])
+        if not causal:
+            for p in (P[f"{o}.r_layer.weight"], P[f"{o}.r_layer.bias"]):
+                if trains(p):
+                    self._grad(p, torch.zeros_like(p, dtype=F32))
+        if dxhat is None:
+            return None, dmem
         # pre_r_ln (plain norm of the block input)
         g = P[f"{b}.pre_r_ln.weight"]
         dx = self._norm_bwd(dxhat, S["x"], S["mr_x"], g.detach().float().contiguous(), 1, h, g, P[f"{b}.pre_r_ln.bias"],
-                            relu_x=(l == 0))  # block 0's input is relu(img_process.linear)
+                            relu_x=(l == 0), want_dx=self._below(f"{b}.pre_r_ln."))  # block 0's input is relu(img_process.linear)
         return dx, dmem
 
     def _cnn_bwd(self, dout, tape, wts, P):
         """Backward of lib/impala_cnn.py:187-195; `dout` is the gradient wrt the last stack's output (ZP).  Returns the gradient wrt the
-        CNN input when stack 0's first conv is a normalised one (the IDM: the conv3d output, ReLU backward applied), else None."""
+        CNN input when stack 0's first conv is a normalised one and the conv3d pre-stage trains (the IDM: the conv3d output, ReLU backward
+        applied), else None.  Stops at the lowest unit that needs a gradient."""
         cfg = self.net.cfg
         pfx = "img_process.cnn"
         dx = dout
@@ -376,12 +505,19 @@ class _Trainer:
                 dz0 = self._normconv_bwd(dz1, blk["h"], blk["mrh"], H, W, wts["stacks"][i]["convs"][2 * j + 1], f"{s}.blocks.{j}.conv1", P,
                                          relu_x=True)
                 del dz1
+                if dz0 is None:
+                    return None
                 dx = self._normconv_bwd(dz0, x_in, mr_in, H, W, wts["stacks"][i]["convs"][2 * j], f"{s}.blocks.{j}.conv0", P, add=dx)
                 del dz0
+                if dx is None:
+                    return None
             # x0 = GN_n(y1) (plain norm)
             g = P[f"{s}.n.weight"]
             dy1 = self._norm_bwd(dx.view(R, C), rec["y1"].view(R, C), rec["mr1"], g.detach().float().contiguous(), (H + 1) * (W + 1), H * W * C,
-                                 g, P[f"{s}.n.bias"], zp=(H, W, C)).view(rec["y1"].shape)
+                                 g, P[f"{s}.n.bias"], zp=(H, W, C), want_dx=self._below(f"{s}.n."))
+            if dy1 is None:
+                return None
+            dy1 = dy1.view(rec["y1"].shape)
             if i == 0 and not cfg.first_conv_norm:
                 st = tape["prep"].stacks[0]  # (the weights the forward used)
                 dWk, db = ops.firstconv_bwd(tape["frames"], st["fc_w"], st["fc_b"], dy1, C)
@@ -395,6 +531,8 @@ class _Trainer:
             dx = self._normconv_bwd(dfull, rec["x_in"], rec["mr_in"], rec["H_in"], rec["W_in"], wts["stacks"][i]["first"],
                                     f"{s}.firstconv", P, relu_x=(i == 0))
             del dfull
+            if dx is None:
+                return None
         return dx
 
 
@@ -409,6 +547,11 @@ class BCTrainer(_Trainer):
     runs the CNN in chunks of F frames (at most `net.cnn_chunk_frames`) and the backward re-runs each chunk's forward before
     back-propagating through it.  That costs one more CNN forward per call and allows `max_call_frames` frames per call (e.g. B = 128,
     T = 128 in one call at 2x width); the gradients are those of the stored tape.
+
+    Parameters with requires_grad=False when the call starts are frozen: their `.grad` is left as it is, their weight-side work is skipped
+    and the backward stops at the lowest unit that trains.  With the whole ImpalaCNN (`img_process.cnn.*`) frozen the forward keeps no
+    CNN activation, so a call is bounded by `max_call_frames` instead of the stored tape, and `upper_grads_ready` fires at the end of the
+    backward.  With nothing trainable the call returns the loss and state_out and runs no backward.
     """
 
     def __init__(self, policy: MinecraftAgentPolicy, recompute_frames=None):
@@ -431,22 +574,24 @@ class BCTrainer(_Trainer):
         backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`."""
         self._check_heads()
         lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
-        loss, dlog = self._bc_dlog(pd, actions, img.shape[0] * img.shape[1])
+        loss, dlog = self._bc_dlog(pd, actions, img.shape[0] * img.shape[1], want_dlog=tape["lowest"] <= len(self._units))
         self._backward_from_dlog(dlog, lat_bf16, tape, img.shape[0], img.shape[1], upper_grads_ready)
         return loss, state_out
 
-    def _bc_dlog(self, pd, actions, N):
-        """The BC loss -mean log p(action) over the N frames and its gradient wrt the logits, bf16 [N][ld_logits]."""
+    def _bc_dlog(self, pd, actions, N, want_dlog=True):
+        """The BC loss -mean log p(action) over the N frames and its gradient wrt the logits, bf16 [N][ld_logits] (None without
+        `want_dlog`: nothing trains)."""
         pol = self.policy
         hp = pol._heads_prepared()
-        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=pol.net.final_ln.weight.device)
+        dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=pol.net.final_ln.weight.device) if want_dlog else None
         scale = 1.0 / (pol.temperature * N)
         logp = None
         for name, (shape, n) in pol.head_specs.items():
             idx = actions[name].reshape(N).to(torch.int64)
             lp = ops.gather_logprob(pd[name].reshape(N, n), idx)
             logp = lp if logp is None else logp + lp
-            ops.softmax_bwd(pd[name].reshape(N, n), idx, scale, dlog, hp["cols"][name][0])
+            if want_dlog:
+                ops.softmax_bwd(pd[name].reshape(N, n), idx, scale, dlog, hp["cols"][name][0])
         return -logp.sum() / N, dlog
 
 
@@ -578,9 +723,9 @@ class IDMTrainer(_Trainer):
         B, t = img.shape[:2]
         N = B * t
         # checked before the forward: nothing is accumulated into .grad by a call that cannot finish
-        if self.recompute_frames is None and N > net.idm_chunk_frames:
-            raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls "
-                                      "or pass recompute_frames")
+        if self.recompute_frames is None and N > net.idm_chunk_frames and self._grad_plan()["cnn"]:
+            raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls, "
+                                      "pass recompute_frames or freeze the CNN and the conv3d pre-stage")
         if t > self.max_t:
             raise NotImplementedError(f"IDMTrainer: at most {self.max_t} frames per sequence (got T = {t})")
         lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
@@ -650,7 +795,7 @@ class _AutogradRunner(_Trainer):
         B, t = img.shape[:2]
         N = B * t
         self.recompute_frames = self.module._recompute_frames  # set_autograd(.., recompute_frames=..)
-        stored = self.recompute_frames is None
+        stored = self.recompute_frames is None and self._grad_plan()["cnn"]  # (a frozen CNN keeps no activations)
         if net.cfg.conv3d_out is None:
             if stored and N > net.cnn_chunk_frames:
                 raise NotImplementedError(f"differentiable forward: at most {net.cnn_chunk_frames} frames per call (got B*T = {N}); "
@@ -690,12 +835,14 @@ class _AutogradRunner(_Trainer):
         """Runs the taped forward -> (output tensors, tape)."""
         img = box["img"]
         B, t = img.shape[:2]
+        # with state_grad, a state_in K / V that requires grad is an input whose gradient the backward returns
+        want = [k.requires_grad or v.requires_grad for _, (k, v) in box["state_in"]] if box["state_grad"] else None
         if self.policy is None:
-            lat_bf16, lat_f32, tape, state_out = self._taped_latent(img, box["first"], box["state_in"])
+            lat_bf16, lat_f32, tape, state_out = self._taped_latent(img, box["first"], box["state_in"], want)
             outs = (lat_f32,)
         else:
             mask = box["mask"]
-            lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, box["first"], box["state_in"], mask)
+            lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, box["first"], box["state_in"], mask, want)
             outs = tuple(pd.values()) + ((vpred,) if vpred is not None else ())
             masks = {}
             for name, (shape, n) in self.policy.head_specs.items():
@@ -745,7 +892,7 @@ class _AutogradRunner(_Trainer):
                     dlog[:, hp["ntot"]] = gv.reshape(N).to(BF16)  # d vpred: the value head's column (a strided copy of N values)
             dlat = self._heads_bwd(dlog, tape["lat"], tape)
             del dlog
-            dmem = self._backward_from_dlat(dlat, tape, B, t, None, dstate, want_dmem)
+            dmem = [None] * self.net.cfg.n_layers if dlat is None else self._backward_from_dlat(dlat, tape, B, t, None, dstate, want_dmem)
             for lin in unused:
                 sink.pop(id(lin.weight), None)
                 sink.pop(id(lin.bias), None)
