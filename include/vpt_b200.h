@@ -160,6 +160,11 @@ int vpt_firstconv_pool(const uint8_t* img, const float* w, const float* bias, vo
                        int32_t F, int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream);
 int vpt_firstconv_stat_parts(int32_t F, int32_t H, int32_t W, int32_t C0);
 int vpt_set_firstconv_mode(int32_t mode);
+/* vpt_firstconv_pool on fp32 frames img [F][H][W][3] on the uint8 scale (any value, not clipped).  The patch is split into bf16 hi + lo
+ * (two more k-steps, run only for a tile whose lo part is not all zero), so integer-valued frames in [0, 255] give vpt_firstconv_pool's
+ * outputs and partials bit for bit. */
+int vpt_firstconv_pool_f32(const float* img, const float* w, const float* bias, void* out, float* stat_part,
+                           int32_t F, int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream);
 
 /* IDM temporal pre-stage (lib/policy.py:394-403 + :39-45): u8 -> /255 -> Conv3d(3 -> C, kernel (5,1,1), pad (2,0,0)) + bias -> ReLU,
  * per sample over its T frames (zero padded in time at the chunk ends, like the reference's per-sample loop).
@@ -167,6 +172,10 @@ int vpt_set_firstconv_mode(int32_t mode);
  *   stat_part float2 [B*T][vpt_conv3d_stat_parts(H, W, C)] */
 int vpt_conv3d_t5(const uint8_t* img, const float* w, const float* bias, void* out, float* stat_part, int32_t B, int32_t T,
                   int32_t H, int32_t W, int32_t C, int32_t out_f32, void* stream);  /* out_f32: fp32 output, same layout (precision mode) */
+/* vpt_conv3d_t5 on fp32 frames img [B][T][H][W][3] on the uint8 scale: the same fp32 FMAs, so integer-valued frames give its results bit
+ * for bit. */
+int vpt_conv3d_t5_f32(const float* img, const float* w, const float* bias, void* out, float* stat_part, int32_t B, int32_t T,
+                      int32_t H, int32_t W, int32_t C, int32_t out_f32, void* stream);
 
 /* ----------------------------------------------------------------------------------------------------------
  * On-device action codec (csrc/codec.cuh; SURVEY.md row f-3): table look-ups, one thread per action.
@@ -372,6 +381,16 @@ int vpt_maxpool3s2_bwd(const void* dy, const void* x, void* dx, void* workspace,
 int vpt_firstconv_bwd(const uint8_t* img, const float* w, const float* bias, const void* dy, float* dW, float* db, float* workspace, int64_t F,
                       int32_t H, int32_t W, int32_t C0, void* stream);
 int vpt_firstconv_bwd_parts(int64_t F, int32_t H, int32_t W);
+/* vpt_firstconv_bwd on fp32 frames (vpt_firstconv_pool_f32). */
+int vpt_firstconv_bwd_f32(const float* img, const float* w, const float* bias, const void* dy, float* dW, float* db, float* workspace, int64_t F,
+                          int32_t H, int32_t W, int32_t C0, void* stream);
+/* Image gradient of vpt_firstconv_pool[_f32]: dimg fp32 [F][H][W][3] = d loss / d img (uint8 scale) from dy bf16 ZP [F][H/2+1][W/2+1][C0]
+ * (the same dy as vpt_firstconv_bwd) and the same w / bias.  The pre-pool map is recomputed with vpt_firstconv_bwd's fp32 FMA chain and
+ * each pooled gradient goes to the same position (first maximum in window scan order, only a positive maximum), so the two backward
+ * kernels differentiate one function.  img u8 (img_f32 = 0) or fp32 (img_f32 = 1).  H, W multiples of 16, C0 a multiple of 8 <= 256.
+ * One CTA per 16x16 input block, fixed-order sums, no atomics: bit-reproducible. */
+int vpt_firstconv_dimg(const void* img, int32_t img_f32, const float* w, const float* bias, const void* dy, float* dimg, int64_t F,
+                       int32_t H, int32_t W, int32_t C0, void* stream);
 /* Backward of vpt_attention (causal policy attention): given dO bf16 [B*t][h] writes d q | d k | d v | d R side by side into
  * out bf16 [B*t][ld_out] at columns 0 | h | 2h | 3h (chunk rows only -- the KV memory is detached state,
  * behavioural_cloning.py:111) and d b_nd fp32 [nbasis][maxlen].  workspace: 2*B*heads*t*maxlen floats.   lib/xf.py:18-71,265-271 */
@@ -406,6 +425,13 @@ int vpt_softmax_bwd(const float* logp, const int64_t* idx, float scale, void* ou
 int64_t vpt_conv3d_t5_bwd_workspace(int64_t F, int32_t H, int32_t W, int32_t C);
 int vpt_conv3d_t5_bwd(const uint8_t* img, const void* dy, float* dW, float* db, float* workspace, int32_t B, int32_t T, int32_t H, int32_t W,
                       int32_t C, void* stream);
+/* vpt_conv3d_t5_bwd on fp32 frames (vpt_conv3d_t5_f32). */
+int vpt_conv3d_t5_bwd_f32(const float* img, const void* dy, float* dW, float* db, float* workspace, int32_t B, int32_t T, int32_t H, int32_t W,
+                          int32_t C, void* stream);
+/* Image gradient of vpt_conv3d_t5[_f32]: dimg fp32 [B][T][H][W][3] (uint8 scale) from the same dy as vpt_conv3d_t5_bwd and w fp32 [C][15]
+ * (dt, c), already divided by 255:  dimg[b][s] = sum_dt dy[b][s + 2 - dt] * w[dt], zero padding in time at both ends of each sequence.
+ * dy is read once; fixed-order sums, no atomics.  C = 8 * a power of two <= 256; B <= 65535. */
+int vpt_conv3d_t5_dimg(const void* dy, const float* w, float* dimg, int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream);
 /* Backward of vpt_attention with causal = 0 (mask "none", maxlen = 0: every query sees the t keys of its chunk, logits q.k / D).
  * Q, K, V, dO bf16 [B*t][h]; writes d q | d k | d v into out bf16 [B*t][ld_out] at columns 0 | h | 2h.  t <= 128, D = 128.
  * workspace: vpt_attention_full_bwd_workspace(B, t, heads) floats.  No atomics: bit-reproducible. */

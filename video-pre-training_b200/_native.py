@@ -93,6 +93,8 @@ SIGNATURES = {
     "vpt_firstconv_stat_parts": (_I, [_I, _I, _I, _I]),
     "vpt_set_firstconv_mode": (_I, [_I]),
     "vpt_conv3d_t5": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "vpt_firstconv_pool_f32": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "vpt_conv3d_t5_f32": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "vpt_group_stats_f32": (_I, [_P, _P, _L, _L, _F, _P]),
     "vpt_norm_split_f32": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _I, _L, _P]),
     "vpt_add_f32": (_I, [_P, _P, _P, _L, _I, _P]),
@@ -151,6 +153,11 @@ SIGNATURES = {
     "vpt_value_bwd": (_I, [_P, _P, _P, _D, _P, _P, _P, _F, _F, _F, _P, _L, _I, _P, _L, _P]),
     # differentiable forward (training.py, set_autograd)
     "vpt_log_softmax_bwd": (_I, [_P, _L, _P, _L, _P, _I, _I, _F, _P, _L, _I, _L, _P]),
+    # the image gradient (training.py, set_autograd with an img that requires grad)
+    "vpt_firstconv_bwd_f32": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _P]),
+    "vpt_firstconv_dimg": (_I, [_P, _I, _P, _P, _P, _P, _L, _I, _I, _I, _P]),
+    "vpt_conv3d_t5_bwd_f32": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vpt_conv3d_t5_dimg": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
 }
 
 _lib = None

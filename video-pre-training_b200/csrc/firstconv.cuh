@@ -10,6 +10,10 @@
 // One CTA = one 8x8 tile of POOLED outputs of one frame = 17x17 conv outputs (19 m16 tiles) from a 19x19x3 patch.
 // ~99 KB of shared memory at C0 = 128 -> two CTAs per SM overlap one CTA's pooling with the other's MMAs.
 // F32OUT (precision mode): the conv tile is kept in fp32 and the output is fp32; the channels then go through the tile 64 at a time.
+// TIN = float (fp32 frames on the uint8 scale, vpt_firstconv_pool_f32): an fp32 value is not exact in bf16, so the patch is split too,
+// x = x_hi + x_lo, and A = x_hi | x_hi | 1 | x_lo against B = w_hi | w_lo | bias | w_hi (x_lo * w_lo, below 2^-16 relative, dropped):
+// K = 96, 6 k-steps.  The x_lo k-steps run after the other four and only for a tile whose x_lo is not all zero (a CTA-wide vote
+// while the patch is staged), so integer-valued frames take exactly the uint8 path's MMAs in the same order: bit-identical outputs.
 #pragma once
 #include <type_traits>
 
@@ -24,31 +28,43 @@ constexpr int kFcIn = kFcConv + 2;       // 19 input rows/cols
 constexpr int kFcThreads = 256;
 constexpr int kFcPos = kFcConv * kFcConv;        // 289 conv positions
 constexpr int kFcMTiles = (kFcPos + 15) / 16;    // 19
-constexpr int kFcBPitch = 72;                    // bf16 elements per weight row in smem (144 B: conflict-free ldmatrix)
 constexpr int kFcPatchElems = kFcIn * kFcIn * 3; // 1083
 constexpr int kFcPatchBytes = 2192;              // bf16 patch + one zero element, 16-byte multiple
 
-template <bool F32OUT>
-__global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uint8_t* __restrict__ img, const float* __restrict__ w,
+template <typename TIN>
+struct FcIn {
+    static constexpr bool kF32 = std::is_same<TIN, float>::value;
+    static constexpr int kKSteps = kF32 ? 6 : 4;           // k-steps of 16: x_hi (w_hi, w_lo, bias) [+ x_lo (w_hi)]
+    static constexpr int kBPitch = 16 * kKSteps + 8;       // 72 / 104 bf16 per weight row (144 / 208 B: conflict-free ldmatrix)
+    static constexpr int kPatches = kF32 ? 2 : 1;          // x_hi [, x_lo]
+};
+
+template <bool F32OUT, typename TIN>
+__global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const TIN* __restrict__ img, const float* __restrict__ w,
                                                                        const float* __restrict__ bias, void* __restrict__ out_,
                                                                        float2* __restrict__ stat_part, int H, int W, int C0, long long total_tiles, int zp) {
     pdl_sync();
     extern __shared__ __align__(16) uint8_t fc_smem[];
+    using In = FcIn<TIN>;
+    constexpr int kBPitch = In::kBPitch, kKCols = 16 * In::kKSteps;
     __nv_bfloat16* patch = reinterpret_cast<__nv_bfloat16*>(fc_smem);                                  // [19][19][3]
-    __nv_bfloat16* Bs = reinterpret_cast<__nv_bfloat16*>(fc_smem + kFcPatchBytes);                     // [C0][72]
+    __nv_bfloat16* patch_lo = reinterpret_cast<__nv_bfloat16*>(fc_smem + kFcPatchBytes);               // [19][19][3] (fp32 frames)
+    __nv_bfloat16* Bs = reinterpret_cast<__nv_bfloat16*>(fc_smem + In::kPatches * kFcPatchBytes);     // [C0][kBPitch]
     using CT = typename std::conditional<F32OUT, float, __nv_bfloat16>::type;
     const int CB = F32OUT ? 64 : C0;  // channels per pass through the conv tile
     const int cpitch = CB + 8;
-    CT* ctile = reinterpret_cast<CT*>(Bs + (size_t)C0 * kFcBPitch);                                    // [289][CB+8]
+    CT* ctile = reinterpret_cast<CT*>(Bs + (size_t)C0 * kBPitch);                                    // [289][CB+8]
     CT* const out = reinterpret_cast<CT*>(out_);
     const int tiles_x = (W / 2) / kFcTile, tiles_y = (H / 2) / kFcTile;
     const int tiles = tiles_x * tiles_y;
 
     // ---- hi/lo-split weights, staged once per (persistent) CTA
-    for (int i = threadIdx.x; i < C0 * 64; i += kFcThreads) {
-        const int n = i >> 6, k = i & 63;
+    for (int i = threadIdx.x; i < C0 * kKCols; i += kFcThreads) {
+        const int n = i / kKCols, k = i % kKCols;
         float v = 0.f;
-        if (k < 27) {
+        if (k >= 64) {  // fp32 frames: w_hi against x_lo
+            if (k < 64 + 27) v = __ldg(w + n * 27 + k - 64);
+        } else if (k < 27) {
             v = __ldg(w + n * 27 + k);
         } else if (k < 54) {
             const float x = __ldg(w + n * 27 + k - 27);
@@ -59,7 +75,7 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
             const float x = __ldg(bias + n);
             v = x - __bfloat162float(__float2bfloat16_rn(x));
         }
-        Bs[n * kFcBPitch + k] = __float2bfloat16_rn(v);
+        Bs[n * kBPitch + k] = __float2bfloat16_rn(v);
     }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
@@ -75,6 +91,7 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
             kval[s][e] = k < 54;
             koff[s][e] = kval[s][e] ? (kk / 9) * (kFcIn * 3) + kk % 9 : 0;
         }
+
     // (a) patch staging without div/mod in the tile loop: each thread owns fixed patch elements; the NEXT tile's bytes are
     // prefetched into registers while the current tile is computed
     constexpr int kPE = (kFcPatchElems + kFcThreads - 1) / kFcThreads;  // 5
@@ -85,17 +102,17 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
         pe_row[j] = i / (kFcIn * 3);
         pe_col[j] = i % (kFcIn * 3);
     }
-    uint8_t pre[kPE];
+    TIN pre[kPE];
     auto prefetch = [&](long long tid) {
         const long long f = tid / tiles;
         const int tile = (int)(tid % tiles);
         const int Yin0 = 2 * (tile / tiles_x) * kFcTile - 2, Xin0 = 2 * (tile % tiles_x) * kFcTile - 2;
-        const uint8_t* fimg = img + f * (long long)H * W * 3;
+        const TIN* fimg = img + f * (long long)H * W * 3;
 #pragma unroll
         for (int j = 0; j < kPE; ++j) {
             const int Y = Yin0 + pe_row[j], xb = Xin0 * 3 + pe_col[j];  // xb = X*3 + c
             const bool ok = (threadIdx.x + j * kFcThreads < kFcPatchElems) && Y >= 0 && Y < H && xb >= 0 && xb < W * 3;
-            pre[j] = ok ? __ldg(fimg + (long long)Y * W * 3 + xb) : (uint8_t)0;
+            pre[j] = ok ? __ldg(fimg + (long long)Y * W * 3 + xb) : (TIN)0;
         }
     };
     if ((long long)blockIdx.x < total_tiles) prefetch(blockIdx.x);
@@ -104,11 +121,28 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
     const long long f = tid / tiles;
     const int tile = (int)(tid % tiles);
     const int PY0 = (tile / tiles_x) * kFcTile, PX0 = (tile % tiles_x) * kFcTile;
-    // ---- stage the input patch (u8 -> bf16, exact) from the prefetched registers, then prefetch the next tile
+    // ---- stage the input patch (u8 -> bf16, exact; fp32 -> bf16 hi + bf16 lo) from the prefetched registers, then prefetch the next tile
+    int any_lo = 0;  // fp32 frames: some x_lo of this tile is not zero (the x_lo k-steps run)
+    if constexpr (In::kF32) {
+        int nz = 0;
 #pragma unroll
-    for (int j = 0; j < kPE; ++j) {
-        const int i = threadIdx.x + j * kFcThreads;
-        if (i < kFcPatchElems) patch[i] = __float2bfloat16_rn((float)pre[j]);
+        for (int j = 0; j < kPE; ++j) {
+            const int i = threadIdx.x + j * kFcThreads;
+            if (i < kFcPatchElems) {
+                const __nv_bfloat16 hi = __float2bfloat16_rn(pre[j]);
+                const float lo = pre[j] - __bfloat162float(hi);
+                patch[i] = hi;
+                patch_lo[i] = __float2bfloat16_rn(lo);
+                nz |= lo != 0.f;
+            }
+        }
+        any_lo = __syncthreads_or(nz);
+    } else {
+#pragma unroll
+        for (int j = 0; j < kPE; ++j) {
+            const int i = threadIdx.x + j * kFcThreads;
+            if (i < kFcPatchElems) patch[i] = __float2bfloat16_rn((float)pre[j]);
+        }
     }
     if (tid + gridDim.x < total_tiles) prefetch(tid + gridDim.x);
     const int Ho = H / 2, Wo = W / 2, opitch = Wo + zp;  // ZP layout: one extra zero column / row
@@ -143,6 +177,7 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
             }
         }
         if (tg == 3) af[3][0] = af[3][1] = 0x3F803F80u;  // k = 54, 55: constant 1.0 (x the bias columns of B)
+
         for (int nh = cg / 64; nh < (cg + CB) / 64; ++nh) {  // 64 output channels at a time
             float acc[8][4];
 #pragma unroll
@@ -154,9 +189,37 @@ __global__ void __launch_bounds__(kFcThreads, 2) firstconv_pool_kernel(const uin
                     uint32_t b0, b1, b2, b3;
                     const int nrow = nh * 64 + np * 16 + (lane & 7) + ((lane >> 4) << 3);
                     const int kcol = s * 16 + (((lane >> 3) & 1) << 3);
-                    ldsm_x4(smem_u32(Bs + nrow * kFcBPitch + kcol), b0, b1, b2, b3);
+                    ldsm_x4(smem_u32(Bs + nrow * kBPitch + kcol), b0, b1, b2, b3);
                     mma_bf16_16816(acc[2 * np], af[s][0], af[s][1], af[s][2], af[s][3], b0, b1);
                     mma_bf16_16816(acc[2 * np + 1], af[s][0], af[s][1], af[s][2], af[s][3], b2, b3);
+                }
+            }
+            if constexpr (In::kF32) {
+                if (any_lo) {
+                    // A = x_lo at k' = k - 64 in [0, 27): the patch offsets of k' are koff[s] of the first two k-steps (k' < 27).  One
+                    // k-step's fragments at a time (4 registers), gathered after the x_hi MMAs, to keep the register pressure of the u8 path.
+#pragma unroll
+                    for (int s = 0; s < 2; ++s) {
+                        uint32_t af_lo[4];
+#pragma unroll
+                        for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+                            for (int hh = 0; hh < 2; ++hh) {
+                                const int k = 16 * s + 2 * tg + 8 * hh;  // k' of the pair's first element
+                                const uint16_t lo = k < 27 ? *reinterpret_cast<const uint16_t*>(patch_lo + pbase[rr] + koff[s][2 * hh]) : (uint16_t)0;
+                                const uint16_t hi = k + 1 < 27 ? *reinterpret_cast<const uint16_t*>(patch_lo + pbase[rr] + koff[s][2 * hh + 1]) : (uint16_t)0;
+                                af_lo[rr + 2 * hh] = (uint32_t)lo | ((uint32_t)hi << 16);
+                            }
+#pragma unroll
+                        for (int np = 0; np < 4; ++np) {
+                            uint32_t b0, b1, b2, b3;
+                            const int nrow = nh * 64 + np * 16 + (lane & 7) + ((lane >> 4) << 3);
+                            const int kcol = 64 + s * 16 + (((lane >> 3) & 1) << 3);
+                            ldsm_x4(smem_u32(Bs + nrow * kBPitch + kcol), b0, b1, b2, b3);
+                            mma_bf16_16816(acc[2 * np], af_lo[0], af_lo[1], af_lo[2], af_lo[3], b0, b1);
+                            mma_bf16_16816(acc[2 * np + 1], af_lo[0], af_lo[1], af_lo[2], af_lo[3], b2, b3);
+                        }
+                    }
                 }
             }
             // raw pre-activation values; ReLU is applied after the max (monotone), positions outside the image hold 0
@@ -254,19 +317,22 @@ extern "C" int vpt_set_firstconv_mode(int32_t mode) {
     return VPT_OK;
 }
 
-extern "C" int vpt_firstconv_pool(const uint8_t* img, const float* w, const float* bias, void* out, float* stat_part, int32_t F,
-                                  int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream) {
-    using namespace vpt;
-    VPT_CHECK(img && w && bias && out && F > 0, "vpt_firstconv_pool: null argument");
-    VPT_CHECK(H % 16 == 0 && W % 16 == 0 && H >= 16 && W >= 16, "vpt_firstconv_pool: H, W must be multiples of 16 (H=%d W=%d)", H, W);
-    VPT_CHECK(C0 == 64 || C0 == 128 || C0 == 192 || C0 == 256, "vpt_firstconv_pool: C0=%d not in {64,128,192,256}", C0);
+namespace vpt {
+
+template <typename TIN>
+static int firstconv_pool_launch(const char* fn, const TIN* img, const float* w, const float* bias, void* out, float* stat_part, int32_t F,
+                                 int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream) {
+    VPT_CHECK(img && w && bias && out && F > 0, "%s: null argument", fn);
+    VPT_CHECK(H % 16 == 0 && W % 16 == 0 && H >= 16 && W >= 16, "%s: H, W must be multiples of 16 (H=%d W=%d)", fn, H, W);
+    VPT_CHECK(C0 == 64 || C0 == 128 || C0 == 192 || C0 == 256, "%s: C0=%d not in {64,128,192,256}", fn, C0);
     const long long blocks = (long long)F * (H / 16) * (W / 16);
-    VPT_CHECK(blocks < 2147483647LL, "vpt_firstconv_pool: too many tiles");
+    VPT_CHECK(blocks < 2147483647LL, "%s: too many tiles", fn);
+    using In = FcIn<TIN>;
     const int CB = out_f32 ? 64 : C0;
-    const size_t smem = kFcPatchBytes + (size_t)C0 * kFcBPitch * 2 + (size_t)kFcPos * (CB + 8) * (out_f32 ? 4 : 2);
-    void (*kern)(const uint8_t*, const float*, const float*, void*, float2*, int, int, int, long long, int) =
-        out_f32 ? firstconv_pool_kernel<true> : firstconv_pool_kernel<false>;
-    static size_t attr[2] = {0, 0};
+    const size_t smem = (size_t)In::kPatches * kFcPatchBytes + (size_t)C0 * In::kBPitch * 2 + (size_t)kFcPos * (CB + 8) * (out_f32 ? 4 : 2);
+    void (*kern)(const TIN*, const float*, const float*, void*, float2*, int, int, int, long long, int) =
+        out_f32 ? firstconv_pool_kernel<true, TIN> : firstconv_pool_kernel<false, TIN>;
+    static size_t attr[2] = {0, 0};  // (one table per frame type)
     if (smem > attr[out_f32 ? 1 : 0]) {
         VPT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr[out_f32 ? 1 : 0] = smem;
@@ -280,4 +346,16 @@ extern "C" int vpt_firstconv_pool(const uint8_t* img, const float* w, const floa
              img, w, bias, out, reinterpret_cast<float2*>(stat_part), H, W, C0, blocks, zp ? 1 : 0);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
+}
+
+}  // namespace vpt
+
+extern "C" int vpt_firstconv_pool(const uint8_t* img, const float* w, const float* bias, void* out, float* stat_part, int32_t F,
+                                  int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream) {
+    return vpt::firstconv_pool_launch("vpt_firstconv_pool", img, w, bias, out, stat_part, F, H, W, C0, zp, out_f32, stream);
+}
+
+extern "C" int vpt_firstconv_pool_f32(const float* img, const float* w, const float* bias, void* out, float* stat_part, int32_t F,
+                                      int32_t H, int32_t W, int32_t C0, int32_t zp, int32_t out_f32, void* stream) {
+    return vpt::firstconv_pool_launch("vpt_firstconv_pool_f32", img, w, bias, out, stat_part, F, H, W, C0, zp, out_f32, stream);
 }

@@ -125,8 +125,15 @@ def conv3x3_zp(x, Wb, H, W, *, mr=None, S1=None, S2=None, relu=1, residual=None,
     return out, mr_out
 
 
+def _frames_f32(img, what):
+    """Whether frames are fp32 (the `_f32` entry points) or u8; anything else raises."""
+    if img.dtype not in (torch.uint8, F32) or not img.is_contiguous():
+        raise ValueError(f"{what}: frames must be contiguous uint8 or float32 (got {img.dtype})")
+    return img.dtype == F32
+
+
 def firstconv_pool(img, w, bias, C0, zp=True, out_f32=False, want_chan=False):
-    """img u8 [F,H,W,3] -> (bf16 (fp32 with out_f32) [F,H/2(+1),W/2(+1),C0] (ZP layout when zp), per-frame (mean, rstd)).
+    """img u8 or fp32 (uint8 scale) [F,H,W,3] -> (bf16 (fp32 with out_f32) [F,H/2(+1),W/2(+1),C0] (ZP layout when zp), per-frame (mean, rstd)).
     want_chan: also return the per-channel (sum, sumsq) partials [F, NP, C0, 2] of the pooled tensor (None if the kernel that ran does
     not produce them), for `norm2_fold`."""
     _cuda(img, w, bias)
@@ -135,7 +142,8 @@ def firstconv_pool(img, w, bias, C0, zp=True, out_f32=False, want_chan=False):
     out = torch.empty((F_, H // 2 + z, W // 2 + z, C0), dtype=F32 if out_f32 else BF16, device=img.device)
     P = nat.lib().vpt_firstconv_stat_parts(F_, H, W, C0)
     part = torch.empty((F_, P, 2), dtype=F32, device=img.device)
-    nat.check(nat.lib().vpt_firstconv_pool(_p(img), _p(w), _p(bias), _p(out), _p(part), F_, H, W, C0, z, int(out_f32), _stream()), "vpt_firstconv_pool")
+    fn = "vpt_firstconv_pool_f32" if _frames_f32(img, "firstconv_pool") else "vpt_firstconv_pool"
+    nat.check(getattr(nat.lib(), fn)(_p(img), _p(w), _p(bias), _p(out), _p(part), F_, H, W, C0, z, int(out_f32), _stream()), fn)
     _count()
     mr = stats_finalize(part, F_, P, (H // 2) * (W // 2) * C0)
     if want_chan:  # the kernel's partials are per (8x8 pooled tile, channel)
@@ -144,13 +152,14 @@ def firstconv_pool(img, w, bias, C0, zp=True, out_f32=False, want_chan=False):
 
 
 def conv3d_t5(img, w, bias, C, out_f32=False):
-    """img u8 [B,T,H,W,3] -> (bf16 (fp32 with out_f32) ZP [B*T,H+1,W+1,C], per-frame (mean, rstd)); lib/policy.py:394-403."""
+    """img u8 or fp32 (uint8 scale) [B,T,H,W,3] -> (bf16 (fp32 with out_f32) ZP [B*T,H+1,W+1,C], per-frame (mean, rstd)); lib/policy.py:394-403."""
     _cuda(img, w, bias)
     B, T, H, W, _ = img.shape
     out = torch.empty((B * T, H + 1, W + 1, C), dtype=F32 if out_f32 else BF16, device=img.device)
     P = nat.lib().vpt_conv3d_stat_parts(H, W, C)
     part = torch.empty((B * T, P, 2), dtype=F32, device=img.device)
-    nat.check(nat.lib().vpt_conv3d_t5(_p(img), _p(w), _p(bias), _p(out), _p(part), B, T, H, W, C, int(out_f32), _stream()), "vpt_conv3d_t5")
+    fn = "vpt_conv3d_t5_f32" if _frames_f32(img, "conv3d_t5") else "vpt_conv3d_t5"
+    nat.check(getattr(nat.lib(), fn)(_p(img), _p(w), _p(bias), _p(out), _p(part), B, T, H, W, C, int(out_f32), _stream()), fn)
     _count()
     return out, stats_finalize(part, B * T, P, H * W * C)
 
@@ -473,14 +482,15 @@ def maxpool3s2_bwd(dy, x):
 
 
 def firstconv_bwd(img, w, bias, dy, C0):
-    """Weight / bias gradient of the fused first conv + ReLU + max-pool: (fp32 [C0][27] in (ky,kx,c) order, fp32 [C0])."""
+    """Weight / bias gradient of the fused first conv + ReLU + max-pool on u8 or fp32 frames: (fp32 [C0][27] in (ky,kx,c) order, fp32 [C0])."""
     _cuda(img, w, bias, dy)
+    fn = "vpt_firstconv_bwd_f32" if _frames_f32(img, "firstconv_bwd") else "vpt_firstconv_bwd"
     F_, H, W, _ = img.shape
     S = nat.lib().vpt_firstconv_bwd_parts(F_, H, W)
     ws = torch.empty((S, C0, 28), dtype=F32, device=img.device)
     dW = torch.empty((C0, 27), dtype=F32, device=img.device)
     db = torch.empty((C0,), dtype=F32, device=img.device)
-    nat.check(nat.lib().vpt_firstconv_bwd(_p(img), _p(w), _p(bias), _p(dy), _p(dW), _p(db), _p(ws), F_, H, W, C0, _stream()), "vpt_firstconv_bwd")
+    nat.check(getattr(nat.lib(), fn)(_p(img), _p(w), _p(bias), _p(dy), _p(dW), _p(db), _p(ws), F_, H, W, C0, _stream()), fn)
     _count(2)
     return dW, db
 
@@ -535,6 +545,7 @@ from .ops_idm import conv3d_t5_bwd, softmax_nll_bwd_grouped  # noqa: E402,F401  
 from .ops_rl import ewma_sums, ppo_coef, rl_head_bwd, value_bwd  # noqa: E402,F401  (RL fine-tuning ops, csrc/rl_bwd.cuh)
 from .ops_autograd import log_softmax_bwd  # noqa: E402,F401  (differentiable forward, csrc/log_softmax_bwd.cuh)
 from .ops_bptt import attention_bwd_state  # noqa: E402,F401  (gradients through the KV memory, csrc/attention_bwd.cuh)
+from .ops_pixel import conv3d_t5_dimg, firstconv_dimg  # noqa: E402,F401  (image gradients, csrc/firstconv_bwd.cuh, csrc/idm_bwd.cuh)
 
 
 # ---- on-device action codec (csrc/codec.cuh) -----------------------------------------------------------------------------

@@ -8,19 +8,19 @@ F32 = torch.float32
 
 
 def conv3d_t5_bwd(img, dy, C):
-    """Weight / bias gradient of `ops.conv3d_t5`: img u8 [B,T,H,W,3], dy bf16 ZP [B*T,H+1,W+1,C] = gradient wrt the conv3d output with
-    its ReLU mask already applied -> (dW fp32 [C][15] in (dt, c) order for the /255-scaled kernel weights, db fp32 [C])."""
+    """Weight / bias gradient of `ops.conv3d_t5`: img u8 or fp32 [B,T,H,W,3], dy bf16 ZP [B*T,H+1,W+1,C] = gradient wrt the conv3d output
+    with its ReLU mask already applied -> (dW fp32 [C][15] in (dt, c) order for the /255-scaled kernel weights, db fp32 [C])."""
     ops._cuda(img, dy)
-    if img.dtype != torch.uint8 or img.dim() != 5 or img.shape[-1] != 3 or not img.is_contiguous():
-        raise ValueError(f"conv3d_t5_bwd: img must be contiguous u8 [B,T,H,W,3] (got {img.dtype} {tuple(img.shape)})")
+    if img.dtype not in (torch.uint8, F32) or img.dim() != 5 or img.shape[-1] != 3 or not img.is_contiguous():
+        raise ValueError(f"conv3d_t5_bwd: img must be contiguous u8 or fp32 [B,T,H,W,3] (got {img.dtype} {tuple(img.shape)})")
     B, T, H, W, _ = img.shape
     if dy.dtype != torch.bfloat16 or tuple(dy.shape) != (B * T, H + 1, W + 1, C) or not dy.is_contiguous():
         raise ValueError(f"conv3d_t5_bwd: dy must be contiguous bf16 {(B * T, H + 1, W + 1, C)} (got {dy.dtype} {tuple(dy.shape)})")
     ws = torch.empty((max(nat.lib().vpt_conv3d_t5_bwd_workspace(B * T, H, W, C), 1),), dtype=F32, device=img.device)
     dW = torch.empty((C, 15), dtype=F32, device=img.device)
     db = torch.empty((C,), dtype=F32, device=img.device)
-    nat.check(nat.lib().vpt_conv3d_t5_bwd(ops._p(img), ops._p(dy), ops._p(dW), ops._p(db), ops._p(ws), B, T, H, W, C, ops._stream()),
-              "vpt_conv3d_t5_bwd")
+    fn = "vpt_conv3d_t5_bwd_f32" if img.dtype == F32 else "vpt_conv3d_t5_bwd"
+    nat.check(getattr(nat.lib(), fn)(ops._p(img), ops._p(dy), ops._p(dW), ops._p(db), ops._p(ws), B, T, H, W, C, ops._stream()), fn)
     ops._count(2)
     return dW, db
 

@@ -371,11 +371,23 @@ class _Versioned:
         self.value, self.fp = value, _fingerprint(self.params())
 
 
-def _differentiable(module: nn.Module) -> bool:
+def _differentiable(module: nn.Module, img=None) -> bool:
     """The forward builds an autograd graph only when asked to (`set_autograd`), in grad mode outside inference mode, and when at least
-    one parameter requires grad; otherwise the inference path runs, bit for bit."""
+    one parameter or the image `img` requires grad; otherwise the inference path runs, bit for bit."""
     return module._autograd and torch.is_grad_enabled() and not torch.is_inference_mode_enabled() and \
-        any(p.requires_grad for p in module.parameters())
+        ((img is not None and img.requires_grad) or any(p.requires_grad for p in module.parameters()))
+
+
+def frames_f32(img):
+    """lib/policy.py:39-45 takes any frames `img.to(float32)` converts: uint8 frames stay uint8 (the kernels' u8 path), a floating
+    dtype (values on the uint8 scale, not clipped) becomes fp32 here, so that autograd carries the gradient of a float16 / bfloat16 /
+    float64 leaf back in its own dtype.  Other integer dtypes raise TypeError."""
+    if img.dtype == torch.uint8:
+        return img
+    if not img.dtype.is_floating_point:
+        raise TypeError(f"ob['img'] must be uint8 or a floating dtype on the uint8 scale (B,T,H,W,3) as in the reference (lib/policy.py:39-45); "
+                        f"got {img.dtype}")
+    return img.to(torch.float32)
 
 
 def check_recompute_frames(v):
@@ -638,8 +650,7 @@ class MinecraftPolicy(nn.Module):
     def _forward_impl(self, img, first, state_in):
         cfg = self.cfg
         ops.require_cuda(img)
-        if img.dtype != torch.uint8:
-            raise TypeError("ob['img'] must be uint8 (B,T,H,W,3) as in the reference (lib/policy.py:39-45)")
+        img = frames_f32(img)
         B, t = img.shape[:2]
         frame_shape = (cfg.img_shape[0], cfg.img_shape[1], 3)
         assert tuple(img.shape[2:]) == frame_shape, f"img shape {tuple(img.shape[2:])} != {frame_shape}"
@@ -709,7 +720,7 @@ class MinecraftPolicy(nn.Module):
     def forward(self, ob, state_in, context):
         """lib/policy.py:193-218."""
         first = context["first"]
-        if _differentiable(self):
+        if _differentiable(self, ob["img"]):
             (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
         else:
             _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
@@ -731,7 +742,7 @@ class InverseActionNet(MinecraftPolicy):
     def forward(self, ob, state_in, context):
         """lib/policy.py:374-392 -> ((pi_latent, None), state_out)."""
         first = context["first"]
-        if _differentiable(self):
+        if _differentiable(self, ob["img"]):
             (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
         else:
             _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
@@ -807,7 +818,11 @@ class _PolicyBase(nn.Module):
 
         Frozen parameters (requires_grad=False when the forward runs) get no gradient and the backward skips the work that only served
         them, stopping at the lowest unit that trains; with the ImpalaCNN frozen the forward keeps none of its activations and the
-        stored-tape frame limit does not apply."""
+        stored-tape frame limit does not apply.
+
+        An `img` that requires grad (a floating dtype on the uint8 scale, `frames_f32`) makes the forward differentiable even with every
+        parameter frozen, and `loss.backward()` then writes `img.grad`; the trainable parameters' gradients are those of the same call
+        without it, bit for bit."""
         recompute_frames = check_recompute_frames(recompute_frames)
         self._autograd = bool(on)
         self._state_grad = bool(on) and bool(state_grad)
@@ -995,7 +1010,7 @@ class MinecraftAgentPolicy(_PolicyBase):
             mask = obs.pop("mask", None)
         else:
             mask = None
-        if _differentiable(self):
+        if _differentiable(self, obs["img"]):
             outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
             pi_logits = OrderedDict(zip(self.head_specs, outs[:-1]))
             return (pi_logits, outs[-1], None), state_out
@@ -1091,7 +1106,7 @@ class InverseActionPolicy(_PolicyBase):
             mask = obs.pop("mask", None)
         else:
             mask = None
-        if _differentiable(self):
+        if _differentiable(self, obs["img"]):
             outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
             return (OrderedDict(zip(self.head_specs, outs)), None, None), state_out
         lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in)

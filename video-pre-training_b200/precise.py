@@ -104,7 +104,7 @@ def forward(net, img, first, state_in):
     B, t = img.shape[:2]
     N = B * t
     H, W = cfg.img_shape[0], cfg.img_shape[1]
-    frames = img.reshape(N, H, W, 3).contiguous()
+    frames = img.reshape(N, H, W, 3).contiguous()  # (uint8 or fp32: policy.frames_f32)
     first_u8 = first.to(device=img.device, dtype=torch.bool).contiguous().view(torch.uint8)
     # ---------------- ImpalaCNN (lib/impala_cnn.py:187-195), NHWC fp32 activations
     x, cin = None, 3

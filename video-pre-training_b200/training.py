@@ -126,10 +126,11 @@ class _Trainer:
         pol = self.policy
         return [] if pol is None else [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
 
-    def _grad_plan(self, want_dmem=None):
+    def _grad_plan(self, want_dmem=None, want_dimg=False):
         """What the backward of a forward starting now does, from the parameters' `requires_grad` (and, with `state_grad`, from whether
-        each layer's state_in K / V gradient is wanted) -> dict(train: ids of the parameters that train, lowest: the place in
-        `_grad_units` order of the lowest unit that needs a gradient (the heads: len(units); nothing: len(units) + 1), stacks_from /
+        each layer's state_in K / V gradient is wanted; `want_dimg`: the image gradient is wanted, which, like a wanted input gradient of
+        unit 0, puts `lowest` below every unit) -> dict(train: ids of the parameters that train, lowest: the place in
+        `_grad_units` order of the lowest unit that needs a gradient (the image: -1; the heads: len(units); nothing: len(units) + 1), stacks_from /
         blocks_from: the first CNN stack / transformer block whose activations the backward reads (their count: none), cnn: whether
         the backward enters the CNN)."""
         net, cfg, units = self.net, self.net.cfg, self._units
@@ -141,12 +142,14 @@ class _Trainer:
         for l, want in enumerate(want_dmem or ()):
             if want:  # the attention backward of layer l gives its state_in gradient
                 lowest = min(lowest, self._pos[f"recurrent_layer.blocks.{l}.r.orc_block.b_nd"])
+        if want_dimg:
+            lowest = -1
         nst = len(cfg.chans)
         stacks_from = next((i for i in range(nst) if lowest <= self._pos[f"img_process.cnn.stacks.{i}.blocks.1.conv1."]), nst)
         blocks_from = next((l for l in range(cfg.n_layers) if lowest <= self._pos[f"recurrent_layer.blocks.{l}.mlp1."]), cfg.n_layers)
         if not net.use_lastlayer and lowest <= self._pos["final_ln."]:
             blocks_from = min(blocks_from, cfg.n_layers - 1)  # final_ln reads the last block's output
-        return dict(train=train, lowest=lowest, stacks_from=stacks_from, blocks_from=blocks_from, cnn=stacks_from < nst)
+        return dict(train=train, lowest=lowest, stacks_from=stacks_from, blocks_from=blocks_from, cnn=stacks_from < nst, want_dimg=want_dimg)
 
     def _use_plan(self, tape):
         self._train, self._lowest = tape["train"], tape["lowest"]
@@ -254,12 +257,12 @@ class _Trainer:
             raise NotImplementedError(f"{type(self).__name__}: at most {self.max_call_frames} frames and B <= {self.max_call_batch} per call "
                                       f"(got B = {B}, T = {t})")
 
-    def _taped_latent(self, img, first, state_in, want_dmem=None):
+    def _taped_latent(self, img, first, state_in, want_dmem=None, want_dimg=False):
         """The network's inference kernels, recording what the backward needs -> (latent bf16 [N][h], latent fp32 (B,t,h), tape, state_out).
         The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`, `heads_t`), and
-        the backward's `_grad_plan` (want_dmem: see there)."""
+        the backward's `_grad_plan` (want_dmem, want_dimg: see there)."""
         net, pol = self.net, self.policy
-        tape = self._grad_plan(want_dmem)
+        tape = self._grad_plan(want_dmem, want_dimg)
         self.check_call_frames(img, tape)
         if pol is not None:
             pol.refresh_weights()  # (a bare network: the getters rebuild eagerly on use)
@@ -278,10 +281,10 @@ class _Trainer:
             self.last_tape = tape
         return lat_bf16, lat_f32, tape, state_out
 
-    def _taped_forward(self, img, first, state_in, mask=None, want_dmem=None):
+    def _taped_forward(self, img, first, state_in, mask=None, want_dmem=None, want_dimg=False):
         """The inference kernels, recording what the backward needs -> (latent bf16, pd, vpred, tape, state_out)."""
         B, t = img.shape[:2]
-        lat_bf16, _, tape, state_out = self._taped_latent(img, first, state_in, want_dmem)
+        lat_bf16, _, tape, state_out = self._taped_latent(img, first, state_in, want_dmem, want_dimg)
         pd, vpred = self.policy._heads(lat_bf16, B, t, mask)
         return lat_bf16, pd, vpred, tape, state_out
 
@@ -317,7 +320,8 @@ class _Trainer:
         ImpalaCNN and, for the IDM, the conv3d pre-stage.  dstate: None or per layer None / (dk, dv), the gradient wrt that layer's
         state_out K / V; want_dmem: None or per layer whether its state_in gradient is wanted.  Returns per layer (dmem_k, dmem_v) or None.
         Each stage runs only while a unit at or below it needs a gradient (`_grad_plan`); `upper_grads_ready` is called once, before the
-        CNN or, when the backward does not enter it, at its end."""
+        CNN or, when the backward does not enter it, at its end.  With the image gradient wanted (`_grad_plan`'s want_dimg) it is left in
+        tape["dimg"], fp32 [N, H, W, 3] on the uint8 scale."""
         self._use_plan(tape)
         net = self.net
         cfg = net.cfg
@@ -352,19 +356,40 @@ class _Trainer:
         # ---------------- ImpalaCNN, last stack to first, chunk by chunk (last chunk first) ----------------
         # The stored tape is the one-chunk case: its per-stack activations come from the forward.  With `recompute` every chunk's are made
         # again from the frames and the forward's weights, used, and dropped before the next chunk.  (No chunk when the CNN is frozen.)
+        # The gradient wrt the CNN input (`_cnn_bwd`) is the image gradient for the agent's fused first conv, and for the IDM the gradient
+        # wrt the conv3d output, which its own backward takes to the weights and, when wanted, to the image; each chunk writes its frames'.
         frames = tape["frames"]
-        for f0, f1 in reversed(tape["cnn_chunks"]):
+        chunks = tape["cnn_chunks"]
+        dimg = None
+        if tape["want_dimg"] and len(chunks) > 1:
+            dimg = torch.empty((frames.shape[0], *frames.shape[1:3], 3), dtype=F32, device=frames.device)
+        for f0, f1 in reversed(chunks):
             ct = tape if tape["recompute"] is None else self._recompute_cnn(tape, f0, f1, t)
             dx3 = self._cnn_bwd(dcnn[f0:f1], ct, wts, P)
             del ct
-            if cfg.conv3d_out is not None and dx3 is not None:
+            di = None
+            if cfg.conv3d_out is None:
+                di = dx3
+            elif dx3 is not None:
                 # the IDM's conv3d pre-stage: kernel weights are W_ref[C][c][dt] / 255 laid out [C][dt][c] (policy._Prepared)
                 C3 = cfg.conv3d_out
-                dW3, db3 = ops.conv3d_t5_bwd(frames[f0:f1].view((f1 - f0) // t, t, *frames.shape[1:]), dx3, C3)
-                self._grad(net.conv3d_layer.layer.weight, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
-                self._grad(net.conv3d_layer.layer.bias, db3)
+                w3, b3 = net.conv3d_layer.layer.weight, net.conv3d_layer.layer.bias
+                if self._trains(w3) or self._trains(b3):
+                    dW3, db3 = ops.conv3d_t5_bwd(frames[f0:f1].view((f1 - f0) // t, t, *frames.shape[1:]), dx3, C3)
+                    self._grad(w3, (dW3 / 255.0).view(C3, 5, 3).permute(0, 2, 1))
+                    self._grad(b3, db3)
+                if tape["want_dimg"]:
+                    di = ops.conv3d_t5_dimg(dx3, tape["prep"].conv3d[0], (f1 - f0) // t, t, *frames.shape[1:3])
             del dx3
+            if di is not None:
+                if dimg is None:
+                    dimg = di
+                else:
+                    dimg[f0:f1] = di
+            del di
         del dcnn
+        if tape["want_dimg"]:
+            tape["dimg"] = dimg
         return dmem
 
     def _recompute_cnn(self, tape, f0, f1, t):
@@ -485,8 +510,9 @@ class _Trainer:
 
     def _cnn_bwd(self, dout, tape, wts, P):
         """Backward of lib/impala_cnn.py:187-195; `dout` is the gradient wrt the last stack's output (ZP).  Returns the gradient wrt the
-        CNN input when stack 0's first conv is a normalised one and the conv3d pre-stage trains (the IDM: the conv3d output, ReLU backward
-        applied), else None.  Stops at the lowest unit that needs a gradient."""
+        CNN input when a unit below needs it: when stack 0's first conv is a normalised one (the IDM) the gradient wrt the conv3d output,
+        ReLU backward applied; for the fused first conv the image gradient (fp32 [F, H, W, 3]), when it is wanted; else None.  Stops at the
+        lowest unit that needs a gradient."""
         cfg = self.net.cfg
         pfx = "img_process.cnn"
         dx = dout
@@ -520,11 +546,13 @@ class _Trainer:
             dy1 = dy1.view(rec["y1"].shape)
             if i == 0 and not cfg.first_conv_norm:
                 st = tape["prep"].stacks[0]  # (the weights the forward used)
-                dWk, db = ops.firstconv_bwd(tape["frames"], st["fc_w"], st["fc_b"], dy1, C)
-                # kernel weights are W[c0][ky][kx][c] / 255 (lib/policy.py:44 folded in)
-                self._grad(P[f"{s}.firstconv.layer.weight"], (dWk / 255.0).view(C, 3, 3, 3).permute(0, 3, 1, 2))
-                self._grad(P[f"{s}.firstconv.layer.bias"], db)
-                return None
+                wp, bp = P[f"{s}.firstconv.layer.weight"], P[f"{s}.firstconv.layer.bias"]
+                if self._trains(wp) or self._trains(bp):
+                    dWk, db = ops.firstconv_bwd(tape["frames"], st["fc_w"], st["fc_b"], dy1, C)
+                    # kernel weights are W[c0][ky][kx][c] / 255 (lib/policy.py:44 folded in)
+                    self._grad(wp, (dWk / 255.0).view(C, 3, 3, 3).permute(0, 3, 1, 2))
+                    self._grad(bp, db)
+                return ops.firstconv_dimg(tape["frames"], st["fc_w"], st["fc_b"], dy1, C) if self._lowest < 0 else None
             dfull = ops.maxpool3s2_bwd(dy1, rec["full"])  # includes the ReLU in front of the pool
             del dy1
             # (IDM stack 0: the input is the ReLU output of the conv3d pre-stage; its ReLU backward rides on this norm's apply pass)
@@ -788,14 +816,15 @@ class _AutogradRunner(_Trainer):
         return bool(getattr(self.module, "_state_grad", False)) and self.net.cfg.maxlen > 0
 
     def check(self, img, state_in):
-        """The limits of one differentiable call, checked before any work."""
+        """The limits of one differentiable call, checked before any work (`img` requiring grad asks for the image gradient)."""
         net = self.net
         if net.precision != "bf16":
             raise NotImplementedError("the differentiable forward runs in the bf16 mode only (set_precision('bf16'))")
         B, t = img.shape[:2]
         N = B * t
         self.recompute_frames = self.module._recompute_frames  # set_autograd(.., recompute_frames=..)
-        stored = self.recompute_frames is None and self._grad_plan()["cnn"]  # (a frozen CNN keeps no activations)
+        plan = self._grad_plan(want_dimg=img.requires_grad)
+        stored = self.recompute_frames is None and plan["cnn"]  # (a frozen CNN keeps no activations)
         if net.cfg.conv3d_out is None:
             if stored and N > net.cnn_chunk_frames:
                 raise NotImplementedError(f"differentiable forward: at most {net.cnn_chunk_frames} frames per call (got B*T = {N}); "
@@ -806,7 +835,7 @@ class _AutogradRunner(_Trainer):
                                           "accumulate over calls or set_autograd(True, recompute_frames=...)")
             if t > IDMTrainer.max_t:
                 raise NotImplementedError(f"differentiable forward: at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
-        self.check_call_frames(img)
+        self.check_call_frames(img, plan)
         if self.state_grad():
             return
         for _, (k, v) in state_in:
@@ -817,13 +846,19 @@ class _AutogradRunner(_Trainer):
 
     def run(self, img, first, state_in, mask=None):
         """-> (outputs, state_out): outputs attached to the graph (pd per head [+ vpred], or the latent); state_out detached, or with
-        `state_grad` its K / V attached (state_mask is a plain bool tensor either way)."""
+        `state_grad` its K / V attached (state_mask is a plain bool tensor either way).  An `img` that requires grad is one more input (its
+        fp32 copy, `policy.frames_f32`, so that autograd casts the gradient back to the leaf's dtype) whose gradient the backward returns."""
+        from .policy import frames_f32
+
         self.check(img, state_in)
         params = [p for p in self.module.parameters()]
         sg = self.state_grad()
         kv = [x for _, (k, v) in state_in for x in (k, v)] if sg else []
-        box = dict(img=img, first=first, state_in=state_in, mask=mask, state_grad=sg)
-        outs = _TapedForward.apply(self, box, *params, *kv)
+        ig = img.requires_grad
+        if ig:
+            img = frames_f32(img)
+        box = dict(img=img, first=first, state_in=state_in, mask=mask, state_grad=sg, img_grad=ig)
+        outs = _TapedForward.apply(self, box, *params, *kv, *((img,) if ig else ()))
         outs = (outs,) if isinstance(outs, torch.Tensor) else outs
         if not sg:
             return outs, box["state_out"]
@@ -837,12 +872,13 @@ class _AutogradRunner(_Trainer):
         B, t = img.shape[:2]
         # with state_grad, a state_in K / V that requires grad is an input whose gradient the backward returns
         want = [k.requires_grad or v.requires_grad for _, (k, v) in box["state_in"]] if box["state_grad"] else None
+        ig = box["img_grad"]
         if self.policy is None:
-            lat_bf16, lat_f32, tape, state_out = self._taped_latent(img, box["first"], box["state_in"], want)
+            lat_bf16, lat_f32, tape, state_out = self._taped_latent(img, box["first"], box["state_in"], want, ig)
             outs = (lat_f32,)
         else:
             mask = box["mask"]
-            lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, box["first"], box["state_in"], mask, want)
+            lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, box["first"], box["state_in"], mask, want, ig)
             outs = tuple(pd.values()) + ((vpred,) if vpred is not None else ())
             masks = {}
             for name, (shape, n) in self.policy.head_specs.items():
@@ -908,17 +944,19 @@ def _aligned_f32(x):
 
 
 class _TapedForward(torch.autograd.Function):
-    """forward(runner, box, *params[, *state K / V]): the taped forward; the tape lives in ctx until the backward frees it.  The parameters
-    are inputs (saved, so that an in-place change before the backward raises torch's version-check error); the kernel-layout weights the
-    forward used are in the tape, so the backward never re-lays out newer parameters.  With `box["state_grad"]` the state_in K / V of
-    every layer follow the parameters as inputs, and the state_out K / V follow the outputs."""
+    """forward(runner, box, *params[, *state K / V][, img]): the taped forward; the tape lives in ctx until the backward frees it.  The
+    parameters are inputs (saved, so that an in-place change before the backward raises torch's version-check error); the kernel-layout
+    weights the forward used are in the tape, so the backward never re-lays out newer parameters.  With `box["state_grad"]` the state_in
+    K / V of every layer follow the parameters as inputs, and the state_out K / V follow the outputs.  With `box["img_grad"]` the fp32
+    frames are the last input and the backward returns the image gradient for them."""
 
     @staticmethod
     def forward(ctx, runner, box, *inputs):
         ctx.set_materialize_grads(False)
         outs, tape = runner.forward_outputs(box)
-        n_params = len(inputs) - (2 * len(box["state_in"]) if box["state_grad"] else 0)
+        n_params = len(inputs) - (2 * len(box["state_in"]) if box["state_grad"] else 0) - (1 if box["img_grad"] else 0)
         ctx.runner, ctx.tape, ctx.n_params, ctx.n_outs = runner, tape, n_params, len(outs)
+        ctx.img_shape = tuple(box["img"].shape) if box["img_grad"] else None
         ctx.save_for_backward(*inputs[:n_params], *outs)
         if box["state_grad"]:
             outs = outs + tuple(x for _, (k, v) in box["state_out"] for x in (k, v))
@@ -942,6 +980,7 @@ class _TapedForward(torch.autograd.Function):
             dstate = [None if d is None else tuple(None if x is None else _aligned_f32(x) for x in d) for d in dstate]
             want_dmem = [need[2 * l] or need[2 * l + 1] for l in range(L)]
         sink, dmem = ctx.runner.backward_grads(tape, outs, grads[:ctx.n_outs], dstate, want_dmem)
+        dimg = tape.get("dimg")
         del tape
         mods = list(ctx.runner.module.parameters())
         res = [sink.get(id(p)) if ctx.needs_input_grad[2 + i] else None for i, p in enumerate(mods)]
@@ -949,4 +988,6 @@ class _TapedForward(torch.autograd.Function):
             need = ctx.needs_input_grad[2 + ctx.n_params:]
             for l, d in enumerate(dmem):
                 res += [d[0] if d is not None and need[2 * l] else None, d[1] if d is not None and need[2 * l + 1] else None]
+        if ctx.img_shape is not None:
+            res.append(dimg.view(ctx.img_shape) if ctx.needs_input_grad[-1] else None)
         return (None, None) + tuple(res)
