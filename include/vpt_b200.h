@@ -206,7 +206,8 @@ int vpt_codec_from_env(const int64_t* buttons, const double* camera, const doubl
  *   vpt_maxpool3s2_f32    max_pool2d(3, 2, 1) on NHWC fp32 [F][H][W][C] -> [F][H/2][W/2][C] (lib/impala_cnn.py:117)
  *   vpt_attention_f32     lib/xf.py:18-71 with the mask of lib/masked_attention.py:11-94 and the relative term of lib/xf.py:265-271:
  *                         q [B*t][h], full_k / full_v [B][maxlen+t][h], R [B*t][10*heads] or NULL, b_nd [10][maxlen], first u8 [B][t],
- *                         state_mask u8 [B][maxlen] or NULL (= all False), out [B*t][h]; head_dim 128; causal = clipped_causal mask
+ *                         state_mask u8 [B][maxlen] or NULL (= all False), out [B*t][h]; head_dim 128; causal = clipped_causal mask;
+ *                         maxlen + t <= 51200 (one query's scores in shared memory)
  * -------------------------------------------------------------------------------------------------------- */
 int vpt_group_stats_f32(const float* x, float* mr, int64_t groups, int64_t per_group, float eps, void* stream);
 int vpt_norm_split_f32(const float* x, const float* mr, const float* gamma, const float* beta, void* hi, void* lo, float* out_f32,
@@ -282,7 +283,9 @@ int vpt_state_mask_update(const uint8_t* mask_in, const uint8_t* first, int64_t 
  *   out   bf16 [B][t][h]
  * logit = q.k / 128 + sum_n R[i][n] b_nd[n][d] over allowed keys, d = maxlen + i - j in [0, maxlen),
  * allowed = j >= maxlen || (!first[b] && smask[b][j]).   causal = 0 selects the IDM variant (mask "none":
- * every chunk key visible, no memory, no relative bias; lib/policy.py:342-392). */
+ * every chunk key visible, no memory, no relative bias; lib/policy.py:342-392).
+ * Any maxlen: bands whose [64][maxlen] bias table does not fit shared memory (maxlen > 598 with nbasis 10) run the key-tiled kernels of
+ * csrc/attention_long.cuh (nbasis <= 10; t = 1 calls split each band across a thread-block cluster), the rest the original kernel. */
 int vpt_attention(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
                   const uint8_t* first, int64_t first_stride, const uint8_t* smask, void* out, int32_t B, int32_t t,
                   int32_t maxlen, int32_t heads, int32_t nbasis, int32_t causal, void* stream);
@@ -393,7 +396,8 @@ int vpt_firstconv_dimg(const void* img, int32_t img_f32, const float* w, const f
                        int32_t H, int32_t W, int32_t C0, void* stream);
 /* Backward of vpt_attention (causal policy attention): given dO bf16 [B*t][h] writes d q | d k | d v | d R side by side into
  * out bf16 [B*t][ld_out] at columns 0 | h | 2h | 3h (chunk rows only -- the KV memory is detached state,
- * behavioural_cloning.py:111) and d b_nd fp32 [nbasis][maxlen].  workspace: 2*B*heads*t*maxlen floats.   lib/xf.py:18-71,265-271 */
+ * behavioural_cloning.py:111) and d b_nd fp32 [nbasis][maxlen].  workspace: 2*B*heads*t*maxlen floats.   lib/xf.py:18-71,265-271
+ * Any maxlen >= 1 (nbasis <= 10): up to 128 the band is staged whole, above it in 64-row tiles (csrc/attention_long.cuh). */
 int vpt_attention_bwd(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
                       int64_t first_stride, const uint8_t* smask, const void* dO, void* out, int64_t ld_out, float* db_nd, float* workspace,
                       int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream);

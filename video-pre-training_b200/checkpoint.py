@@ -3,6 +3,8 @@
     .model    pickle holding the constructor arguments of the policy            run_agent.py:11-14, behavioural_cloning.py:42-47
     .weights  torch.save of MinecraftAgentPolicy.state_dict()                    agent.py:132-135, behavioural_cloning.py:131-132
     training  state_dict + FlatAdamDP state (moments, step count) in one file    (the reference saves weights only)
+
+`resize_memory` adapts a state dict to another KV-memory length (`attention_memory_size - timesteps`).
 """
 import pickle
 
@@ -34,6 +36,26 @@ def load_weights(policy, path, map_location=None):
     In-place copies, so it also works after FlatAdamDP has re-pointed the parameters into its flat bucket."""
     sd = torch.load(path, map_location=map_location or "cpu")
     return policy.load_state_dict(sd, strict=False)
+
+
+def resize_memory(state_dict, maxlen):
+    """A copy of `state_dict` whose relative-position biases (every `...orc_block.b_nd`, shape (nbasis, old maxlen)) are cut or
+    zero-padded to (nbasis, maxlen), so that weights trained with one memory length load into a policy built with another
+    (`load_state_dict` raises on the shape mismatch otherwise, even with strict=False).  Distance d keeps its column; distances the
+    checkpoint never trained get no relative bias.  Every other entry is the same tensor object."""
+    maxlen = int(maxlen)
+    if maxlen < 0:
+        raise ValueError(f"resize_memory: maxlen must be >= 0 (got {maxlen})")
+    out = dict(state_dict)
+    for k, v in state_dict.items():
+        if k.endswith("orc_block.b_nd"):
+            if v.dim() != 2:
+                raise ValueError(f"resize_memory: {k} has shape {tuple(v.shape)}, expected (nbasis, maxlen)")
+            w = v.new_zeros((v.shape[0], maxlen))
+            n = min(maxlen, v.shape[1])
+            w[:, :n] = v[:, :n]
+            out[k] = w
+    return out
 
 
 def save_training_state(path, policy, optimizer):

@@ -223,6 +223,11 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
     }
 }
 
+// attention_long.cuh: the causal forward for a KV memory whose bias table does not fit this kernel's shared memory
+int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
+                       const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
+                       int nbasis, cudaStream_t stream);
+
 }  // namespace vpt
 
 extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
@@ -236,7 +241,11 @@ extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, cons
     const int nb = causal ? nbasis : 0;
     size_t smem = (size_t)(kAttBQ + 2 * kAttBK) * kAttPitch * 2 + ((size_t)kAttBQ * maxlen + (size_t)nb * maxlen + (size_t)kAttBQ * nb) * 4 +
                   (size_t)((maxlen + 15) / 16 * 16) + 16;
-    VPT_CHECK(smem <= 227 * 1024, "vpt_attention: maxlen=%d too large for the shared-memory budget", maxlen);
+    if (smem > 227 * 1024) {  // only a causal band can be this long (mask 'none' has no memory): tile it over keys
+        return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf),
+                                  reinterpret_cast<const __nv_bfloat16*>(Vf), R, ld_r, b_nd, first, first_stride, smask,
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, (cudaStream_t)stream);
+    }
     static size_t attr = 0;
     if (smem > attr) {
         VPT_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

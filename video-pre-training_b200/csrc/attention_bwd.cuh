@@ -334,6 +334,15 @@ __global__ void __launch_bounds__(256) attn_bwd_bnd_kernel(const float* __restri
     }
 }
 
+// attention_long.cuh: the backward for maxlen > 32 * kAbMaxPerLane
+int attention_bwd_long(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
+                       const uint8_t* first, long long first_stride, const uint8_t* smask, const __nv_bfloat16* dO, __nv_bfloat16* out,
+                       long long ld_out, float* wsP, float* wsS, int B, int t, int maxlen, int heads, int nbasis, const float* dstate_k,
+                       const float* dstate_v, cudaStream_t stream);
+int attention_bwd_long_mem(const __nv_bfloat16* Q, const __nv_bfloat16* dO, const float* wsP, const float* wsS, const uint8_t* first,
+                           long long first_stride, const uint8_t* smask, const float* dstate_k, const float* dstate_v, float* dmem_k, float* dmem_v,
+                           int B, int t, int maxlen, int heads, cudaStream_t stream);
+
 }  // namespace vpt
 
 extern "C" int vpt_attention_bwd_state(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
@@ -342,7 +351,7 @@ extern "C" int vpt_attention_bwd_state(const void* Q, const void* Kf, const void
                                        const float* dstate_k, const float* dstate_v, float* dmem_k, float* dmem_v, void* stream) {
     using namespace vpt;
     VPT_CHECK(Q && Kf && Vf && R && b_nd && first && dO && out && db_nd && workspace, "vpt_attention_bwd: null argument");
-    VPT_CHECK(B > 0 && B <= 65535 && t > 0 && heads > 0 && maxlen > 0 && maxlen <= 32 * kAbMaxPerLane && nbasis > 0 && nbasis <= 10,
+    VPT_CHECK(B > 0 && B <= 65535 && t > 0 && heads > 0 && maxlen > 0 && nbasis > 0 && nbasis <= 10,
               "vpt_attention_bwd: unsupported shape (B=%d t=%d maxlen=%d heads=%d nbasis=%d)", B, t, maxlen, heads, nbasis);
     VPT_CHECK(ld_out % 4 == 0 && ld_out >= 3 * (int64_t)heads * kAbD + heads * nbasis, "vpt_attention_bwd: gradient buffer too narrow");
     VPT_CHECK((dmem_k == nullptr) == (dmem_v == nullptr), "vpt_attention_bwd_state: dmem_k and dmem_v are given together or not at all");
@@ -351,6 +360,18 @@ extern "C" int vpt_attention_bwd_state(const void* Q, const void* Kf, const void
     const size_t ws_half = (size_t)B * heads * t * maxlen;
     float* wsP = workspace;
     float* wsS = workspace + ws_half;
+    if (maxlen > 32 * kAbMaxPerLane) {  // longer memories: the band-tiled kernels of attention_long.cuh
+        const int rc = attention_bwd_long(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf),
+                                          reinterpret_cast<const __nv_bfloat16*>(Vf), R, ld_r, b_nd, first, first_stride, smask,
+                                          reinterpret_cast<const __nv_bfloat16*>(dO), reinterpret_cast<__nv_bfloat16*>(out), ld_out, wsP, wsS, B, t,
+                                          maxlen, heads, nbasis, dstate_k, dstate_v, (cudaStream_t)stream);
+        if (rc != VPT_OK) return rc;
+        attn_bwd_bnd_kernel<<<maxlen, 256, 0, (cudaStream_t)stream>>>(R, ld_r, wsS, db_nd, B, t, maxlen, heads, nbasis);
+        VPT_LAUNCH_CHECK();
+        if (dmem_k == nullptr) return VPT_OK;
+        return attention_bwd_long_mem(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(dO), wsP, wsS, first,
+                                      first_stride, smask, dstate_k, dstate_v, dmem_k, dmem_v, B, t, maxlen, heads, (cudaStream_t)stream);
+    }
     const int nk = maxlen + kAbRows - 1;
     const size_t smem_rows = (size_t)(2 * nk + 2 * kAbRows) * kAbPitch * 2 + ((size_t)nbasis * maxlen + (size_t)kAbRows * maxlen) * 4 + maxlen + 16;
     const size_t smem_keys = (size_t)(2 * nk) * kAbPitch * 2;

@@ -99,12 +99,12 @@ __global__ void __launch_bounds__(128) attention_f32_kernel(const float* __restr
                                                               const float* __restrict__ R, const float* __restrict__ b_nd, const uint8_t* __restrict__ first,
                                                               const uint8_t* __restrict__ smask, float* __restrict__ out, int B, int t, int maxlen,
                                                               int heads, int causal) {
-    constexpr int DH = 128, NB = 10, MAXT = 512;
+    constexpr int DH = 128, NB = 10;
     const int T = maxlen + t;
     const int i = blockIdx.x % t, hd = (blockIdx.x / t) % heads, b = blockIdx.x / (t * heads);
     const int h = heads * DH;
     __shared__ float sq[DH];
-    __shared__ float sp[MAXT];
+    extern __shared__ float sp[];  // [maxlen + t] logits, then probabilities
     __shared__ float sr[NB];
     __shared__ float red[4];
     const int tid = threadIdx.x;
@@ -196,9 +196,15 @@ extern "C" int vpt_attention_f32(const float* q, const float* full_k, const floa
                                  void* stream) {
     using namespace vpt;
     VPT_CHECK(q && full_k && full_v && out && B > 0 && t > 0 && heads > 0 && maxlen >= 0, "vpt_attention_f32: bad argument");
-    VPT_CHECK(maxlen + t <= 512, "vpt_attention_f32: at most 512 keys per query (maxlen=%d t=%d)", maxlen, t);
+    const size_t smem = (size_t)(maxlen + t) * 4;  // the score row of one query
+    VPT_CHECK(smem <= 200 * 1024, "vpt_attention_f32: at most %d keys per query (maxlen=%d t=%d)", 200 * 1024 / 4, maxlen, t);
     VPT_CHECK(!causal || (first && (!R || b_nd)), "vpt_attention_f32: causal attention needs `first` (and b_nd with R)");
-    attention_f32_kernel<<<(unsigned)(B * heads * t), 128, 0, (cudaStream_t)stream>>>(q, full_k, full_v, R, b_nd, first, state_mask, out, B, t, maxlen, heads,
+    static size_t attr = 0;
+    if (smem > 48 * 1024 && smem > attr) {
+        VPT_CUDA(cudaFuncSetAttribute(attention_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        attr = 200 * 1024;
+    }
+    attention_f32_kernel<<<(unsigned)(B * heads * t), 128, smem, (cudaStream_t)stream>>>(q, full_k, full_v, R, b_nd, first, state_mask, out, B, t, maxlen, heads,
                                                                                       causal);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
