@@ -461,6 +461,12 @@ int vpt_ppo_coef(const float* lp, const float* old_lp, const float* adv, int64_t
  *   kl[r] (+)= sum_j exp(logq_j) * (logq_j - logp_j)   (fp32, fixed order; 0 without logq)             lib/action_head.py:209-220 */
 int vpt_rl_head_bwd(const float* logp, int64_t ld_logp, const float* logq, int64_t ld_logq, const int64_t* idx, const float* c, float k,
                     float inv_temp, int32_t n, void* out, int64_t ld_out, int32_t col0, float* kl, int32_t accumulate, int64_t rows, void* stream);
+/* vpt_rl_head_bwd with the entropy bonus (loss - ent_coef * mean H): with H[r] = -sum_j exp(logp_j) * logp_j (fp32, fixed order),
+ *   out[r][col0 + j] = (c[r] * (p - [j == idx[r]]) + k * (p - q) + e * p * (logp_j + H[r])) * inv_temp   (bf16; e = ent_coef / N, the term
+ *                      skipped when e == 0, so that the bits are vpt_rl_head_bwd's),   kl[r] (+)= as above,   ent[r] (+)= H[r]   (fp32) */
+int vpt_rl_head_bwd_ent(const float* logp, int64_t ld_logp, const float* logq, int64_t ld_logq, const int64_t* idx, const float* c, float k,
+                        float e, float inv_temp, int32_t n, void* out, int64_t ld_out, int32_t col0, float* kl, float* ent, int32_t accumulate,
+                        int64_t rows, void* stream);
 /* sums float64 [2] = (sum x, sum x^2) over x fp32 [rows] (one block, fixed order) */
 int vpt_ewma_sums(const float* x, int64_t rows, double* sums, void* stream);
 /* Value head (lib/scaled_mse_head.py:37-43 in training mode): updates the EWMA normaliser in place from the batch statistics
@@ -481,6 +487,22 @@ int vpt_value_bwd(const float* vpred, const float* returns, const double* sums, 
  * Fixed-order sums, no atomics: bit-reproducible. */
 int vpt_log_softmax_bwd(const float* logp, int64_t ld_logp, const float* g, int64_t ld_g, const uint8_t* mask, int32_t groups, int32_t n, float scale,
                         void* out, int64_t ld_out, int32_t col0, int64_t rows, void* stream);
+
+/* ----------------------------------------------------------------------------------------------------------
+ * Distributions of the categorical heads (policy.py `pi_head.entropy` / `pi_head.kl_divergence`, lib/action_head.py:186-220).
+ * logp, logq fp32 [rows][ld], each row `groups` groups of n log-probs (the IDM's factored heads: groups > 1), summed over all of them:
+ *   vpt_head_entropy      ent[r] = -sum_j exp(logp[r][j]) * logp[r][j]
+ *   vpt_head_kl           kl[r]  =  sum_j exp(logq[r][j]) * (logq[r][j] - logp[r][j])                      (KL(q || p))
+ *   vpt_head_entropy_bwd  dlogp[r][j] = -g[r] * exp(logp) * (logp + 1)                                   (g = d loss / d ent, fp32 [rows])
+ *   vpt_head_kl_bwd       dlogq[r][j] =  g[r] * exp(logq) * (logq - logp + 1),  dlogp[r][j] = -g[r] * exp(logq)   (either may be NULL)
+ * fp32 throughout; one pass over the inputs, fixed-order sums, no atomics: bit-reproducible.
+ * ---------------------------------------------------------------------------------------------------------- */
+int vpt_head_entropy(const float* logp, int64_t ld, int32_t groups, int32_t n, float* ent, int64_t rows, void* stream);
+int vpt_head_kl(const float* logq, int64_t ld_q, const float* logp, int64_t ld_p, int32_t groups, int32_t n, float* kl, int64_t rows, void* stream);
+int vpt_head_entropy_bwd(const float* logp, int64_t ld, const float* g, int32_t groups, int32_t n, float* dlogp, int64_t ld_d, int64_t rows,
+                         void* stream);
+int vpt_head_kl_bwd(const float* logq, int64_t ld_q, const float* logp, int64_t ld_p, const float* g, int32_t groups, int32_t n, float* dlogq,
+                    int64_t ld_dq, float* dlogp, int64_t ld_dp, int64_t rows, void* stream);
 
 #ifdef __cplusplus
 }

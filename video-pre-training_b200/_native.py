@@ -149,6 +149,7 @@ SIGNATURES = {
     # RL fine-tuning (training.py, RLTrainer)
     "vpt_ppo_coef": (_I, [_P, _P, _P, _L, _F, _F, _F, _P, _P, _P, _P]),
     "vpt_rl_head_bwd": (_I, [_P, _L, _P, _L, _P, _P, _F, _F, _I, _P, _L, _I, _P, _I, _L, _P]),
+    "vpt_rl_head_bwd_ent": (_I, [_P, _L, _P, _L, _P, _P, _F, _F, _F, _I, _P, _L, _I, _P, _P, _I, _L, _P]),
     "vpt_ewma_sums": (_I, [_P, _L, _P, _P]),
     "vpt_value_bwd": (_I, [_P, _P, _P, _D, _P, _P, _P, _F, _F, _F, _P, _L, _I, _P, _L, _P]),
     # differentiable forward (training.py, set_autograd)
@@ -158,6 +159,11 @@ SIGNATURES = {
     "vpt_firstconv_dimg": (_I, [_P, _I, _P, _P, _P, _P, _L, _I, _I, _I, _P]),
     "vpt_conv3d_t5_bwd_f32": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "vpt_conv3d_t5_dimg": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    # distributions of the categorical heads (policy.py, pi_head.entropy / kl_divergence and their backward)
+    "vpt_head_entropy": (_I, [_P, _L, _I, _I, _P, _L, _P]),
+    "vpt_head_kl": (_I, [_P, _L, _P, _L, _I, _I, _P, _L, _P]),
+    "vpt_head_entropy_bwd": (_I, [_P, _L, _P, _I, _I, _P, _L, _L, _P]),
+    "vpt_head_kl_bwd": (_I, [_P, _L, _P, _L, _P, _I, _I, _P, _L, _P, _L, _L, _P]),
 }
 
 _lib = None

@@ -9,6 +9,8 @@
 //                   logits gradient, p = exp(logp), q = exp(logq) of the frozen reference policy (k * (p - q) dropped without it),
 //                   and the row's KL(q || p) = sum_j q_j (logq_j - logp_j) (fixed-order sum) for the statistics.
 //                   Bandwidth bound: one pass over logp (and logq), one bf16 write per column.
+//                   rl_head_bwd_ent: the same with the entropy bonus, loss - ent_coef * mean H(pi): one more read of logp for the row's
+//                   entropy H, then + ent_coef / N * p * (logp + H) in each column's gradient, and H per row for the statistics.
 //   ewma_sums       (sum, sum of squares) of the returns in float64, one block, fixed order (all-reduced by the caller under DP).
 //   value_bwd       one block: the EWMA normaliser update (lib/normalize_ewma.py:41-55, per_element_update = False) from those sums,
 //                   then per row the normalised target with the UPDATED statistics, dvpred = scale * (vpred - target) as bf16 into
@@ -33,17 +35,41 @@ __global__ void __launch_bounds__(256) ppo_coef_kernel(const float* __restrict__
     clipped[r] = clip ? 1.f : 0.f;
 }
 
-// TPR threads per row (32: one warp per row for small heads; 256: one block per row), 256 threads per block
-template <int TPR>
+// TPR threads per row (32: one warp per row for small heads; 256: one block per row), 256 threads per block.
+// ENT (vpt_rl_head_bwd_ent): a first pass gives the row's entropy H = -sum_j p_j logp_j (fixed order, every thread holds it), the second
+// adds e * p_j * (logp_j + H) to each column's gradient, the gradient of -ent_coef * mean H with e = ent_coef / N (skipped when e == 0:
+// adding +0 would turn a -0 gradient into +0), and the row's H is written to ent (accumulated like kl).
+template <int TPR, bool ENT = false>
 __global__ void __launch_bounds__(256) rl_head_bwd_kernel(const float* __restrict__ logp, long long ld_logp, const float* __restrict__ logq,
                                                           long long ld_logq, const long long* __restrict__ idx, const float* __restrict__ c,
                                                           float k, float inv_temp, int n, __nv_bfloat16* __restrict__ out, long long ld_out,
-                                                          int col0, float* __restrict__ kl, int accumulate, long long rows) {
+                                                          int col0, float* __restrict__ kl, int accumulate, long long rows, float e = 0.f,
+                                                          float* __restrict__ ent = nullptr) {
     constexpr int RPB = 256 / TPR;
     __shared__ float red[256 / 32];
     const int tr = threadIdx.x % TPR;
     const long long r = (long long)blockIdx.x * RPB + threadIdx.x / TPR;
     const bool live = r < rows;
+    float h = 0.f;
+    if (ENT) {
+        if (live) {
+            const float* lr = logp + r * ld_logp;
+            for (int j = tr; j < n; j += TPR) {
+                const float lpj = __ldg(lr + j);
+                h = fmaf(expf(lpj), lpj, h);
+            }
+            h = -h;
+        }
+        h = warp_sum(h);  // (butterfly: every lane ends with the same bits)
+        if (TPR > 32) {
+            if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = h;
+            __syncthreads();
+            h = 0.f;
+#pragma unroll
+            for (int w = 0; w < TPR / 32; ++w) h += red[w];
+            __syncthreads();  // every thread has read red before the KL sum below reuses it
+        }
+    }
     float s = 0.f;
     if (live) {
         const float* lr = logp + r * ld_logp;
@@ -61,6 +87,7 @@ __global__ void __launch_bounds__(256) rl_head_bwd_kernel(const float* __restric
                 g = fmaf(k, p - q, g);
                 s = fmaf(q, lqj - lpj, s);
             }
+            if (ENT && e != 0.f) g = fmaf(e * p, lpj + h, g);
             orow[j] = __float2bfloat16_rn(g * inv_temp);
         }
     }
@@ -74,7 +101,10 @@ __global__ void __launch_bounds__(256) rl_head_bwd_kernel(const float* __restric
     } else if ((threadIdx.x & 31) != 0) {
         return;
     }
-    if (live) kl[r] = accumulate ? kl[r] + s : s;
+    if (live) {
+        kl[r] = accumulate ? kl[r] + s : s;
+        if (ENT) ent[r] = accumulate ? ent[r] + h : h;
+    }
 }
 
 __global__ void __launch_bounds__(256) ewma_sums_kernel(const float* __restrict__ x, long long rows, double* __restrict__ sums) {
@@ -149,6 +179,27 @@ extern "C" int vpt_rl_head_bwd(const float* logp, int64_t ld_logp, const float* 
     } else {
         rl_head_bwd_kernel<256><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logp, ld_logp, logq, ld_logq, ix, c, k, inv_temp, n, o, ld_out,
                                                                                  col0, kl, accumulate, rows);
+    }
+    VPT_LAUNCH_CHECK();
+    return VPT_OK;
+}
+
+extern "C" int vpt_rl_head_bwd_ent(const float* logp, int64_t ld_logp, const float* logq, int64_t ld_logq, const int64_t* idx, const float* c,
+                                   float k, float e, float inv_temp, int32_t n, void* out, int64_t ld_out, int32_t col0, float* kl, float* ent,
+                                   int32_t accumulate, int64_t rows, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(logp && idx && c && out && kl && ent && rows > 0 && n > 0 && col0 >= 0 && ld_logp >= n && ld_out >= col0 + (int64_t)n &&
+                  (logq == nullptr || ld_logq >= n),
+              "vpt_rl_head_bwd_ent: bad arguments");
+    const long long* ix = reinterpret_cast<const long long*>(idx);
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+    if (n <= 1024) {
+        rl_head_bwd_kernel<32, true><<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(logp, ld_logp, logq, ld_logq, ix, c, k,
+                                                                                                 inv_temp, n, o, ld_out, col0, kl,
+                                                                                                 accumulate, rows, e, ent);
+    } else {
+        rl_head_bwd_kernel<256, true><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(logp, ld_logp, logq, ld_logq, ix, c, k, inv_temp, n, o,
+                                                                                       ld_out, col0, kl, accumulate, rows, e, ent);
     }
     VPT_LAUNCH_CHECK();
     return VPT_OK;

@@ -34,6 +34,7 @@ void set_error(const char* fmt, ...) {
 #include "idm_bwd.cuh"
 #include "rl_bwd.cuh"
 #include "log_softmax_bwd.cuh"
+#include "head_dist.cuh"
 #include "firstconv_bwd.cuh"
 #include "precise.cuh"
 #include "codec.cuh"

@@ -544,6 +544,8 @@ def softmax_bwd(logp, idx, scale, out, col0):
 from .ops_idm import conv3d_t5_bwd, softmax_nll_bwd_grouped  # noqa: E402,F401  (IDM backward ops, csrc/idm_bwd.cuh)
 from .ops_rl import ewma_sums, ppo_coef, rl_head_bwd, value_bwd  # noqa: E402,F401  (RL fine-tuning ops, csrc/rl_bwd.cuh)
 from .ops_autograd import log_softmax_bwd  # noqa: E402,F401  (differentiable forward, csrc/log_softmax_bwd.cuh)
+from .ops_dist import (head_entropy, head_entropy_bwd, head_kl, head_kl_bwd,  # noqa: E402,F401  (head distributions, csrc/head_dist.cuh)
+                       rl_head_bwd_ent)
 from .ops_bptt import attention_bwd_state  # noqa: E402,F401  (gradients through the KV memory, csrc/attention_bwd.cuh)
 from .ops_pixel import conv3d_t5_dimg, firstconv_dimg  # noqa: E402,F401  (image gradients, csrc/firstconv_bwd.cuh, csrc/idm_bwd.cuh)
 

@@ -5,6 +5,7 @@ hand-written sm_90a kernels of libvpt_b200.so.
     MinecraftAgentPolicy   lib/policy.py:227-339   forward / act / get_output_for_observation / get_logprob_of_action /
                                                    get_kl_of_action_dists / v / initial_state
     InverseActionPolicy    lib/policy.py:406-467   (see idm.py)
+    pi_head                lib/action_head.py:136-260  logprob / sample / entropy / kl_divergence, on the dict and on each sub-head
 
 Same constructor kwargs, same state pytree (list over layers of (state_mask bool (B,1,maxlen) | None, (K, V) fp32
 (B,maxlen,hidsize))), same `state_dict()` keys / shapes (SURVEY.md App. B), so reference weight files load with
@@ -771,12 +772,14 @@ class _PolicyBase(nn.Module):
             _set(self, "value_head.normalizer.debiasing_term", torch.tensor(0.0), requires_grad=False)
         # pi head: lib/action_head.py:263-275 -> one CategoricalActionHead per Discrete TensorType, in dict order
         self.head_specs = OrderedDict()
+        self.pi_head = _DictActionHead()
         for name, space in action_space.items():
             n = space.eltype.n
             shape = tuple(space.shape)
             cnt = 1
             for s_ in shape:
                 cnt *= s_
+            self.pi_head.add_module(name, _CategoricalActionHead(shape, n))
             w, b = _default_linear(cnt * n, h)
             _set(self, f"pi_head.{name}.linear_layer.weight", w)
             _set(self, f"pi_head.{name}.linear_layer.bias", b)
@@ -950,31 +953,155 @@ class _PolicyBase(nn.Module):
             return pd, None
         vpred, _ = self.net._linear(lat_bf16, hp["v"], 1, out_dtype=F32)
         return pd, vpred.view(B, t, 1)
-    # -- distribution helpers (lib/action_head.py:176-220, 250-260) ---------------------------------------------
+    # -- distribution helpers (lib/action_head.py:176-220, 250-260): the reference's policy calls them on its pi_head --------------
     def sample(self, pd, deterministic: bool = False):
-        """DictActionHead.sample: per head in dict order; `torch.rand_like` supplies the uniforms so the Philox stream
-        is consumed exactly like the reference's (lib/action_head.py:200)."""
-        ac = OrderedDict()
-        for name in self.head_specs:
-            lg = pd[name].contiguous()
-            u = None if deterministic else torch.rand_like(lg)
-            ac[name] = ops.gumbel_argmax(lg, u)
-        return ac
+        """`pi_head.sample`."""
+        return self.pi_head.sample(pd, deterministic)
 
     def logprob(self, ac, pd):
+        """`pi_head.logprob`."""
+        return self.pi_head.logprob(ac, pd)
+
+
+class _CategoricalActionHead(_Node):
+    """lib/action_head.py:136-220 on the kernels: the distribution methods of one categorical head, whose log-probs `pd` have the shape
+    (..., *shape, n).  Holds the head's `linear_layer` parameters (the policy's forward computes every head's logits in one GEMM, `_heads`).
+    `entropy` and `kl_divergence` are differentiable (autograd `Function`s on their backward kernels) in any input that requires grad."""
+
+    def __init__(self, shape, num_actions: int):
+        super().__init__()
+        self.num_actions = num_actions
+        self.output_shape = tuple(shape) + (num_actions,)
+
+    def _rows(self, logits):
+        """-> (the leading shape, fp32 [rows, groups*n] with unit column stride, groups)."""
+        k = len(self.output_shape)
+        if tuple(logits.shape[logits.dim() - k:]) != self.output_shape:
+            raise ValueError(f"log-probs of shape {tuple(logits.shape)} do not end in the head's {self.output_shape}")
+        groups = math.prod(self.output_shape[:-1])
+        x = logits.reshape(-1, groups * self.num_actions).to(F32)
+        return logits.shape[:logits.dim() - k], (x if x.stride(1) == 1 else x.contiguous()), groups
+
+    def logprob(self, actions, logits):
+        """log p(actions) summed over the head's sub-actions: shape (...)."""
+        lg = logits.contiguous()
+        idx = actions.to(torch.int64)
+        if lg.requires_grad and torch.is_grad_enabled():
+            lp = _GatherLogprob.apply(lg, idx)  # pd from the differentiable forward
+        else:
+            lp = ops.gather_logprob(lg, idx)
+        for _ in self.output_shape[:-1]:
+            lp = lp.sum(dim=-1)
+        return lp
+
+    def sample(self, logits, deterministic: bool = False):
+        """Gumbel-max sample (or the argmax); `torch.rand_like` supplies the uniforms so the Philox stream is consumed exactly like the
+        reference's (lib/action_head.py:200)."""
+        lg = logits.contiguous()
+        u = None if deterministic else torch.rand_like(lg)
+        return ops.gumbel_argmax(lg, u)
+
+    def entropy(self, logits):
+        """-sum exp(logits) * logits over the classes and the sub-actions: shape (...)."""
+        lead, x, groups = self._rows(logits)
+        if x.requires_grad and torch.is_grad_enabled():
+            ent = _HeadEntropy.apply(x, groups)
+        else:
+            ent = ops.head_entropy(x, groups)
+        return ent.view(lead)
+
+    def kl_divergence(self, logits_q, logits_p):
+        """KL(q || p) = sum exp(logits_q) * (logits_q - logits_p) over the classes and the sub-actions: shape (..., 1), the reference's
+        `keepdim` (lib/action_head.py:216-220)."""
+        lead, q, groups = self._rows(logits_q)
+        lead_p, p, _ = self._rows(logits_p)
+        if lead_p != lead:
+            raise ValueError(f"kl_divergence: log-probs of shapes {tuple(logits_q.shape)} and {tuple(logits_p.shape)}")
+        if (q.requires_grad or p.requires_grad) and torch.is_grad_enabled():
+            kl = _HeadKL.apply(q, p, groups)
+        else:
+            kl = ops.head_kl(q, p, groups)
+        return kl.view(*lead, 1)
+
+
+class _DictActionHead(_Node):
+    """lib/action_head.py:223-260: the policy's `pi_head`, one `_CategoricalActionHead` per action, in the action space's order.  Each
+    method takes dicts of per-head tensors and sums the heads' results (a dict of samples for `sample`)."""
+
+    def __getitem__(self, key):
+        return self._modules[key]
+
+    def __iter__(self):
+        return iter(self._modules)
+
+    def __len__(self):
+        return len(self._modules)
+
+    def keys(self):
+        return self._modules.keys()
+
+    def values(self):
+        return self._modules.values()
+
+    def items(self):
+        return self._modules.items()
+
+    @staticmethod
+    def _sum(parts):
         tot = None
-        for name, (shape, n) in self.head_specs.items():
-            lg = pd[name].contiguous()
-            idx = ac[name].to(torch.int64)
-            if lg.requires_grad and torch.is_grad_enabled():
-                lp = _GatherLogprob.apply(lg, idx)  # pd from the differentiable forward
-            else:
-                lp = ops.gather_logprob(lg, idx)
-            for _ in shape:
-                lp = lp.sum(dim=-1)
-            tot = lp if tot is None else tot + lp
+        for x in parts:
+            tot = x if tot is None else tot + x
         return tot
 
+    def logprob(self, actions, logits):
+        return self._sum(head.logprob(actions[k], logits[k]) for k, head in self.items())
+
+    def sample(self, logits, deterministic: bool = False):
+        return OrderedDict((k, head.sample(logits[k], deterministic)) for k, head in self.items())
+
+    def entropy(self, logits):
+        return self._sum(head.entropy(logits[k]) for k, head in self.items())
+
+    def kl_divergence(self, logits_q, logits_p):
+        return self._sum(head.kl_divergence(logits_q[k], logits_p[k]) for k, head in self.items())
+
+
+def _no_double_backward():
+    if torch.is_grad_enabled():
+        raise NotImplementedError("the head distribution kernels have no double backward (create_graph=True)")
+
+
+class _HeadEntropy(torch.autograd.Function):
+    """`ops.head_entropy` attached to the graph; the backward is `ops.head_entropy_bwd`."""
+
+    @staticmethod
+    def forward(ctx, lp, groups):
+        ctx.save_for_backward(lp)
+        ctx.groups = groups
+        return ops.head_entropy(lp, groups)
+
+    @staticmethod
+    def backward(ctx, g):
+        _no_double_backward()
+        (lp,) = ctx.saved_tensors
+        return ops.head_entropy_bwd(lp, g.to(F32).contiguous(), ctx.groups), None
+
+
+class _HeadKL(torch.autograd.Function):
+    """`ops.head_kl` attached to the graph; the backward (`ops.head_kl_bwd`) computes only the sides that require grad."""
+
+    @staticmethod
+    def forward(ctx, lq, lp, groups):
+        ctx.save_for_backward(lq, lp)
+        ctx.groups = groups
+        return ops.head_kl(lq, lp, groups)
+
+    @staticmethod
+    def backward(ctx, g):
+        _no_double_backward()
+        lq, lp = ctx.saved_tensors
+        dq, dp = ops.head_kl_bwd(lq, lp, g.to(F32).contiguous(), ctx.groups, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return dq, dp, None
 
 
 class _GatherLogprob(torch.autograd.Function):
@@ -1039,14 +1166,8 @@ class MinecraftAgentPolicy(_PolicyBase):
         return log_prob[:, 0]
 
     def get_kl_of_action_dists(self, pd1, pd2):
-        """lib/policy.py:281-285 / lib/action_head.py:209-220 (diagnostic, not on the hot path: torch ops)."""
-        tot = 0
-        for name, (shape, n) in self.head_specs.items():
-            kl = (torch.exp(pd1[name]) * (pd1[name] - pd2[name])).sum(-1, keepdim=True)
-            for _ in shape:
-                kl = kl.sum(dim=-2)
-            tot = tot + kl
-        return tot
+        """lib/policy.py:281-285: KL(pd1 || pd2) per frame, shape (..., 1)."""
+        return self.pi_head.kl_divergence(pd1, pd2)
 
     def get_output_for_observation(self, obs, state_in, first):
         """lib/policy.py:287-305."""

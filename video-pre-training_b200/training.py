@@ -633,14 +633,18 @@ class RLTrainer(BCTrainer):
         L_v     = mean (vpred - normalizer(returns))^2            (ScaledMSEHead.loss in training mode, lib/scaled_mse_head.py:37-43:
                                                                    the EWMA normaliser is updated with this batch first)
         L_kl    = mean KL(pi_ref || pi)                           (get_kl_of_action_dists(pd_ref, pd), lib/policy.py:281-285)
-        loss    = L_pi + vf_coef * L_v + kl_coef * L_kl
+        H       = mean H(pi)                                      (pi_head.entropy(pd), lib/action_head.py:186-194)
+        loss    = L_pi + vf_coef * L_v + kl_coef * L_kl - ent_coef * H
 
     `loss, state_out = trainer.loss_and_grad(img, first, state_in, actions, old_logprob, advantages, returns, pd_ref, vf_coef=..,
-    kl_coef=..)` accumulates d loss / d param into `.grad` (the value head included) and updates the normaliser once in place; under
-    `torch.distributed` its batch statistics are all-reduced first, so every rank holds the normaliser of the global batch.
+    kl_coef=.., ent_coef=..)` accumulates d loss / d param into `.grad` (the value head included) and updates the normaliser once in place;
+    under `torch.distributed` its batch statistics are all-reduced first, so every rank holds the normaliser of the global batch.
     `old_logprob`, `advantages` and `returns` are fp32 (B, T), `returns` in the denormalised space; `pd_ref` is what the frozen
-    reference policy's forward returns for the same frames (None only with kl_coef == 0).  `trainer.stats` holds 0-d device tensors
-    pi_loss, vf_loss, kl_ref and clipfrac of the last call.  Hand every parameter with `requires_grad` to the optimizer (the three
+    reference policy's forward returns for the same frames (None only with kl_coef == 0).  `ent_coef` (default 0) is the entropy bonus;
+    with 0 the step runs exactly as without the term.  `trainer.stats` holds 0-d device tensors pi_loss, vf_loss, kl_ref, clipfrac and
+    entropy (H) of the last call.  With ent_coef == 0 the step runs the kernels of the step without the term and does not compute the
+    entropy: `stats["entropy"]` (or `.get("entropy")`) computes it, one read of the call's log-probs, when first read; the next call frees
+    those log-probs, so read it before then (`_RLStats`).  Hand every parameter with `requires_grad` to the optimizer (the three
     normaliser tensors have none).  `recompute_frames` as in `BCTrainer`."""
 
     ewma_beta = 0.99999  # NormalizeEwma's default (lib/normalize_ewma.py:9; per_element_update=False, norm over (B, T))
@@ -655,7 +659,7 @@ class RLTrainer(BCTrainer):
         return super()._head_layers() + [self.policy.value_head.linear]
 
     def loss_and_grad(self, img, first, state_in, actions, old_logprob, advantages, returns, pd_ref=None, *, vf_coef, kl_coef, clip=0.2,
-                      upper_grads_ready=None):
+                      ent_coef=0.0, upper_grads_ready=None):
         """`upper_grads_ready` as in `BCTrainer.loss_and_grad`."""
         pol = self.policy
         B, t = img.shape[:2]
@@ -670,12 +674,14 @@ class RLTrainer(BCTrainer):
                 if pd_ref[name].dtype != F32 or pd_ref[name].numel() != N * n:
                     raise ValueError(f"RLTrainer: pd_ref[{name!r}] must be fp32 with {N} x {n} log-probs (got {tuple(pd_ref[name].shape)})")
         self._check_heads()
+        if isinstance(self.stats, _RLStats):  # the last call's unread statistics: free their log-probs before this call's forward
+            self.stats.release()
         lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, first, state_in)
-        loss, dlog = self._rl_dlog(pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N)
+        loss, dlog = self._rl_dlog(pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N, ent_coef)
         self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
         return loss, state_out
 
-    def _rl_dlog(self, pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N):
+    def _rl_dlog(self, pd, vpred, actions, old_logprob, advantages, returns, pd_ref, vf_coef, kl_coef, clip, N, ent_coef=0.0):
         pol = self.policy
         hp = pol._heads_prepared()
         dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=vpred.device)
@@ -685,10 +691,14 @@ class RLTrainer(BCTrainer):
             lp = ops.gather_logprob(pd[name].reshape(N, n), idx[name])
             logp = lp if logp is None else logp + lp
         c, pi_loss, clipped = ops.ppo_coef(logp, old_logprob.reshape(N).contiguous(), advantages.reshape(N).contiguous(), clip)
-        kl = None
+        kl = ent = None
         for name, (shape, n) in pol.head_specs.items():
             q = None if pd_ref is None else pd_ref[name].reshape(N, n)
-            kl = ops.rl_head_bwd(pd[name].reshape(N, n), idx[name], c, q, kl_coef / N, 1.0 / pol.temperature, dlog, hp["cols"][name][0], kl)
+            if ent_coef:  # the fused entropy bonus; it also gives the entropy per row
+                kl, ent = ops.rl_head_bwd_ent(pd[name].reshape(N, n), idx[name], c, q, kl_coef / N, ent_coef / N, 1.0 / pol.temperature, dlog,
+                                              hp["cols"][name][0], kl, ent)
+            else:
+                kl = ops.rl_head_bwd(pd[name].reshape(N, n), idx[name], c, q, kl_coef / N, 1.0 / pol.temperature, dlog, hp["cols"][name][0], kl)
         # value head: the normaliser sees the global batch (one 2-element all-reduce under data parallelism), then the scaled MSE
         ret = returns.reshape(N).contiguous()
         sums = ops.ewma_sums(ret)
@@ -699,9 +709,41 @@ class RLTrainer(BCTrainer):
         nz = pol.value_head.normalizer
         sq = ops.value_bwd(vpred.reshape(N), ret, sums, count, nz.running_mean, nz.running_mean_sq, nz.debiasing_term, self.ewma_beta,
                            2.0 * vf_coef / N, dlog, hp["ntot"])
-        self.stats = dict(pi_loss=pi_loss.mean(), vf_loss=sq.mean(), kl_ref=kl.mean(), clipfrac=clipped.mean())
-        loss = self.stats["pi_loss"] + vf_coef * self.stats["vf_loss"] + kl_coef * self.stats["kl_ref"]
+        stats = dict(pi_loss=pi_loss.mean(), vf_loss=sq.mean(), kl_ref=kl.mean(), clipfrac=clipped.mean())
+        loss = stats["pi_loss"] + vf_coef * stats["vf_loss"] + kl_coef * stats["kl_ref"]
+        if ent_coef:
+            stats["entropy"] = ent.mean()
+            loss = loss - ent_coef * stats["entropy"]
+            self.stats = stats
+        else:
+            self.stats = _RLStats(stats, entropy=lambda: pol.pi_head.entropy(pd).mean())
         return loss, dlog
+
+
+class _RLStats(dict):
+    """`RLTrainer.stats`: a dict of 0-d device tensors, with the statistics the step did not compute (the entropy when ent_coef == 0) made
+    on first read by their function, which holds the call's log-probs until then.  `stats[key]`, `stats.get(key)` and `key in stats` see
+    such a statistic; iteration, `len` and `items()` show it once it has been read.  The trainer's next call drops what is still unread
+    (`release`), so the held log-probs never overlap that call's own."""
+
+    def __init__(self, stats, **lazy):
+        super().__init__(stats)
+        self._lazy = lazy
+
+    def __missing__(self, key):
+        if key not in self._lazy:
+            raise KeyError(key)
+        self[key] = v = self._lazy.pop(key)()
+        return v
+
+    def __contains__(self, key):
+        return super().__contains__(key) or key in self._lazy
+
+    def get(self, key, default=None):
+        return self[key] if key in self else default
+
+    def release(self):
+        self._lazy.clear()
 
 
 class IDMTrainer(_Trainer):
