@@ -165,3 +165,29 @@ def linear(x, sd, p, relu=True):
 def plain_linear(x, sd, p, bias=True):
     """F.linear with the weight / bias `p`.weight / `p`.bias (the attention's projections and the heads: no norm, no ReLU)."""
     return F.linear(x.to(F64), sd[p + ".weight"], sd[p + ".bias"] if bias else None)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# plain-NHWC forms (the fp32-parity mode, video-pre-training_b200/precise.py: fp32 [F, H, W, C] activations, no ZP pads)
+# ---------------------------------------------------------------------------------------------------------------------
+def conv_nhwc(x, sd, p):
+    """fanin_conv on plain NHWC x: [GroupNorm(1)] -> conv3x3 -> ReLU, NHWC float64."""
+    return nhwc(O.fanin_conv(x.to(F64).permute(0, 3, 1, 2), sd, p))
+
+
+def maxpool_nhwc(x):
+    return nhwc(F.max_pool2d(x.to(F64).permute(0, 3, 1, 2), 3, 2, 1))
+
+
+def group_norm_nhwc(x, sd, p):
+    """the stack's post-pool GroupNorm(1) `p` (.weight / .bias) on plain NHWC x, float64."""
+    return nhwc(F.group_norm(x.to(F64).permute(0, 3, 1, 2), 1, sd[p + ".weight"], sd[p + ".bias"], eps=1e-5))
+
+
+def layer_norm(x, sd, p):
+    return F.layer_norm(x.to(F64), (x.shape[-1],), sd[p + ".weight"], sd[p + ".bias"], eps=1e-5)
+
+
+def dense_from_nhwc(x, Hf, Wf, C):
+    """rows of the final activation flattened H, W, C (as the fp32 mode feeds the dense layer) -> flattened C, H, W (the reference's order)."""
+    return x.reshape(x.shape[0], Hf, Wf, C).permute(0, 3, 1, 2).reshape(x.shape[0], -1)

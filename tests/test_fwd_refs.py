@@ -123,6 +123,52 @@ def test_linear_folds_match_the_unfused_layers(small):
     close("proj", run(prep.layers[0]["proj"], a, h, residual=rows), ref, LIN)
 
 
+def test_plain_nhwc_references_match_the_fp32_mode_forward():
+    """precise.forward (the fp32-parity mode) through the emulated ops at the small config, stage by stage: each plain-NHWC reference is fed
+    the forward's previous tap, so the stacks (first conv, max-pool, post-pool GroupNorm, blocks), the dense layer on rows flattened H, W, C
+    and the linear layer are each held to their float64 layer"""
+    from common import emulation
+    from video_pre_training_b200 import precise as P
+
+    pol, _, _ = make_policy(small_kwargs(), seed=4)
+    net = pol.net
+    cfg = net.cfg
+    sd = Rf.SD64({k: v.detach() for k, v in net.state_dict().items()}, "cpu")
+    B, t = 2, 3
+    H, W, _ = cfg.img_shape
+    img = torch.randint(0, 256, (B, t, H, W, 3), dtype=torch.uint8, generator=torch.Generator().manual_seed(5))
+    net.debug_taps = {}
+    try:
+        with emulation():
+            P.forward(net, img, torch.zeros(B, t, dtype=torch.bool), net.initial_state(B))
+        taps = net.debug_taps
+    finally:
+        net.debug_taps = None
+
+    def near(name, out, ref, bound=1e-4):  # measured 2.6e-5 (the hi / lo splits and fp32 sums of the emulation)
+        o, r = out.reshape(out.shape[0], -1).to(F64), ref.reshape(ref.shape[0], -1)
+        e = ((o - r).abs().amax(1) / r.pow(2).mean(1).sqrt()).max().item()
+        print(f"{name}: max |err| / rms(ref) {e:.2e} (bound {bound:.0e})")
+        assert e <= bound, (name, e)
+
+    x = img.reshape(B * t, H, W, 3)
+    for i in range(len(cfg.chans)):
+        p = f"img_process.cnn.stacks.{i}"
+        if i == 0 and not cfg.first_conv_norm:
+            pool = Rf.firstconv_pool(x, sd, p)
+        else:
+            pool = Rf.maxpool_nhwc(Rf.conv_nhwc(x, sd, p + ".firstconv"))
+        near(f"stack {i} pool", taps[p + ".pool"], pool)
+        x = Rf.group_norm_nhwc(taps[p + ".pool"], sd, p + ".n")
+        for j in range(2):
+            y = Rf.nhwc(Rf.O.cnn_basic_block(x.to(F64).permute(0, 3, 1, 2), sd, f"{p}.blocks.{j}"))
+            near(f"stack {i} block {j}", taps[f"{p}.blocks.{j}"], y)
+            x = taps[f"{p}.blocks.{j}"]
+    Hf, Wf = cfg.final_hw
+    near("dense", taps["img_process.cnn.dense"], Rf.linear(Rf.dense_from_nhwc(x.reshape(B * t, -1), Hf, Wf, cfg.chans[-1]), sd, "img_process.cnn.dense"))
+    near("linear", taps["img_process"], Rf.linear(taps["img_process.cnn.dense"], sd, "img_process.linear"))
+
+
 def test_conv3d_and_firstconv_references_match_emulation():
     g = torch.Generator().manual_seed(2)
     sd = {"c.layer.weight": torch.randn(16, 3, 5, 1, 1, generator=g), "c.layer.bias": torch.randn(16, generator=g) * 0.1,

@@ -54,10 +54,10 @@ def test_precise_kernels_match_torch():
     nat.device_check()
 
 
-def test_precise_mode_config_c1_logits_within_1e3():
-    """BASELINE configs[0]: 1x foundation model, B=1, T=1, a single 128x128 frame: log-probs within 1e-3 (relative) of the reference
-    algorithm in fp32 (oracle, bit-exact vs the live reference)."""
-    kw = vpt_b200.policy_kwargs("1x")
+def _c1_logits_within_1e3(width):
+    """BASELINE configs[0] at `width`: B=1, T=1, a single 128x128 frame: log-probs within 1e-3 (relative) of the reference algorithm in
+    fp32 (oracle, bit-exact vs the live reference)."""
+    kw = vpt_b200.policy_kwargs(width)
     for pert in (False, True):
         pol, sd, cfg = make_policy(kw, pert=pert)
         pol = pol.to(DEV).set_precision("fp32")
@@ -69,10 +69,22 @@ def test_precise_mode_config_c1_logits_within_1e3():
             (pd_o, v_o, _), st_o = O.agent_policy_forward(sd, cfg, img, first, O.initial_state(cfg, 1))
         for k in pd_o:
             e = rel_err(pd[k].cpu(), pd_o[k])
-            print(f"C1 fp32 mode (perturbed={pert}) {k}: max rel err {e:.2e}")
+            print(f"C1 fp32 mode {width} (perturbed={pert}) {k}: max rel err {e:.2e}")
             assert e < 1e-3, (k, e)
         assert (v.cpu() - v_o).abs().max() < 1e-3 * (1 + v_o.abs().max())
         assert torch.allclose(st[0][1][0].cpu(), st_o[0][1][0], rtol=1e-3, atol=1e-4)
+
+
+def test_precise_mode_config_c1_logits_within_1e3():
+    """BASELINE configs[0]: 1x foundation model, B=1, T=1, a single 128x128 frame: log-probs within 1e-3 (relative) of the reference
+    algorithm in fp32 (oracle, bit-exact vs the live reference)."""
+    _c1_logits_within_1e3("1x")
+
+
+@pytest.mark.parametrize("width", ["2x", "3x"])
+def test_precise_mode_config_c1_wider_logits_within_1e3(width):
+    """the same single-frame check at the 2x and 3x widths"""
+    _c1_logits_within_1e3(width)
 
 
 def test_precise_mode_multichunk_state_and_resets():

@@ -199,8 +199,14 @@ extern "C" int vpt_attention_f32(const float* q, const float* full_k, const floa
     const size_t smem = (size_t)(maxlen + t) * 4;  // the score row of one query
     VPT_CHECK(smem <= 200 * 1024, "vpt_attention_f32: at most %d keys per query (maxlen=%d t=%d)", 200 * 1024 / 4, maxlen, t);
     VPT_CHECK(!causal || (first && (!R || b_nd)), "vpt_attention_f32: causal attention needs `first` (and b_nd with R)");
-    static size_t attr = 0;
-    if (smem > 48 * 1024 && smem > attr) {
+    // Without the opt-in, static and dynamic shared memory together are limited to 48 KB: the kernel's own static arrays count too.
+    static size_t static_smem = 0, attr = 0;
+    if (static_smem == 0) {
+        cudaFuncAttributes fa;
+        VPT_CUDA(cudaFuncGetAttributes(&fa, attention_f32_kernel));
+        static_smem = fa.sharedSizeBytes;
+    }
+    if (static_smem + smem > 48 * 1024 && smem > attr) {
         VPT_CUDA(cudaFuncSetAttribute(attention_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr = 200 * 1024;
     }

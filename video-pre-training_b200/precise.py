@@ -76,12 +76,15 @@ class PreparedPrecise:
         self.fin = (_f(g("final_ln.weight")), _f(g("final_ln.bias")))
 
 
-def gemm3(xh, xl, W, M, N, K, *, conv=None, bias=None, relu=False, out_scale=1.0, ld=None):
-    """fp32 [M][ld >= N] = epilogue(x W^T) with x = xh + xl, W = Wh + Wl (bf16 parts): three wgmma launches (see the module docstring)."""
+def gemm3(xh, xl, W, M, N, K, *, conv=None, bias=None, relu=False, out_scale=1.0, ld=None, acc=None, out=None):
+    """fp32 [M][ld >= N] = epilogue(x W^T) with x = xh + xl, W = Wh + Wl (bf16 parts): three wgmma launches (see the module docstring).
+    acc / out: fp32 [M][ld] buffers for the running sum and the result (allocated here when not given)."""
     Wh, Wl = W
     ld = ld or N
-    acc = torch.empty((M, ld), dtype=F32, device=xh.device)
-    out = torch.empty((M, ld), dtype=F32, device=xh.device)
+    if acc is None:
+        acc = torch.empty((M, ld), dtype=F32, device=xh.device)
+    if out is None:
+        out = torch.empty((M, ld), dtype=F32, device=xh.device)
     ops.gemm(xh, Wh, acc, M, N, K, conv=conv, ld_out=ld)
     ops.gemm(xl, Wh, acc, M, N, K, conv=conv, residual=acc, ld_out=ld)        # in place: each element is read, then rewritten, by one thread
     ops.gemm(xh, Wl, out, M, N, K, conv=conv, residual=acc, S2=bias, relu=2 if relu else 0, out_scale=out_scale, ld_out=ld)
