@@ -6,7 +6,7 @@ import torch
 
 import bwd_refs as Rf
 import emu_ops as E
-from video_pre_training_b200.training import _rot
+from video_pre_training_b200.policy import _rot
 
 BF16 = torch.bfloat16
 

@@ -15,7 +15,8 @@ import vpt_b200
 from common import make_policy
 from video_pre_training_b200 import _native as nat
 from video_pre_training_b200 import ops
-from video_pre_training_b200.training import BCTrainer, _rot
+from video_pre_training_b200.policy import _rot
+from video_pre_training_b200.training import BCTrainer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"

@@ -124,6 +124,29 @@ def test_call_above_the_stored_limits_runs(emu, exact, monkeypatch):
             assert ((g_ - grads_o[n]).norm() / grads_o[n].norm()).item() < (5e-2 if cnn else 1e-3), n
 
 
+def test_call_above_the_stored_limit_launches_nothing(emu, monkeypatch):
+    """With cnn_chunk_frames at 8, a 16-frame BCTrainer or RLTrainer call on the stored tape raises before its first op: the CNN does not
+    run (and tape) chunk after chunk first."""
+    pol, _, _ = make_policy(small_kwargs())
+    monkeypatch.setattr(pol.net, "cnn_chunk_frames", 8)
+    launched = []
+    for name in dir(ops):
+        fn = getattr(ops, name)
+        if not name.startswith("_") and callable(fn) and getattr(fn, "__module__", "").startswith(("emu_", "test_", "common")):
+            monkeypatch.setattr(ops, name, lambda *a, _name=name, _fn=fn, **k: (launched.append(_name), _fn(*a, **k))[1])
+    g = torch.Generator().manual_seed(5)
+    img, first, actions = batch(g, 2, 8)
+    z = torch.zeros(2, 8)
+    with pytest.raises(NotImplementedError):
+        BCTrainer(pol).loss_and_grad(img, first, pol.initial_state(2), actions)
+    with pytest.raises(NotImplementedError):
+        RLTrainer(pol).loss_and_grad(img, first, pol.initial_state(2), actions, z, z, z, vf_coef=0.5, kl_coef=0.0)
+    assert launched == []
+    assert all(p.grad is None for p in pol.parameters())
+    BCTrainer(pol).loss_and_grad(img[:1], first[:1], pol.initial_state(1), actions_of(actions, 1))  # 8 frames: one chunk
+    assert "conv3x3_zp" in launched
+
+
 def test_bad_recompute_frames_and_the_call_limit(emu, monkeypatch):
     pol, _, _ = make_policy(small_kwargs())
     idm, _, _ = make_idm(pert=False)

@@ -287,6 +287,19 @@ def _dense_from_zp(v, cfg: NetConfig):
     return v.movedim(-1, -3).reshape(*v.shape[:-3], -1)
 
 
+def _rot(W):
+    """conv weight [Cout, Cin, 3, 3] -> dgrad weight bf16 [Cin][tap'][Cout] with tap' = 8 - tap (180-degree rotation)."""
+    return W.detach().flip(2, 3).permute(1, 2, 3, 0).reshape(W.shape[1], -1).to(BF16).contiguous()
+
+
+def _tr(W, pad_to=None):
+    """linear weight [out, in] -> dgrad weight bf16 [in][out] (optionally zero-padded along `out` to `pad_to` columns)."""
+    Wt = W.detach().t().to(BF16)
+    if pad_to is not None and pad_to != Wt.shape[1]:
+        Wt = torch.nn.functional.pad(Wt, (0, pad_to - Wt.shape[1]))
+    return Wt.contiguous()
+
+
 class _Prepared:
     """Device-side, kernel-layout copy of the parameters of one MinecraftPolicy (+ optional heads)."""
 
@@ -474,7 +487,6 @@ class MinecraftPolicy(nn.Module):
         return PreparedPrecise(self.cfg, dict(self.named_parameters()))
 
     def _build_backward(self):
-        from .training import _rot, _tr
         cfg = self.cfg
         P = dict(self.named_parameters())
         w = dict(stacks=[], layers=[])
@@ -694,8 +706,7 @@ class MinecraftPolicy(nn.Module):
         Kd = (Hf + 1) * (Wf + 1) * C2  # ZP rows flattened; the zero row / column meets zero weight columns
         xd, mr_d = self._linear(cnn_out.view(N, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
         if tape is not None:
-            if cnn_bwd and recompute is None and len(mrs) != 1:
-                raise NotImplementedError(f"training forward: at most {step} frames per call (got {N})")
+            assert not (cnn_bwd and recompute is None and len(mrs) != 1), "the stored tape holds one CNN chunk (training._Trainer.check_call)"
             tape.update(prep=prep, frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d,
                         cnn_chunks=[(f0, min(f0 + step, N)) for f0 in range(0, N, step)] if cnn_bwd else [])
         del cnn_out
@@ -888,7 +899,6 @@ class _PolicyBase(nn.Module):
         return hp
 
     def _build_heads_backward(self, layers):
-        from .training import _tr
         rows = sum(lin.weight.shape[0] for lin in layers)
         return _tr(torch.cat([lin.weight for lin in layers], 0), (rows + 7) // 8 * 8)
 

@@ -46,19 +46,7 @@ import torch.distributed as dist
 
 from . import ops
 from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy, _dense_from_zp
-
-
-def _rot(W):
-    """conv weight [Cout, Cin, 3, 3] -> dgrad weight bf16 [Cin][tap'][Cout] with tap' = 8 - tap (180-degree rotation)."""
-    return W.detach().flip(2, 3).permute(1, 2, 3, 0).reshape(W.shape[1], -1).to(BF16).contiguous()
-
-
-def _tr(W, pad_to=None):
-    """linear weight [out, in] -> dgrad weight bf16 [in][out] (optionally zero-padded along `out` to `pad_to` columns)."""
-    Wt = W.detach().t().to(BF16)
-    if pad_to is not None and pad_to != Wt.shape[1]:
-        Wt = torch.nn.functional.pad(Wt, (0, pad_to - Wt.shape[1]))
-    return Wt.contiguous()
+from .policy import _rot  # noqa: F401  (the dgrad weight layout lived here; code that imports it from this module keeps working)
 
 
 def _grad_units(net):
@@ -103,6 +91,7 @@ class _Trainer:
     # grid's y axis.  So N <= 2^31 - 128 and B <= 65535; device memory (about 1 MB per frame above the CNN at 2x width) binds first.
     max_call_frames = 2 ** 31 - 128
     max_call_batch = 65535
+    value_column = False  # whether the value head's output is one more column of the logits gradient (`_head_layers`)
 
     def __init__(self, policy, net=None, recompute_frames=None):
         """`policy` may be None with `net` given: a bare MinecraftPolicy / InverseActionNet (no heads; the differentiable forward).
@@ -122,9 +111,13 @@ class _Trainer:
         self._train, self._lowest = frozenset(), len(self._units) + 1  # the running backward's `_grad_plan` (set from its tape)
 
     def _head_layers(self):
-        """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order."""
+        """The linear layers whose outputs are the columns of the logits gradient `dlog` (and the rows of `heads_t`), in column order: the
+        action heads, then with `value_column` the value head, so that the dgrad GEMM, `wgrad` and `col_sums` of the heads give d latent,
+        dW_v and db_v as well."""
         pol = self.policy
-        return [] if pol is None else [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs]
+        if pol is None:
+            return []
+        return [getattr(pol.pi_head, name).linear_layer for name in pol.head_specs] + ([pol.value_head.linear] if self.value_column else [])
 
     def _grad_plan(self, want_dmem=None, want_dimg=False):
         """What the backward of a forward starting now does, from the parameters' `requires_grad` (and, with `state_grad`, from whether
@@ -183,12 +176,18 @@ class _Trainer:
         ops.gemm(A, Bt, out, M, N, K, residual=residual)
         return out
 
-    def _wgrad_linear(self, dz, u, weight_param=None):
-        """dW [out][in] = dz^T u (wgmma GEMM over the token dimension); accumulated into `weight_param.grad` when given."""
-        dW = ops.wgrad(dz, u)
-        if weight_param is not None:
-            self._grad(weight_param, dW)
-        return dW
+    def _split_grads(self, dz, u, parts):
+        """The weight and bias gradients of layers whose outputs are column blocks of one GEMM: dz [rows][out] is the gradient wrt that
+        output, u [rows][in] its input, and parts lists (weight, bias, r0, r1): output columns [r0, r1) are that layer's (bias None: it
+        has none).  One `wgrad` (dW = dz^T u) when a weight trains and one `col_sums` when a bias does; each parameter that trains gets
+        its rows."""
+        dW = ops.wgrad(dz, u) if any(self._trains(w) for w, _, _, _ in parts) else None
+        db = ops.col_sums(dz)[1] if any(self._trains(b) for _, b, _, _ in parts) else None
+        for w, b, r0, r1 in parts:
+            if self._trains(w):
+                self._grad(w, dW[r0:r1])
+            if self._trains(b):
+                self._grad(b, db[r0:r1])
 
     def _norm_bwd(self, du, x, mr, gamma, rows_per_group, count, g_param, b_param, grad_map=None, zp=None, add=None, relu_x=False,
                   want_dx=True):
@@ -207,63 +206,73 @@ class _Trainer:
             return None
         return ops.norm_bwd_apply(du, x, mr, gamma, ms, rows_per_group, zp=zp, add=add, relu_x=relu_x)
 
-    def _normconv_bwd(self, dz, x, mr, H, W, W_rot, names, P, add=None, relu_x=False):
-        """dz: gradient wrt the conv output (ReLU already applied), ZP [F,H+1,W+1,Cout]; x: the layer input (ZP, pre-norm).
-        Accumulates the weight / norm gradients and returns the gradient wrt x (+ add), or None when no unit below needs it."""
-        Fn, Cin, Cout = x.shape[0], x.shape[3], dz.shape[3]
-        R = Fn * (H + 1) * (W + 1)
-        gam, bet, wt = P[names + ".norm.weight"], P[names + ".norm.bias"], P[names + ".layer.weight"]
-        want_dx = self._below(names + ".")
+    def _normed_bwd(self, pfx, P, dz, x, mr, dgrad, renorm, geom, dW_map=None, shifts=(0,), gb=None, add=None, relu_x=False):
+        """Backward of the normalised layer `pfx` (z = layer(u), u = gamma * n + beta) given dz [rows][out], the gradient wrt z (ReLU
+        already applied); x [rows][in] is the layer input and mr its statistics.  The layer kind supplies what differs: dgrad() -> du
+        [rows][in], the forward kernel on the dgrad weight; renorm(gamma, beta) -> u; geom: the norm geometry (`_norm_bwd`'s
+        rows_per_group, count, zp, grad_map); dW_map: `wgrad(dz, u, shifts)` -> the weight's shape (None: it has that shape); gb: the
+        kernel-side fp32 (gamma, beta) when they are not the parameters'.  Accumulates the gradients of the parameters that train and
+        returns the gradient wrt x (+ add), [rows][in], or None when no unit below needs it."""
+        gam, bet, wt = P[pfx + ".norm.weight"], P[pfx + ".norm.bias"], P[pfx + ".layer.weight"]
+        g32, b32 = gb or (gam.detach().float().contiguous(), bet.detach().float().contiguous())
+        want_dx = self._below(pfx + ".")
         norm = want_dx or self._trains(gam) or self._trains(bet)
-        g32 = gam.detach().float().contiguous()
-        du = ops.conv3x3_zp(dz, W_rot, H, W, relu=0, want_stats=False)[0] if norm else None
+        du = dgrad() if norm else None
         if self._trains(wt):
-            u, _ = ops.affine_norm_zp(x, mr, g32, bet.detach().float().contiguous())
-            shifts = [(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)]
-            dWk = ops.wgrad(dz.view(R, Cout), u.view(R, Cin), shifts)  # [Cout][tap][Cin]
-            del u
-            self._grad(wt, dWk.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2))
+            dW = ops.wgrad(dz, renorm(g32, b32).view(x.shape), shifts)
+            self._grad(wt, dW if dW_map is None else dW_map(dW))
+            del dW
         if not norm:
             return None
-        dx = self._norm_bwd(du.view(R, Cin), x.view(R, Cin), mr, g32, (H + 1) * (W + 1), H * W * Cin, gam, bet,
-                            zp=(H, W, Cin), add=None if add is None else add.view(R, Cin), relu_x=relu_x, want_dx=want_dx)
+        return self._norm_bwd(du, x, mr, g32, g_param=gam, b_param=bet, add=add, relu_x=relu_x, want_dx=want_dx, **geom)
+
+    def _normconv_bwd(self, dz, x, mr, H, W, W_rot, pfx, P, add=None, relu_x=False):
+        """GroupNorm over each frame -> 3x3 conv (`_normed_bwd`): dz ZP [F, H+1, W+1, Cout], x ZP [F, H+1, W+1, Cin]; W_rot the
+        rotated weight (`policy._rot`).  Returns the gradient wrt x (+ add) or None."""
+        Cin, Cout = x.shape[3], dz.shape[3]
+        R = x.shape[0] * (H + 1) * (W + 1)
+        dx = self._normed_bwd(pfx, P, dz.view(R, Cout), x.view(R, Cin), mr,
+                              dgrad=lambda: ops.conv3x3_zp(dz, W_rot, H, W, relu=0, want_stats=False)[0].view(R, Cin),
+                              renorm=lambda g, b: ops.affine_norm_zp(x, mr, g, b)[0],
+                              shifts=[(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)],
+                              dW_map=lambda dW: dW.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2),  # [Cout][tap][Cin]
+                              geom=dict(rows_per_group=(H + 1) * (W + 1), count=H * W * Cin, zp=(H, W, Cin)),
+                              add=None if add is None else add.view(R, Cin), relu_x=relu_x)
         return None if dx is None else dx.view(x.shape)
 
-    def _normlinear_bwd(self, dz, x, mr, Wt, names, P, add=None, relu_x=False):
-        """[LayerNorm ->] Linear backward; dz [rows][out] is the gradient wrt the GEMM output (after ReLU masking).  Returns the gradient
-        wrt x (+ add), or None when no unit below needs it."""
-        gam, bet, wt = P[names + ".norm.weight"], P[names + ".norm.bias"], P[names + ".layer.weight"]
-        want_dx = self._below(names + ".")
-        norm = want_dx or self._trains(gam) or self._trains(bet)
-        g32, b32 = gam.detach().float().contiguous(), bet.detach().float().contiguous()
-        du = self._gemm(dz, Wt, Wt.shape[0]) if norm else None
-        if self._trains(wt):
-            u, _, _ = ops.affine_norm(x, mr, g32, b32, rows_per_group=1)
-            self._wgrad_linear(dz, u, wt)
-            del u
-        if not norm:
-            return None
-        return self._norm_bwd(du, x, mr, g32, 1, x.shape[1], gam, bet, add=add, relu_x=relu_x, want_dx=want_dx)
+    def _normlinear_bwd(self, dz, x, mr, Wt, pfx, P, add=None, relu_x=False):
+        """LayerNorm over each row -> Linear (`_normed_bwd`): dz [rows][out], x [rows][in]; Wt the transposed weight (`policy._tr`).
+        Returns the gradient wrt x (+ add) or None."""
+        return self._normed_bwd(pfx, P, dz, x, mr, dgrad=lambda: self._gemm(dz, Wt, Wt.shape[0]),
+                                renorm=lambda g, b: ops.affine_norm(x, mr, g, b, rows_per_group=1)[0],
+                                geom=dict(rows_per_group=1, count=x.shape[1]), add=add, relu_x=relu_x)
 
     # -- the step ---------------------------------------------------------------------------------------------------------
-    def check_call_frames(self, img, plan=None):
-        """With `recompute_frames`, or when the backward does not enter the CNN (`plan`, default `_grad_plan()`): the per-call limits
-        (`max_call_frames`, `max_call_batch`), checked before any work so that a call that cannot finish accumulates nothing.  (The stored
-        tape's limits are checked by the trainers and the differentiable forward.)"""
-        if self.recompute_frames is None and (plan or self._grad_plan())["cnn"]:
-            return
+    def check_call(self, img, want_dimg=False):
+        """The limits of one call, checked by every entry point before any launch so that a call that cannot finish accumulates nothing:
+        the bf16 mode; for the IDM at most `IDMTrainer.max_t` frames per sequence; with the stored tape (recompute_frames None) and a
+        backward that enters the CNN (`_grad_plan`, want_dimg: see there) at most `net.cnn_chunk_frames` (the IDM: `net.idm_chunk_frames`)
+        frames, the one CNN chunk the tape holds; otherwise `max_call_frames` frames and B <= `max_call_batch`."""
+        net = self.net
         B, t = img.shape[:2]
-        if B * t > self.max_call_frames or B > self.max_call_batch:
-            raise NotImplementedError(f"{type(self).__name__}: at most {self.max_call_frames} frames and B <= {self.max_call_batch} per call "
-                                      f"(got B = {B}, T = {t})")
+        if net.precision != "bf16":
+            raise NotImplementedError("training and the differentiable forward run in the bf16 mode only (set_precision('bf16'))")
+        if net.cfg.conv3d_out is not None and t > IDMTrainer.max_t:
+            raise NotImplementedError(f"the IDM's backward takes at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
+        if self.recompute_frames is None and self._grad_plan(want_dimg=want_dimg)["cnn"]:
+            limit = net.cnn_chunk_frames if net.cfg.conv3d_out is None else net.idm_chunk_frames
+            if B * t > limit:
+                raise NotImplementedError(f"at most {limit} frames per call with the stored CNN tape (got B*T = {B * t}); accumulate over "
+                                          "calls, pass recompute_frames (set_autograd(True, recompute_frames=...)) or freeze the CNN")
+        elif B * t > self.max_call_frames or B > self.max_call_batch:
+            raise NotImplementedError(f"at most {self.max_call_frames} frames and B <= {self.max_call_batch} per call (got B = {B}, T = {t})")
 
     def _taped_latent(self, img, first, state_in, want_dmem=None, want_dimg=False):
         """The network's inference kernels, recording what the backward needs -> (latent bf16 [N][h], latent fp32 (B,t,h), tape, state_out).
         The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`, `heads_t`), and
-        the backward's `_grad_plan` (want_dmem, want_dimg: see there)."""
+        the backward's `_grad_plan` (want_dmem, want_dimg: see there).  The caller has checked the call's limits (`check_call`)."""
         net, pol = self.net, self.policy
         tape = self._grad_plan(want_dmem, want_dimg)
-        self.check_call_frames(img, tape)
         if pol is not None:
             pol.refresh_weights()  # (a bare network: the getters rebuild eagerly on use)
         layers = self._head_layers()
@@ -302,17 +311,11 @@ class _Trainer:
         """The head weights' gradients from dlog bf16 [N][ld_logits] (one column block per `_head_layers()` entry) -> d latent bf16 [N][h],
         or None when nothing below the heads trains."""
         self._use_plan(tape)
-        layers = self._head_layers()
-        dWh = ops.wgrad(dlog, lat_bf16) if any(self._trains(lin.weight) for lin in layers) else None
-        dbh = ops.col_sums(dlog)[1] if any(self._trains(lin.bias) for lin in layers) else None
-        c0 = 0
-        for lin in layers:
-            m = lin.weight.shape[0]
-            if self._trains(lin.weight):
-                self._grad(lin.weight, dWh[c0:c0 + m])
-            if self._trains(lin.bias):
-                self._grad(lin.bias, dbh[c0:c0 + m])
-            c0 += m
+        parts, c0 = [], 0
+        for lin in self._head_layers():
+            parts.append((lin.weight, lin.bias, c0, c0 + lin.weight.shape[0]))
+            c0 += lin.weight.shape[0]
+        self._split_grads(dlog, lat_bf16, parts)
         return self._gemm(dlog, tape["heads_t"], self.net.cfg.hidsize) if self._lowest < len(self._units) else None
 
     def _backward_from_dlat(self, dlat, tape, B, t, upper_grads_ready, dstate=None, want_dmem=None):
@@ -409,27 +412,20 @@ class _Trainer:
         return dict(stacks=stacks, prep=tape["prep"], frames=frames)
 
     def _dense_bwd(self, dz, tape, wts, P):
+        """The dense layer: LayerNorm -> Linear over the CNN output's ZP rows (`_normed_bwd`), with its kernel-side gamma / beta and weight
+        columns in ZP order (`policy._dense_to_zp`); its gradients go back to the reference's order.  Returns the gradient wrt the CNN
+        output, ZP [N, Hf+1, Wf+1, C2], or None."""
         cfg = self.net.cfg
         Hf, Wf = cfg.final_hw
         C2 = cfg.chans[-1]
         N = dz.shape[0]
         Kd = (Hf + 1) * (Wf + 1) * C2
-        x = tape["cnn_out"].view(N, Kd)
-        pfx = "img_process.cnn.dense"
-        gam, bet, wt = P[pfx + ".norm.weight"], P[pfx + ".norm.bias"], P[pfx + ".layer.weight"]
-        want_dx = self._below(pfx + ".")
-        norm = want_dx or self._trains(gam) or self._trains(bet)
-        du = self._gemm(dz, wts["dense_t"], Kd) if norm else None
+        x, mr = tape["cnn_out"].view(N, Kd), tape["mr_c"]
         unperm = lambda v: _dense_from_zp(v, cfg)
-        if self._trains(wt):
-            u, _, _ = ops.affine_norm(x, tape["mr_c"], wts["dense_g"], wts["dense_b"], rows_per_group=1)
-            dWz = self._wgrad_linear(dz, u)  # [out][Kd] in ZP column order
-            del u
-            self._grad(wt, unperm(dWz))
-            del dWz
-        if not norm:
-            return None
-        dx = self._norm_bwd(du, x, tape["mr_c"], wts["dense_g"], 1, Hf * Wf * C2, gam, bet, grad_map=unperm, zp=(Hf, Wf, C2), want_dx=want_dx)
+        dx = self._normed_bwd("img_process.cnn.dense", P, dz, x, mr, dgrad=lambda: self._gemm(dz, wts["dense_t"], Kd),
+                              renorm=lambda g, b: ops.affine_norm(x, mr, g, b, rows_per_group=1)[0],
+                              geom=dict(rows_per_group=1, count=Hf * Wf * C2, zp=(Hf, Wf, C2), grad_map=unperm), dW_map=unperm,
+                              gb=(wts["dense_g"], wts["dense_b"]))
         return None if dx is None else dx.view(N, Hf + 1, Wf + 1, C2)
 
     def _block_bwd(self, l, dzo, S, first_u8, W, P, B, t, dstate=None, want_dmem=False):
@@ -447,10 +443,7 @@ class _Trainer:
         dz = dzo  # (last block: z is relu(..) (lib/policy.py:211 fused into its epilogue); the norm backward above already masked dzo)
         # mlp1: z = y + hmid W1^T + b1
         dh = self._gemm(dz, W["mlp1_t"], h * cfg.pointwise_ratio) if self._below(f"{b}.mlp1.") else None
-        if trains(P[f"{b}.mlp1.layer.weight"]):
-            self._wgrad_linear(dz, S["hmid"], P[f"{b}.mlp1.layer.weight"])
-        if trains(P[f"{b}.mlp1.layer.bias"]):
-            self._grad(P[f"{b}.mlp1.layer.bias"], ops.col_sums(dz)[1])
+        self._split_grads(dz, S["hmid"], [(P[f"{b}.mlp1.layer.weight"], P[f"{b}.mlp1.layer.bias"], 0, h)])
         if dh is None:
             return None, None
         # mlp0: hmid = relu(LN(y) W0^T)
@@ -462,10 +455,7 @@ class _Trainer:
             return None, None
         # proj: y = xhat + a Wp^T + bp
         da = self._gemm(dy, W["proj_t"], h) if self._below(f"{o}.proj_layer.") else None
-        if trains(P[f"{o}.proj_layer.weight"]):
-            self._wgrad_linear(dy, S["a"], P[f"{o}.proj_layer.weight"])
-        if trains(P[f"{o}.proj_layer.bias"]):
-            self._grad(P[f"{o}.proj_layer.bias"], ops.col_sums(dy)[1])
+        self._split_grads(dy, S["a"], [(P[f"{o}.proj_layer.weight"], P[f"{o}.proj_layer.bias"], 0, h)])
         if da is None:
             return None, None
         # attention: gradients wrt q | k | v | R side by side (one buffer = one dgrad GEMM + one wgrad GEMM for all four)
@@ -485,17 +475,12 @@ class _Trainer:
         if not self._below(f"{o}.b_nd"):
             return None, dmem
         # q | k | v | r: one dgrad GEMM and one wgrad GEMM for the four (r only where the mask has a band)
-        ws = [P[f"{o}.{c}_layer.weight"] for c in ("q", "k", "v")] + ([P[f"{o}.r_layer.weight"]] if causal else [])
-        bs = [P[f"{o}.q_layer.bias"]] + ([P[f"{o}.r_layer.bias"]] if causal else [])
         dxhat = self._gemm(dqkvr, W["qkvr_t"], h, residual=dy) if self._below(f"{o}.q_layer.") else None
-        dWc = self._wgrad_linear(dqkvr, S["xhat"]) if any(map(trains, ws)) else None
-        dbc = ops.col_sums(dqkvr)[1] if any(map(trains, bs)) else None
-        for p, r0, r1 in zip(ws, (0, h, 2 * h, 3 * h), (h, 2 * h, 3 * h, 3 * h + nr)):
-            if trains(p):
-                self._grad(p, dWc[r0:r1])
-        for p, r0, r1 in zip(bs, (0, 3 * h), (h, 3 * h + nr)):
-            if trains(p):
-                self._grad(p, dbc[r0:r1])
+        parts = [(P[f"{o}.q_layer.weight"], P[f"{o}.q_layer.bias"], 0, h), (P[f"{o}.k_layer.weight"], None, h, 2 * h),
+                 (P[f"{o}.v_layer.weight"], None, 2 * h, 3 * h)]
+        if causal:
+            parts.append((P[f"{o}.r_layer.weight"], P[f"{o}.r_layer.bias"], 3 * h, 3 * h + nr))
+        self._split_grads(dqkvr, S["xhat"], parts)
         if not causal:
             for p in (P[f"{o}.r_layer.weight"], P[f"{o}.r_layer.bias"]):
                 if trains(p):
@@ -601,6 +586,7 @@ class BCTrainer(_Trainer):
         """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` is final (the ImpalaCNN
         backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`."""
         self._check_heads()
+        self.check_call(img)
         lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
         loss, dlog = self._bc_dlog(pd, actions, img.shape[0] * img.shape[1], want_dlog=tape["lowest"] <= len(self._units))
         self._backward_from_dlog(dlog, lat_bf16, tape, img.shape[0], img.shape[1], upper_grads_ready)
@@ -648,15 +634,11 @@ class RLTrainer(BCTrainer):
     normaliser tensors have none).  `recompute_frames` as in `BCTrainer`."""
 
     ewma_beta = 0.99999  # NormalizeEwma's default (lib/normalize_ewma.py:9; per_element_update=False, norm over (B, T))
+    value_column = True   # the value head trains with the action heads
 
     def __init__(self, policy: MinecraftAgentPolicy, recompute_frames=None):
         super().__init__(policy, recompute_frames=recompute_frames)
         self.stats = None
-
-    def _head_layers(self):
-        """The value head's output is one more column of the logits gradient (after the action heads), so that the dgrad GEMM, `wgrad`
-        and `col_sums` of the heads give d latent, dW_v and db_v as well."""
-        return super()._head_layers() + [self.policy.value_head.linear]
 
     def loss_and_grad(self, img, first, state_in, actions, old_logprob, advantages, returns, pd_ref=None, *, vf_coef, kl_coef, clip=0.2,
                       ent_coef=0.0, upper_grads_ready=None):
@@ -674,6 +656,7 @@ class RLTrainer(BCTrainer):
                 if pd_ref[name].dtype != F32 or pd_ref[name].numel() != N * n:
                     raise ValueError(f"RLTrainer: pd_ref[{name!r}] must be fp32 with {N} x {n} log-probs (got {tuple(pd_ref[name].shape)})")
         self._check_heads()
+        self.check_call(img)
         if isinstance(self.stats, _RLStats):  # the last call's unread statistics: free their log-probs before this call's forward
             self.stats.release()
         lat_bf16, pd, vpred, tape, state_out = self._taped_forward(img, first, state_in)
@@ -789,17 +772,10 @@ class IDMTrainer(_Trainer):
         """`upper_grads_ready()` is called once every gradient except those of `img_process.cnn.stacks.*` and `conv3d_layer.*` is final
         (the CNN backward, most of the step's time, is still to come): the hook for `FlatAdamDP.reduce_async`.  Build the optimizer from
         `optimizer_params(policy)` so that those final gradients are one contiguous bucket slice."""
-        net = self.policy.net
         B, t = img.shape[:2]
-        N = B * t
-        # checked before the forward: nothing is accumulated into .grad by a call that cannot finish
-        if self.recompute_frames is None and N > net.idm_chunk_frames and self._grad_plan()["cnn"]:
-            raise NotImplementedError(f"IDMTrainer: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); accumulate over calls, "
-                                      "pass recompute_frames or freeze the CNN and the conv3d pre-stage")
-        if t > self.max_t:
-            raise NotImplementedError(f"IDMTrainer: at most {self.max_t} frames per sequence (got T = {t})")
+        self.check_call(img)
         lat_bf16, pd, _, tape, state_out = self._taped_forward(img, first, state_in)
-        loss, dlog = self._idm_dlog(pd, actions, N)
+        loss, dlog = self._idm_dlog(pd, actions, B * t)
         self._backward_from_dlog(dlog, lat_bf16, tape, B, t, upper_grads_ready)
         return loss, state_out
 
@@ -842,42 +818,17 @@ class _AutogradRunner(_Trainer):
         from .policy import _PolicyBase
 
         pol = module if isinstance(module, _PolicyBase) else None
+        self.value_column = pol is not None and pol.has_value_head  # vpred is an output
         super().__init__(pol, None if pol is not None else module)
         self.module = module
-
-    def _head_layers(self):
-        """The value head's output is one more column of the logits gradient, as in RLTrainer."""
-        pol = self.policy
-        if pol is None:
-            return []
-        return super()._head_layers() + ([pol.value_head.linear] if pol.has_value_head else [])
 
     def state_grad(self):
         """Whether this module's differentiable forward carries gradients through the KV memory (`set_autograd(.., state_grad=True)`;
         nothing changes for a model without memory, maxlen = 0: the IDM)."""
         return bool(getattr(self.module, "_state_grad", False)) and self.net.cfg.maxlen > 0
 
-    def check(self, img, state_in):
-        """The limits of one differentiable call, checked before any work (`img` requiring grad asks for the image gradient)."""
-        net = self.net
-        if net.precision != "bf16":
-            raise NotImplementedError("the differentiable forward runs in the bf16 mode only (set_precision('bf16'))")
-        B, t = img.shape[:2]
-        N = B * t
-        self.recompute_frames = self.module._recompute_frames  # set_autograd(.., recompute_frames=..)
-        plan = self._grad_plan(want_dimg=img.requires_grad)
-        stored = self.recompute_frames is None and plan["cnn"]  # (a frozen CNN keeps no activations)
-        if net.cfg.conv3d_out is None:
-            if stored and N > net.cnn_chunk_frames:
-                raise NotImplementedError(f"differentiable forward: at most {net.cnn_chunk_frames} frames per call (got B*T = {N}); "
-                                          "accumulate over calls or set_autograd(True, recompute_frames=...)")
-        else:
-            if stored and N > net.idm_chunk_frames:
-                raise NotImplementedError(f"differentiable forward: at most {net.idm_chunk_frames} frames per call (got B*T = {N}); "
-                                          "accumulate over calls or set_autograd(True, recompute_frames=...)")
-            if t > IDMTrainer.max_t:
-                raise NotImplementedError(f"differentiable forward: at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
-        self.check_call_frames(img, plan)
+    def check_state_in(self, state_in):
+        """Without `state_grad`, a state_in that requires grad is refused: no gradient flows through the KV memory across calls."""
         if self.state_grad():
             return
         for _, (k, v) in state_in:
@@ -892,7 +843,9 @@ class _AutogradRunner(_Trainer):
         fp32 copy, `policy.frames_f32`, so that autograd casts the gradient back to the leaf's dtype) whose gradient the backward returns."""
         from .policy import frames_f32
 
-        self.check(img, state_in)
+        self.recompute_frames = self.module._recompute_frames  # set_autograd(.., recompute_frames=..)
+        self.check_call(img, want_dimg=img.requires_grad)
+        self.check_state_in(state_in)
         params = [p for p in self.module.parameters()]
         sg = self.state_grad()
         kv = [x for _, (k, v) in state_in for x in (k, v)] if sg else []
@@ -941,16 +894,12 @@ class _AutogradRunner(_Trainer):
         self._sink = sink
         h = self.net.cfg.hidsize
         try:
-            if self.policy is None:
-                if grads[0] is None:  # only the state_out feeds the loss
-                    dlat = torch.zeros((N, h), dtype=BF16, device=tape["lat"].device)
-                else:
-                    dlat = grads[0].reshape(N, -1).to(BF16).contiguous()
-                return sink, self._backward_from_dlat(dlat, tape, B, t, None, dstate, want_dmem)
-            pol = self.policy
             if all(g is None for g in grads):  # only the state_out feeds the loss: no head gradient, a zero d latent
                 return sink, self._backward_from_dlat(torch.zeros((N, h), dtype=BF16, device=tape["lat"].device), tape, B, t, None, dstate,
                                                       want_dmem)
+            if self.policy is None:
+                return sink, self._backward_from_dlat(grads[0].reshape(N, -1).to(BF16).contiguous(), tape, B, t, None, dstate, want_dmem)
+            pol = self.policy
             hp = pol._heads_prepared()
             dlog = torch.zeros((N, self.ld_logits), dtype=BF16, device=tape["lat"].device)
             unused = []
