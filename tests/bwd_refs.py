@@ -19,39 +19,59 @@ NBASIS = 10
 # ---------------------------------------------------------------------------------------------------------------------
 # shapes
 # ---------------------------------------------------------------------------------------------------------------------
-def backward_shapes(width, B=16, T=128):
-    """The call shapes the BC backward (training.py) reaches for `policy_kwargs(width)` at B x T frames / tokens."""
-    cfg = NetConfig(**vpt_b200.policy_kwargs(width))
+def backward_shapes(width, B=None, T=128):
+    """The call shapes the backward (training.py) reaches for the released model `width`: `policy_kwargs(width)` (1x / 2x / 3x, the BC
+    and RL steps, B = 16) or `idm_net_kwargs()` ("idm", B = 4: the 512 frames of `idm_chunk_frames`), at B x T frames / tokens.
+
+    head_cols lists (name, first column, columns) of the logits gradient, head_groups (name, first column, classes, sub-actions) (the
+    IDM's factored heads: 20 x 2 and 2 x 11).  dgrads lists the input-gradient GEMMs `_gemm` runs, (name, M, N, K, residual):
+    out [M][N] = dz [M][K] @ W_t[N][K]^T; "heads_value" is the RL step's heads GEMM with the value head's column."""
+    idm = width == "idm"
+    cfg = NetConfig(**(vpt_b200.idm_net_kwargs() if idm else vpt_b200.policy_kwargs(width)))
+    B = B or (4 if idm else 16)
     H0, W0, _ = cfg.img_shape
     c = cfg.chans
     h, heads = cfg.hidsize, cfg.heads
+    causal = cfg.mask_style == "clipped_causal"
     Hf, Wf = cfg.final_hw
     kd = (Hf + 1) * (Wf + 1) * c[-1]                 # dense input row in ZP (h, w, c) order
-    kcat = (3 * h + NBASIS * heads + 7) // 8 * 8      # q | k | v | R gradient buffer (training.py)
-    heads_n = [(name, sp.eltype.n) for name, sp in vpt_b200.minecraft_action_space().items()]
-    cols, c0 = [], 0
-    for name, n in heads_n:
-        cols.append((name, c0, n))
-        c0 += n
+    kcat = (3 * h + NBASIS * heads + 7) // 8 * 8 if causal else 3 * h  # q | k | v [| R] gradient buffer (training.py)
+    space = vpt_b200.idm_action_space() if idm else vpt_b200.minecraft_action_space()
+    cols, groups, c0 = [], [], 0
+    for name, sp in space.items():
+        n, cnt = sp.eltype.n, 1
+        for d in sp.shape:
+            cnt *= d
+        cols.append((name, c0, n * cnt))
+        groups.append((name, c0, n, cnt))
+        c0 += n * cnt
     ld_logits = (c0 + 7) // 8 * 8
-    # 3x3 convs of the CNN backward, (H, W, Cin, Cout) at their frame size: stack i > 0 opens with a conv at the previous size
+    # 3x3 convs of the CNN backward, (H, W, Cin, Cout) at their frame size: stack i > 0 (and the IDM's stack 0) opens with a normalised
+    # conv at the stack's input size, followed by the max-pool
     convs, norms, pools = [], [], []
-    Hs, Ws = H0 // 2, W0 // 2
+    Hs, Ws, cin = H0, W0, cfg.conv3d_out
     for i, C in enumerate(c):
-        if i > 0:
-            convs.append((Hs, Ws, c[i - 1], C))
+        if i > 0 or cfg.first_conv_norm:
+            convs.append((Hs, Ws, cin, C))
+            if i == 0:
+                norms.append((Hs, Ws, cin))              # the GroupNorm(1) of the conv3d output
             pools.append((Hs, Ws, C))                    # max-pool backward input (pre-pool size)
-            Hs, Ws = Hs // 2, Ws // 2
+        Hs, Ws, cin = Hs // 2, Ws // 2, C
         convs.append((Hs, Ws, C, C))
         norms.append((Hs, Ws, C))                        # GroupNorm(1) ZP frames of this stack
     assert (Hs, Ws) == (Hf, Wf)
     uniq = lambda v: list(dict.fromkeys(v))
+    N, f = B * T, h * cfg.pointwise_ratio
+    dgrads = [("heads", N, h, ld_logits, False)]
+    if not idm:
+        dgrads += [("heads_value", N, h, (c0 + 1 + 7) // 8 * 8, False), ("lastlayer", N, h, h, False)]
+    dgrads += [("mlp1", N, f, h, False), ("mlp0", N, h, f, False), ("proj", N, h, h, False), ("qkvr", N, h, kcat, True),
+               ("linear", N, cfg.cnn_outsize, h, False), ("dense", N, kd, cfg.cnn_outsize, False)]
     return dict(
-        cfg=cfg, B=B, T=T, N=B * T, h=h, heads=heads, maxlen=cfg.maxlen, kcat=kcat, ld_logits=ld_logits, head_cols=cols,
-        convs=uniq(convs), gn=uniq(norms), pools=uniq(pools), firstconv=(H0, W0, c[0]),
-        ln=uniq([h, cfg.cnn_outsize]), dense=(Hf, Wf, c[-1], kd),
-        linears=uniq([(ld_logits, h), (kcat, h), (h, h * cfg.pointwise_ratio), (h * cfg.pointwise_ratio, h), (h, h),
-                      (h, cfg.cnn_outsize), (cfg.cnn_outsize, kd)]),
+        cfg=cfg, B=B, T=T, N=N, h=h, heads=heads, maxlen=cfg.maxlen, causal=causal, kcat=kcat, ld_logits=ld_logits, head_cols=cols,
+        head_groups=groups, convs=uniq(convs), gn=uniq(norms), pools=uniq(pools), firstconv=None if cfg.first_conv_norm else (H0, W0, c[0]),
+        ln=uniq([h, cfg.cnn_outsize]), dense=(Hf, Wf, c[-1], kd), dgrads=dgrads,
+        linears=uniq([(ld_logits, h), (kcat, h), (h, f), (f, h), (h, h), (h, cfg.cnn_outsize), (cfg.cnn_outsize, kd)]),
     )
 
 
@@ -88,6 +108,17 @@ def conv_wgrad(dz, u):
     return perm(g), perm(s)
 
 
+def conv_wgrad_taps(dz, u):
+    """conv_wgrad as nine float64 GEMMs over the zero-padded interiors (dW[:, tap] = dz^T u shifted by the tap), for frame counts where
+    a float64 convolution is slow; [Cout][tap][Cin] and the same over |dz|, |u|."""
+    H, W = dz.shape[1] - 1, dz.shape[2] - 1
+    Cout, Cin = dz.shape[3], u.shape[3]
+    g = dz[:, :H, :W].to(F64).reshape(-1, Cout)
+    up = F.pad(u[:, :H, :W].to(F64), (0, 0, 1, 1, 1, 1))
+    taps = [up[:, ky:ky + H, kx:kx + W].reshape(-1, Cin) for ky in range(3) for kx in range(3)]
+    return torch.cat([g.T @ x for x in taps], 1), torch.cat([g.abs().T @ x.abs() for x in taps], 1)
+
+
 def linear_wgrad(a, b):
     """a^T b over the rows, and |a|^T |b|."""
     a, b = a.to(F64), b.to(F64)
@@ -111,10 +142,20 @@ def _real(v, rows_per_group, zp):
     return v.reshape(G, H + 1, W + 1, Cc)[:, :H, :W].reshape(G, -1)
 
 
-def norm_bwd(du, x, gamma, rows_per_group, zp=None):
+def norm_bwd(du, x, gamma, rows_per_group, zp=None, add=None, relu_x=False):
     """Autograd of GroupNorm(1) over a ZP frame (rows_per_group > 1) or LayerNorm over a row (rows_per_group == 1; with zp the row
-    is a ZP image whose pads are not part of the norm) in float64.  gamma: fp32 [C].
+    is a ZP image whose pads are not part of the norm) in float64.  gamma: fp32 [C].  add: a gradient that reaches x by another path
+    (a residual), added to dx; relu_x: x is the output of a ReLU, whose backward then zeroes the total where x == 0.
     Returns dict(dx [rows][C] (zero at pads), dgamma [C], dbeta [C], ms [G][2] = (mean gamma*du, mean gamma*du*n))."""
+    r = _norm_bwd(du, x, gamma, rows_per_group, zp)
+    if add is not None:
+        r["dx"] = r["dx"] + add.to(F64).reshape(r["dx"].shape)
+    if relu_x:
+        r["dx"] = torch.where(x.reshape(r["dx"].shape) != 0, r["dx"], torch.zeros((), dtype=F64, device=x.device))
+    return r
+
+
+def _norm_bwd(du, x, gamma, rows_per_group, zp):
     rows, C = x.shape
     G = rows // rows_per_group
     dev = x.device
@@ -202,3 +243,41 @@ def softmax_bwd(logp, idx, scale):
     g = torch.exp(logp.to(F64))
     g[torch.arange(g.shape[0], device=g.device), idx.long()] -= 1.0
     return g * scale
+
+
+def full_attention_bwd(q, k, v, dO, B, t, heads):
+    """Autograd of the IDM's unmasked attention softmax(q k^T / D) v per head (D = 128, every key of the sequence) in float64.
+    q, dO [B*t][h], k, v [B, t, h] -> (dq, dk, dv) [B*t][h]."""
+    h = q.shape[-1]
+    D = h // heads
+    split = lambda x: x.to(F64).reshape(B, t, heads, D).permute(0, 2, 1, 3)
+    qq, kk, vv = (split(x).clone().requires_grad_(True) for x in (q, k, v))
+    o = torch.softmax(qq @ kk.transpose(-1, -2) / D, -1) @ vv
+    grads = torch.autograd.grad(o, (qq, kk, vv), split(dO))
+    return [g.permute(0, 2, 1, 3).reshape(B * t, h) for g in grads]
+
+
+def conv3d_t5_wgrad(img, dy, C, chunk=16):
+    """Weight / bias gradient of the IDM's conv3d pre-stage (kernel (5, 1, 1), zero padding of 2 frames at both ends of each sequence)
+    in float64, on the device of the inputs, `chunk` frames of dy at a time.  img u8 or fp32 [B, T, H, W, 3] on the uint8 scale, dy ZP
+    [B*T, H+1, W+1, C] (the gradient wrt the conv3d output; its pad row / column is not part of the conv).  Returns (dW [C][15] in
+    (dt, c) order, db [C], and the same sums over |dy|, |img|) -- dW with respect to weights that multiply the uint8-scale values."""
+    B, T, H, W, _ = img.shape
+    dev = dy.device
+    dW, sW = torch.zeros(C, 5, 3, dtype=F64, device=dev), torch.zeros(C, 5, 3, dtype=F64, device=dev)
+    db, sb = torch.zeros(C, dtype=F64, device=dev), torch.zeros(C, dtype=F64, device=dev)
+    for b in range(B):
+        for t0 in range(0, T, chunk):
+            t1 = min(T, t0 + chunk)
+            g = dy[b * T + t0:b * T + t1, :H, :W].to(F64).reshape(t1 - t0, H * W, C)
+            db += g.sum((0, 1))
+            sb += g.abs().sum((0, 1))
+            for dt in range(5):  # output frame t reads input frame t + dt - 2
+                lo, hi = max(t0, 2 - dt), min(t1, T + 2 - dt)
+                if lo >= hi:
+                    continue
+                x = img[b, lo + dt - 2:hi + dt - 2].to(F64).reshape(hi - lo, H * W, 3)
+                gg = g[lo - t0:hi - t0]
+                dW[:, dt] += torch.einsum("fpo,fpc->oc", gg, x)
+                sW[:, dt] += torch.einsum("fpo,fpc->oc", gg.abs(), x.abs())
+    return dW.reshape(C, 15), db, sW.reshape(C, 15), sb

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 import bwd_refs as Rf
+import emu_idm_ops
 import emu_ops as E
 from video_pre_training_b200.policy import _rot
 
@@ -28,6 +29,18 @@ def test_shape_table_follows_the_model():
     assert s["head_cols"] == [("camera", 0, 121), ("buttons", 121, 8641)]
     assert s["firstconv"] == (128, 128, 192) and (s["h"], s["heads"]) == (3072, 24)
     assert Rf.backward_shapes("1x")["convs"][0] == (64, 64, 64, 64)
+    assert [d[0] for d in s["dgrads"]] == ["heads", "heads_value", "lastlayer", "mlp1", "mlp0", "proj", "qkvr", "linear", "dense"]
+    assert ("qkvr", 2048, 3072, 9456, True) in s["dgrads"] and ("dense", 2048, 17 * 17 * 384, 256, False) in s["dgrads"]
+
+
+def test_idm_shape_table_follows_the_model():
+    s = Rf.backward_shapes("idm")
+    assert (s["N"], s["h"], s["heads"], s["kcat"], s["ld_logits"], s["causal"]) == (512, 4096, 32, 3 * 4096, 64, False)
+    assert s["convs"][0] == (128, 128, 128, 256) and s["gn"][0] == (128, 128, 128) and s["pools"][0] == (128, 128, 256)
+    assert s["firstconv"] is None and s["dense"] == (16, 16, 512, 147968)
+    assert s["head_groups"] == [("buttons", 0, 2, 20), ("camera", 40, 11, 2)]
+    assert [d[0] for d in s["dgrads"]] == ["heads", "mlp1", "mlp0", "proj", "qkvr", "linear", "dense"]  # no lastlayer, no value column
+    assert ("heads", 512, 4096, 64, False) in s["dgrads"] and ("dense", 512, 147968, 256, False) in s["dgrads"]
 
 
 def test_conv_references_match_emulation():
@@ -45,6 +58,8 @@ def test_conv_references_match_emulation():
     shifts = [(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)]
     emu = E.wgrad(dz.reshape(R, Cout), u.reshape(R, Cin), shifts)          # the ZP shift identity
     assert ((emu.double() - ref).abs() <= 1e-6 * scale).all()
+    taps, tscale = Rf.conv_wgrad_taps(dz, u)
+    assert ((taps - ref).abs() <= 1e-12 * scale).all() and ((tscale - scale).abs() <= 1e-12 * scale).all()
 
 
 def test_linear_wgrad_reference_matches_emulation():
@@ -75,6 +90,43 @@ def test_norm_reference_matches_emulation(rpg, C, zp):
     assert rel(cs[0], ref["dgamma"]) < 1e-5 and rel(cs[1], ref["dbeta"]) < 1e-6
     dx = E.norm_bwd_apply(du, x, mr, gamma, ref["ms"].float(), rpg, zp=zp)
     assert ((dx.double() - ref["dx"]).abs() <= 2 ** -8 * ref["dx"].abs() + 1e-5 * ref["dx"].abs().max()).all()
+
+
+@pytest.mark.parametrize("rpg,C,zp", [(8 * 7, 16, (7, 6, 16)), (1, 64, None)])
+def test_norm_reference_with_relu_x_and_add_matches_emulation(rpg, C, zp):
+    """dx + add, zeroed where the ReLU output x is 0 (the apply pass of a norm whose input is a ReLU output and a residual)"""
+    g = torch.Generator().manual_seed(6)
+    G = 3
+    if zp is None:
+        x = (torch.randn(G, C, generator=g) * 0.7 + 0.3).relu().to(BF16)
+        du, add = torch.randn(G, C, generator=g).to(BF16), torch.randn(G, C, generator=g).to(BF16)
+    else:
+        H, W, Cc = zp
+        x = zp_rand(g, G, H, W, Cc, relu=True).reshape(G * rpg, C)
+        du, add = zp_rand(g, G, H, W, Cc).reshape(G * rpg, C), zp_rand(g, G, H, W, Cc).reshape(G * rpg, C)
+    assert (x == 0).float().mean() > 0.2
+    gamma = torch.randn(C, generator=g) * 0.3 + 1
+    mr = Rf.norm_stats(x, rpg, zp)
+    ref = Rf.norm_bwd(du, x, gamma, rpg, zp, add=add, relu_x=True)
+    plain = Rf.norm_bwd(du, x, gamma, rpg, zp)
+    assert torch.equal(ref["dx"], torch.where(x != 0, plain["dx"] + add.double(), torch.zeros((), dtype=torch.float64)))
+    dx = E.norm_bwd_apply(du, x, mr, gamma, ref["ms"].float(), rpg, zp=zp, add=add, relu_x=True)
+    assert ((dx.double() - ref["dx"]).abs() <= 2 ** -8 * ref["dx"].abs() + 1e-5 * ref["dx"].abs().max()).all()
+
+
+@pytest.mark.parametrize("f32", [False, True])
+def test_chunked_conv3d_reference_matches_emulation(f32):
+    """the frame-chunked float64 conv3d weight gradient against autograd of the whole conv3d: chunks of 3 frames over sequences of 7
+    cross the 2-frame time padding at both ends"""
+    g = torch.Generator().manual_seed(7)
+    B, T, H, W, C = 2, 7, 5, 4, 16
+    img = torch.rand(B, T, H, W, 3, generator=g) * 300 - 20 if f32 else torch.randint(0, 256, (B, T, H, W, 3), dtype=torch.uint8, generator=g)
+    dy = E.to_zp(torch.randn(B * T, H, W, C, generator=g).to(BF16))
+    ref_w, ref_b = emu_idm_ops.conv3d_t5_bwd(img, dy, C)
+    dy[:, -1], dy[:, :, -1] = 3.0, -2.0  # the pad row / column is not part of the conv
+    dW, db, sW, sb = Rf.conv3d_t5_wgrad(img, dy, C, chunk=3)
+    assert rel(dW, ref_w) < 1e-6 and rel(db, ref_b) < 1e-6
+    assert (sW >= dW.abs()).all() and (sb >= db.abs()).all()
 
 
 def test_maxpool_and_firstconv_references_match_emulation():

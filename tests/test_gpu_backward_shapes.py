@@ -1,6 +1,6 @@
-"""Backward kernels of the BC step at the shapes a training step reaches (B x T = 2048 frames / tokens, widths 1x / 2x / 3x), against
-the float64 references of tests/bwd_refs.py, plus: every write stays inside its declared buffer, every reduction is bit-reproducible,
-and the whole 3x-width step matches forced autograd.
+"""Backward kernels of the training steps at the shapes they reach (B x T = 2048 frames / tokens at the widths 1x / 2x / 3x, 512 for the
+4x IDM), against the float64 references of tests/bwd_refs.py, plus: every write stays inside its declared buffer, every reduction is
+bit-reproducible, and the whole 3x-width step matches forced autograd.
 
 The conv side runs F = 16..128 frames instead of 2048: F is the smallest count whose launch plan (wgrad K splits, norm slabs) equals
 the production one, read back from the library's own workspace queries.  Each check prints its measured error beside its bound."""
@@ -22,7 +22,8 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 WIDTHS = ["1x", "2x", "3x"]
-SHAPES = {w: Rf.backward_shapes(w) for w in WIDTHS}
+MODELS = WIDTHS + ["idm"]  # the IDM where a test body takes its shapes unchanged
+SHAPES = {w: Rf.backward_shapes(w) for w in MODELS}
 ROWS = SHAPES["3x"]["N"]  # tokens of a training step (B = 16, T = 128)
 
 # Bounds: each is at most 4x the worst value measured on an H100 80GB HBM3 (SXM) at a 400 W power limit, given beside it.
@@ -31,8 +32,12 @@ ROWS = SHAPES["3x"]["N"]  # tokens of a training step (B = 16, T = 128)
 WG_ELEM_ROW, WG_L2_ROW = 1.5e-9, 4e-9
 BF_FLOOR_CONV = 8e-6            # dgrad conv: |err| <= 2^-8 |ref| + floor * (max |ref| of the pixel); measured 2.1e-6
 BF_FLOOR_NORM = 1.2e-9          # norm dx; measured 2.9e-10
+# norm dx + add with relu_x: where dx and add nearly cancel the fp32 error of dx shows above 2^-8 |ref|; measured 3.6e-8 (H100 80GB HBM3,
+# 700 W)
+BF_FLOOR_NORM_ADD = 1.4e-7
 BF_FLOOR_ATTN = 6e-7            # dq / dk / dv / dR; measured 1.6e-7
 BF_FLOOR_SOFTMAX = 0.0          # measured < 0: every element within 2^-8 |ref|
+BF_FLOOR_GROUPED = 2.3e-7       # the IDM's grouped heads: exp(logp) - 1 near p = 1 cancels; measured 5.7e-8 (H100 80GB HBM3, 700 W)
 NORM_ELEM, NORM_L2 = 3e-7, 6e-7  # ms, dgamma, dbeta: |err| / (sum of the absolute terms), rel-L2; measured 7.6e-8, 1.4e-7
 FC_L2 = 4e-7                    # first conv dW / db rel-L2; measured 9.5e-8
 DBND_L2 = 1.1e-6                # attention d b_nd rel-L2; measured 2.7e-7
@@ -94,9 +99,9 @@ def conv_shifts(W):
     return [(ky - 1) * (W + 1) + (kx - 1) for ky in range(3) for kx in range(3)]
 
 
-def frames_for_plan(plan, per_frame, lo=16, hi=128):
-    """smallest frame count in [lo, hi] (steps of 8) whose launch plan equals the one at ROWS frames"""
-    want = plan(ROWS * per_frame)
+def frames_for_plan(plan, per_frame, lo=16, hi=128, rows=ROWS):
+    """smallest frame count in [lo, hi] (steps of 8) whose launch plan equals the one at `rows` frames"""
+    want = plan(rows * per_frame)
     for Fn in range(lo, hi + 1, 8):
         if plan(Fn * per_frame) == want:
             return Fn, want
@@ -106,11 +111,11 @@ def frames_for_plan(plan, per_frame, lo=16, hi=128):
 # ---------------------------------------------------------------------------------------------------------------------
 # weight gradients and dgrad convolutions
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("width", WIDTHS)
+@pytest.mark.parametrize("width", MODELS)
 def test_conv_wgrad_and_dgrad_at_production_plans(width):
     for i, (H, W, Cin, Cout) in enumerate(SHAPES[width]["convs"]):
         P = (H + 1) * (W + 1)
-        Fn, splits = frames_for_plan(lambda R: wgrad_splits(Cout, Cin, 9, R), P)
+        Fn, splits = frames_for_plan(lambda R: wgrad_splits(Cout, Cin, 9, R), P, rows=SHAPES[width]["N"])
         if Cout <= 128:  # one (M, N) tile: the production plan splits K over > 16 CTAs (30 on 132 SMs)
             assert splits > 16, (H, W, Cin, Cout, splits)
         g = gen(10 + i)
@@ -139,14 +144,15 @@ def test_wgrad_at_the_split_cap_with_a_ragged_last_split():
     nat.device_check()
 
 
-@pytest.mark.parametrize("width", WIDTHS)
+@pytest.mark.parametrize("width", MODELS)
 def test_linear_wgrad_at_production_shapes(width):
+    rows = SHAPES[width]["N"]
     for i, (M, N) in enumerate(SHAPES[width]["linears"]):
         g = gen(30 + i)
-        a, b = randn((ROWS, M), g).to(BF16), randn((ROWS, N), g).to(BF16)
+        a, b = randn((rows, M), g).to(BF16), randn((rows, N), g).to(BF16)
         ref, scale = Rf.linear_wgrad(a, b)
-        check_sum(f"{width} wgrad linear {M}x{N} splits={wgrad_splits(M, N, 1, ROWS)}", ops.wgrad(a, b), ref, scale,
-                  *wgrad_bounds(M, N, 1, ROWS))
+        check_sum(f"{width} wgrad linear {M}x{N} rows={rows} splits={wgrad_splits(M, N, 1, rows)}", ops.wgrad(a, b), ref, scale,
+                  *wgrad_bounds(M, N, 1, rows))
         del ref, scale
     nat.device_check()
 
@@ -154,19 +160,24 @@ def test_linear_wgrad_at_production_shapes(width):
 # ---------------------------------------------------------------------------------------------------------------------
 # GroupNorm / LayerNorm backward
 # ---------------------------------------------------------------------------------------------------------------------
-def _norm_case(name, G, rpg, C, zpg, seed):
+def _norm_case(name, G, rpg, C, zpg, seed, fused=False):
+    """fused: x is a ReLU output (about a third zeros) and the apply pass also takes `add` and `relu_x`, as for a norm whose input feeds a
+    residual too (add) or comes out of a ReLU (relu_x)"""
     g = gen(seed)
+    act = (lambda v: v.relu()) if fused else (lambda v: v)
     if zpg is not None:
         H, W, Cc = zpg
-        x = zp(randn((G, H, W, Cc), g, 0.7, 0.3)).reshape(G * rpg, C)
+        x = zp(act(randn((G, H, W, Cc), g, 0.7, 0.3))).reshape(G * rpg, C)
         du = zp(randn((G, H, W, Cc), g)).reshape(G * rpg, C)
+        add = zp(randn((G, H, W, Cc), g)).reshape(G * rpg, C) if fused else None
         count = H * W * Cc
     else:
-        x, du = randn((G, C), g, 0.7, 0.3).to(BF16), randn((G, C), g).to(BF16)
+        x, du = act(randn((G, C), g, 0.7, 0.3)).to(BF16), randn((G, C), g).to(BF16)
+        add = randn((G, C), g).to(BF16) if fused else None
         count = C
     gamma = randn((C,), g, 0.3, 1.0)
     mr = Rf.norm_stats(x, rpg, zpg)
-    ref = Rf.norm_bwd(du, x, gamma, rpg, zpg)
+    ref = Rf.norm_bwd(du, x, gamma, rpg, zpg, add=add, relu_x=fused)
     if rpg > 1:
         cs, ms = ops.norm_sums(du, x, mr, gamma, rpg, count)
     else:
@@ -178,8 +189,11 @@ def _norm_case(name, G, rpg, C, zpg, seed):
     check_sum(f"{name} ms", ms, ref["ms"], ms_scale, NORM_ELEM, NORM_L2)
     check_sum(f"{name} dgamma", cs[0], ref["dgamma"], (du.to(F64).abs() * n.abs()).sum(0), NORM_ELEM, NORM_L2)
     check_sum(f"{name} dbeta", cs[1], ref["dbeta"], du.to(F64).abs().sum(0), NORM_ELEM, NORM_L2)
-    dx = ops.norm_bwd_apply(du, x, mr, gamma, ref["ms"].float(), rpg, zp=zpg)
-    check_bf16(f"{name} dx", dx, ref["dx"], BF_FLOOR_NORM)
+    dx = ops.norm_bwd_apply(du, x, mr, gamma, ref["ms"].float(), rpg, zp=zpg, add=add, relu_x=fused)
+    if fused:
+        name = f"{name} (add, relu_x)"
+        assert (dx[x == 0] == 0).all(), f"{name}: non-zero dx where the ReLU output is 0"
+    check_bf16(f"{name} dx", dx, ref["dx"], BF_FLOOR_NORM_ADD if fused else BF_FLOOR_NORM)
     if zpg is not None:
         H, W, Cc = zpg
         d4 = dx.reshape(-1, H + 1, W + 1, Cc) if rpg > 1 else dx.reshape(G, H + 1, W + 1, Cc)
@@ -192,21 +206,26 @@ def norm_spg(rows, C, rpg):
     return lib().vpt_norm_sums_workspace(rows, C, rpg) // (G * (2 * C + 2 * ((C // 8 + 31) // 32)))
 
 
-@pytest.mark.parametrize("width", WIDTHS)
+@pytest.mark.parametrize("width", MODELS)
 def test_norm_backward_at_production_shapes(width):
     s = SHAPES[width]
+    N = s["N"]
     for i, (H, W, C) in enumerate(s["gn"]):  # ZP frames, many slabs per frame
         _norm_case(f"{width} GroupNorm {H}x{W}x{C} F=24", 24, (H + 1) * (W + 1), C, (H, W, C), 40 + i)
+    H, W, C = s["gn"][0]  # the largest frame, with the residual and the ReLU backward in the apply pass
+    _norm_case(f"{width} GroupNorm {H}x{W}x{C} F=24", 24, (H + 1) * (W + 1), C, (H, W, C), 49, fused=True)
     H, W, C = s["gn"][-1]  # the smallest frame at the production plan of whole-frame slabs
     rpg = (H + 1) * (W + 1)
-    want = norm_spg(ROWS * rpg, C, rpg)
-    G = next(G for G in range(64, ROWS + 1, 64) if norm_spg(G * rpg, C, rpg) == want)
+    want = norm_spg(N * rpg, C, rpg)
+    G = next(G for G in range(64, N + 1, 64) if norm_spg(G * rpg, C, rpg) == want)
     _norm_case(f"{width} GroupNorm {H}x{W}x{C} F={G} slabs/frame={want}", G, rpg, C, (H, W, C), 45)
+    _norm_case(f"{width} GroupNorm {H}x{W}x{C} F={G} slabs/frame={want}", G, rpg, C, (H, W, C), 46, fused=True)
     for i, C in enumerate(s["ln"]):  # LayerNorm rows
-        _norm_case(f"{width} LayerNorm {C}", ROWS, 1, C, None, 50 + i)
+        _norm_case(f"{width} LayerNorm {C}", N, 1, C, None, 50 + i)
+        _norm_case(f"{width} LayerNorm {C}", N, 1, C, None, 60 + i, fused=True)
     Hf, Wf, C2, kd = s["dense"]  # the dense layer's ZP input row: rows reproducing the production column-sum plan
-    want = lib().vpt_col_sums_parts(ROWS, kd)
-    rows = next(r for r in range(64, ROWS + 1, 64) if lib().vpt_col_sums_parts(r, kd) == want)
+    want = lib().vpt_col_sums_parts(N, kd)
+    rows = next(r for r in range(64, N + 1, 64) if lib().vpt_col_sums_parts(r, kd) == want)
     _norm_case(f"{width} LayerNorm dense row {kd} rows={rows}", rows, 1, kd, (Hf, Wf, C2), 55)
     nat.device_check()
 
@@ -225,7 +244,7 @@ def unique_max_input(Fn, H, W, C, g):
     return zp(torch.where(keep, v, torch.zeros((), device=DEV)) / 64)
 
 
-@pytest.mark.parametrize("width", WIDTHS)
+@pytest.mark.parametrize("width", MODELS)
 def test_maxpool_backward_at_production_shapes(width):
     for i, (H, W, C) in enumerate(SHAPES[width]["pools"]):
         g = gen(60 + i)
@@ -238,21 +257,43 @@ def test_maxpool_backward_at_production_shapes(width):
     nat.device_check()
 
 
-@pytest.mark.parametrize("C0", sorted({s["firstconv"][2] for s in SHAPES.values()} | {256}))
-def test_firstconv_backward_at_production_frames(C0):
-    """C0 = 256 runs the other template instance of the kernel (one 256-thread block per SM)."""
+def _drop_pool_near_ties(img, w, b, dy, rtol=1e-4):
+    """zero dy (ZP, in place) at the pooled pixels whose two largest positive pre-pool values lie within rtol of each other (float64
+    conv of the first-conv reference); returns how many"""
+    C0 = w.shape[0]
+    x = img.to(F64).permute(0, 3, 1, 2) / 255.0
+    Wt = (w.to(F64) * 255.0).reshape(C0, 3, 3, 3).permute(0, 3, 1, 2)
+    y = F.pad(F.conv2d(x, Wt, b.to(F64), padding=1).relu(), (1, 1, 1, 1), value=float("-inf"))
+    top = y.unfold(2, 3, 2).unfold(3, 3, 2).reshape(*y.shape[:2], (y.shape[2] - 1) // 2, (y.shape[3] - 1) // 2, 9).topk(2, -1).values
+    near = (top[..., 0] > 0) & (top[..., 0] - top[..., 1] <= rtol * top[..., 0])
+    dy[:, :-1, :-1][near.permute(0, 2, 3, 1)] = 0
+    return int(near.sum())
+
+
+FC_C0 = sorted({SHAPES[w]["firstconv"][2] for w in WIDTHS} | {256})
+
+
+@pytest.mark.parametrize("C0,f32", [(c, False) for c in FC_C0] + [(192, True), (256, True)], ids=[str(c) for c in FC_C0] + ["192-f32", "256-f32"])
+def test_firstconv_backward_at_production_frames(C0, f32):
+    """C0 = 256 runs the other template instance of the kernel (one 256-thread block per SM); f32: non-integer fp32 frames on the uint8
+    scale, some outside [0, 255] (vpt_firstconv_bwd_f32, the pixel-gradient path)."""
     H, W = SHAPES["3x"]["firstconv"][:2]
     g = gen(70)
-    img = torch.randint(0, 256, (16, H, W, 3), dtype=torch.uint8, generator=g, device=DEV)
+    if f32:
+        img = torch.rand((16, H, W, 3), generator=g, device=DEV) * 340.0 - 40.0
+    else:
+        img = torch.randint(0, 256, (16, H, W, 3), dtype=torch.uint8, generator=g, device=DEV)
     w = randn((C0, 27), g, 0.2 / 255.0)
     b = randn((C0,), g, 0.1)
     dy = zp(randn((16, H // 2, W // 2, C0), g))
+    # fp32 and float64 may pick different arg-maxima where two pooling-window values nearly tie (one such flip moves rel-L2 to ~5e-4):
+    # those pooled pixels get a zero gradient, so either choice gives the same dW
+    ties = _drop_pool_near_ties(img, w, b, dy)
     dW, db = ops.firstconv_bwd(img, w, b, dy, C0)
     dW_r, db_r = Rf.firstconv_bwd(img, w, b, dy)
-    # fp32 and float64 may pick different arg-maxima where two pooling-window values nearly tie, so the bound is on rel-L2, not per
-    # element; these seeded inputs have no such tie (a flip would move rel-L2 to ~1e-3)
     e_w, e_b = rel(dW / 255.0, dW_r), rel(db, db_r)
-    print(f"firstconv bwd C0={C0} {H}x{W} F=16: rel-L2 dW {e_w:.2e} db {e_b:.2e} (bound {FC_L2:.0e})")
+    print(f"firstconv bwd C0={C0} {'fp32' if f32 else 'u8'} frames {H}x{W} F=16 ({ties} near-tied pooling windows dropped): rel-L2 dW {e_w:.2e} "
+          f"db {e_b:.2e} (bound {FC_L2:.0e})")
     assert e_w <= FC_L2 and e_b <= FC_L2
     nat.device_check()
 
@@ -302,6 +343,60 @@ def test_softmax_backward_and_head_bias_sums(width):
         check_bf16(f"{width} softmax bwd {name} n={n} col0={c0}", dlog[:, c0:c0 + n], Rf.softmax_bwd(logp, idx, scale), BF_FLOOR_SOFTMAX)
     cs = ops.col_sums(dlog)[1]  # head bias gradients
     check_sum(f"{width} col sums of d logits ({s['ld_logits']} columns)", cs, dlog.to(F64).sum(0), dlog.to(F64).abs().sum(0), DLOG_ELEM, DLOG_L2)
+    nat.device_check()
+
+
+def test_unmasked_attention_backward_at_idm_shapes():
+    """the IDM's attention (mask "none": every key of the 128-frame sequence) at B = 4, t = 128, 32 heads, writing d q | d k | d v into
+    a NaN-filled buffer with a row pitch wider than its 3h columns"""
+    s = SHAPES["idm"]
+    B, t, heads = s["B"], s["T"], s["heads"]
+    h = heads * 128
+    assert (B, t, heads, s["kcat"]) == (4, 128, 32, 3 * h)
+    g = gen(85)
+    q = (randn((B * t, h), g) * 3).to(BF16)
+    k, v = (randn((B, t, h), g) * 3).to(BF16), randn((B, t, h), g).to(BF16)
+    dO = randn((B * t, h), g).to(BF16)
+    ld = s["kcat"] + 24
+    ob = Guarded(B * t * ld, BF16)
+    out = ob.t.view(B * t, ld)
+
+    def call():
+        ob.raw.fill_(0xFF)
+        assert ops.attention_bwd(q, k, v, None, None, None, None, dO, out, B, t, 0, heads, causal=False) is None
+        assert (out[:, 3 * h:].view(torch.int16) == -1).all(), "attention_bwd wrote beyond its 3h columns"
+        return [out[:, :3 * h].clone()], [ob]
+
+    _run_twice(f"idm unmasked attention_bwd B={B} t={t} heads={heads}", call)
+    for i, (name, ref) in enumerate(zip(("dq", "dk", "dv"), Rf.full_attention_bwd(q, k, v, dO, B, t, heads))):
+        check_bf16(f"idm attention {heads} heads {name}", out[:, i * h:(i + 1) * h], ref, BF_FLOOR_ATTN)
+    nat.device_check()
+
+
+def test_grouped_softmax_backward_into_the_idm_logits_gradient():
+    """the IDM's factored heads (buttons 20 x 2, camera 2 x 11 classes) into their column blocks of the 64-wide logits gradient at 512
+    rows, as `IDMTrainer._idm_dlog` runs them: both heads accumulate the taken sub-actions' log-probs into one `lp`; the pad columns stay
+    0; then the head bias sums"""
+    s = SHAPES["idm"]
+    rows, ld = s["N"], s["ld_logits"]
+    g = gen(95)
+    dlog = torch.zeros((rows, ld), dtype=BF16, device=DEV)
+    scale = 1.0 / (2.0 * rows)
+    lp, lp_ref, c_end = None, torch.zeros(rows, dtype=F64, device=DEV), 0
+    for name, c0, n, groups in s["head_groups"]:
+        logp = torch.log_softmax(randn((rows, groups, n), g, 3.0), -1)
+        idx = torch.randint(0, n, (rows, groups), generator=g, device=DEV)
+        lp = ops.softmax_nll_bwd_grouped(logp, idx, scale, dlog, c0, lp=lp)
+        ref = Rf.softmax_bwd(logp.reshape(rows * groups, n), idx.reshape(-1), scale).reshape(rows, groups * n)
+        check_bf16(f"idm grouped softmax bwd {name} {groups}x{n} col0={c0}", dlog[:, c0:c0 + groups * n], ref, BF_FLOOR_GROUPED)
+        lp_ref += logp.to(F64).gather(-1, idx[..., None]).squeeze(-1).sum(-1)
+        c_end = c0 + groups * n
+    assert c_end < ld and (dlog[:, c_end:] == 0).all(), "wrote into the pad columns of the logits gradient"
+    e = ((lp.to(F64) - lp_ref).abs() / lp_ref.abs()).max().item()
+    print(f"idm summed log-prob of the taken sub-actions: max relative error {e:.2e} (bound 8e-7)")
+    assert e <= 8e-7  # measured 2.1e-7 (H100 80GB HBM3, 700 W)
+    cs = ops.col_sums(dlog)[1]
+    check_sum(f"idm col sums of d logits ({ld} columns)", cs, dlog.to(F64).sum(0), dlog.to(F64).abs().sum(0), DLOG_ELEM, DLOG_L2)
     nat.device_check()
 
 

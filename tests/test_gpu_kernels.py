@@ -106,6 +106,17 @@ def test_gemm_linear_multi_tile_long_k():
     _gemm_case(20000, 256, 512, g, bias=True, relu=1)     # more tiles than SMs: persistent loop + staging-tile reuse
 
 
+def test_gemm_partial_last_k_tile():
+    """K = 3h + 10 heads rounded up to 8, the q | k | v | r dgrad GEMM of the backward with its residual at the 1x / 2x / 3x widths: the
+    last 64-wide K tile is 16, 32 and 48 columns wide.  K = 64: one K tile (the IDM's heads dgrad)."""
+    g = torch.Generator().manual_seed(5)
+    for K in (3152, 6304, 9456):
+        assert K % 64 in (16, 32, 48)
+        _gemm_case(256, 512, K, g, residual=BF16)
+    _gemm_case(512, 1024, 64, g)
+    _gemm_case(300, 200, 64, g, residual=BF16)
+
+
 def test_gemm_linear_epilogues():
     g = torch.Generator().manual_seed(2)
     _gemm_case(384, 512, 256, g, fold=True, relu=1, stats=1)
