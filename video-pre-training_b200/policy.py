@@ -14,12 +14,16 @@ parameter changes) they are re-laid-out for the kernels (`_Prepared`): conv weig
 the input GroupNorm gamma folded in plus the 9 border-class fold tables, linear weights with LayerNorm folded, the
 `dense` columns permuted from C,H,W to H,W,C order.
 
+`encode(img)` runs the CNN part (frames -> the `dense` layer's output and its row statistics, `FrameLatents`) on its own, and
+`forward({"img_latent": latents}, ...)` the rest of the network from them.
+
 `forward` runs under no_grad and returns detached tensors; the trainers have their own hand-written backward (training.py).
 After `set_autograd(True)` a forward in grad mode (with a parameter that requires grad) is instead an autograd `Function` on that
 same backward, so that `loss.backward()` trains the model (training._AutogradRunner).  There is no CPU path: CPU tensors raise.
 """
 import functools
 import math
+import weakref
 from collections import OrderedDict
 from typing import Dict, Optional
 
@@ -404,6 +408,79 @@ def frames_f32(img):
     return img.to(torch.float32)
 
 
+LATENT_KEY = "img_latent"  # the observation key of cached CNN latents: policy({"img_latent": lat}, first, state)
+CNN_PREFIXES = ("img_process.cnn.", "conv3d_layer.")  # the network's parameters at or below the `dense` layer: the CNN part
+
+
+class FrameLatents:
+    """The output of the CNN part of a network (`MinecraftPolicy.encode`): per frame the `dense` layer's output `x`, bf16 (..., 256), and
+    its row statistics `stats`, fp32 (..., 2) (mean, rstd from the dense GEMM's epilogue, which `img_process.linear`'s folded LayerNorm
+    reads), over the leading dimensions (B, T).  `token` identifies the encoding network's CNN weights (`MinecraftPolicy.check_latents`).
+
+    Only what a data loader needs: indexing over the leading dimensions, `FrameLatents.cat(list, dim)` and `.to(device)`.  Latents carry
+    no autograd graph and cannot require grad.  The IDM's latents hold its conv3d pre-stage, which mixes five neighbouring frames of a
+    sequence: they stay valid when re-batched along B, not when sliced along T."""
+
+    def __init__(self, x, stats, token=None):
+        if x.requires_grad or stats.requires_grad:
+            raise ValueError("FrameLatents carry no autograd graph: x and stats must not require grad")
+        if tuple(stats.shape) != (*x.shape[:-1], 2):
+            raise ValueError(f"FrameLatents: stats {tuple(stats.shape)} must be x's leading shape {tuple(x.shape[:-1])} + (2,)")
+        self.x, self.stats, self.token = x, stats, token
+
+    @property
+    def shape(self):
+        """The leading (frame) dimensions, (B, T) for a forward's input."""
+        return self.x.shape[:-1]
+
+    @property
+    def device(self):
+        return self.x.device
+
+    @property
+    def requires_grad(self):
+        return self.x.requires_grad or self.stats.requires_grad
+
+    def __getitem__(self, idx):
+        parts = idx if isinstance(idx, tuple) else (idx,)
+        used = sum(0 if p is None else p.dim() if isinstance(p, torch.Tensor) and p.dtype == torch.bool else 1 for p in parts)
+        if any(p is Ellipsis for p in parts) or used > self.x.dim() - 1:
+            raise IndexError(f"FrameLatents index only the leading {self.x.dim() - 1} dimension(s), without Ellipsis")
+        return FrameLatents(self.x[idx], self.stats[idx], self.token)
+
+    @staticmethod
+    def cat(latents, dim=0):
+        """torch.cat over a leading dimension of latents encoded with the same CNN weights."""
+        latents = list(latents)
+        lead = latents[0].x.dim() - 1
+        if not -lead <= dim < lead:
+            raise IndexError(f"FrameLatents.cat: dim {dim} is not one of the {lead} leading dimension(s)")
+        dim %= lead
+        if any(lat.token != latents[0].token for lat in latents[1:]):
+            raise ValueError("FrameLatents.cat: the latents were encoded with different CNN weights")
+        return FrameLatents(torch.cat([lat.x for lat in latents], dim), torch.cat([lat.stats for lat in latents], dim), latents[0].token)
+
+    def to(self, device, non_blocking=False):
+        return FrameLatents(self.x.to(device, non_blocking=non_blocking), self.stats.to(device, non_blocking=non_blocking), self.token)
+
+
+def _ob_input(ob):
+    """The network input of an observation dict: the frames `ob["img"]` or the latents `ob["img_latent"]` (exactly one of them)."""
+    if LATENT_KEY not in ob:
+        return ob["img"]
+    if "img" in ob:
+        raise ValueError(f"the observation holds both 'img' and {LATENT_KEY!r}: pass one of them")
+    lat = ob[LATENT_KEY]
+    if not isinstance(lat, FrameLatents):
+        raise TypeError(f"ob[{LATENT_KEY!r}] must be FrameLatents (from encode), got {type(lat).__name__}")
+    return lat
+
+
+def _add_time(v):
+    """(B, ...) -> (B, 1, ...) for frames or latents (get_output_for_observation)."""
+    return v[:, None] if isinstance(v, FrameLatents) else v.unsqueeze(1)
+
+
 def check_recompute_frames(v):
     """`recompute_frames` of the trainers and `set_autograd`: None (keep the CNN's activations for the backward) or a positive int."""
     if v is not None and (isinstance(v, bool) or not isinstance(v, int) or v <= 0):
@@ -658,32 +735,101 @@ class MinecraftPolicy(nn.Module):
                                              mr_y=mr_y, hmid=hmid, z=z, mr_z=mr_z) if l >= self._tape["blocks_from"] else None)
         return z, mr_z, (new_mask, (new_k, new_v))
 
-    # -- whole net -------------------------------------------------------------------------------------------
+    # -- cached CNN latents -----------------------------------------------------------------------------------
+    def _cnn_params(self):
+        """The parameters of the CNN part (`CNN_PREFIXES`): the ImpalaCNN with its `dense` layer and, for the IDM, the conv3d pre-stage."""
+        return [p for n, p in self.named_parameters() if n.startswith(CNN_PREFIXES)]
+
+    def _cnn_token(self):
+        """The token `encode` gives its latents: this network (weakly) and the storage and in-place versions of its CNN parameters, the key
+        the kernel-layout copies are rebuilt by (`_Versioned`)."""
+        return weakref.ref(self), _fingerprint(self._cnn_params())
+
+    def check_latents(self, lat: FrameLatents):
+        """Raises ValueError for latents this network cannot take: not (B, T) of `cnn_outsize` bf16 values with fp32 (mean, rstd), or
+        encoded by this very network before its CNN changed (an optimizer step, a load, a move).  Latents of another network with the same
+        `cnn_outsize` are accepted: whether its CNN weights are this one's is the caller's responsibility.  No launch."""
+        if not isinstance(lat, FrameLatents):
+            raise TypeError(f"expected FrameLatents, got {type(lat).__name__}")
+        if lat.x.dim() != 3 or lat.x.shape[-1] != self.cfg.cnn_outsize or lat.x.dtype != BF16 or lat.stats.dtype != F32:
+            raise ValueError(f"latents must be x bf16 (B, T, {self.cfg.cnn_outsize}) with stats fp32 (B, T, 2) "
+                             f"(got x {lat.x.dtype} {tuple(lat.x.shape)}, stats {lat.stats.dtype} {tuple(lat.stats.shape)})")
+        if lat.token is not None:
+            net, fp = lat.token
+            if net() is self and fp != _fingerprint(self._cnn_params()):
+                raise ValueError("stale latents: this network's CNN parameters changed (an update, a load or a move) since they were encoded")
+        ops.require_cuda(lat.x)
+
     @torch.no_grad()
-    def _forward_impl(self, img, first, state_in):
+    def encode(self, img) -> FrameLatents:
+        """The CNN part of the forward (frames -> the `dense` layer's output and its row statistics) in the training layout: the kernels
+        and chunks of the trainers' forward with the CNN frozen, so that a step from these latents is bit-identical to that step from the
+        frames.  `img` (B, T, H, W, 3), uint8 or float on the uint8 scale as in the forward; bf16 mode only."""
         cfg = self.cfg
         ops.require_cuda(img)
         img = frames_f32(img)
         B, t = img.shape[:2]
         frame_shape = (cfg.img_shape[0], cfg.img_shape[1], 3)
         assert tuple(img.shape[2:]) == frame_shape, f"img shape {tuple(img.shape[2:])} != {frame_shape}"
+        if self.precision != "bf16":
+            raise NotImplementedError("encode runs in the bf16 mode only (set_precision('bf16'))")
+        token = self._cnn_token()
+        xd, mr_d = self._cnn_part(img.reshape(B * t, *frame_shape).contiguous(), t, self.prepared(), train=True)
+        return FrameLatents(xd.view(B, t, cfg.cnn_outsize), mr_d.view(B, t, 2), token)
+
+    # -- whole net -------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def _forward_impl(self, img, first, state_in):
+        """img: frames (B, T, H, W, 3), or FrameLatents (B, T): the CNN part is then skipped."""
+        cfg = self.cfg
+        latents = isinstance(img, FrameLatents)
+        if latents:
+            self.check_latents(img)
+        else:
+            ops.require_cuda(img)
+            img = frames_f32(img)
+        B, t = img.shape[:2]
+        frame_shape = (cfg.img_shape[0], cfg.img_shape[1], 3)
+        if not latents:
+            assert tuple(img.shape[2:]) == frame_shape, f"img shape {tuple(img.shape[2:])} != {frame_shape}"
         assert len(state_in) == cfg.n_layers, \
             f"Length of state {len(state_in)} did not match length of blocks {cfg.n_layers}"  # lib/util.py:117-119
         if self.precision == "fp32":
             if self._tape is not None:
                 raise NotImplementedError("the BC step runs in the bf16 mode only")
+            if latents:
+                raise NotImplementedError("the forward from latents runs in the bf16 mode only")
             from . import precise
             return precise.forward(self, img, first, state_in)
         if self.precision != "bf16":
             raise ValueError(f"unknown precision {self.precision!r} (use 'bf16' or 'fp32')")
         prep = self.prepared()
         N = B * t
-        frames = img.reshape(N, *frame_shape).contiguous()
-        first_u8 = first.to(device=img.device, dtype=torch.bool).contiguous().view(torch.uint8)
+        tape = self._tape
+        if latents:
+            first_u8 = first.to(device=img.device, dtype=torch.bool).contiguous().view(torch.uint8)
+            xd, mr_d = img.x.reshape(N, cfg.cnn_outsize).contiguous(), img.stats.reshape(N, 2).contiguous()
+            if tape is not None:  # nothing of the CNN part: the backward stops above the dense layer
+                tape.update(prep=prep, xd=xd, mr_d=mr_d, cnn_chunks=[])
+        else:
+            frames = img.reshape(N, *frame_shape).contiguous()
+            first_u8 = first.to(device=img.device, dtype=torch.bool).contiguous().view(torch.uint8)
+            xd, mr_d = self._cnn_part(frames, t, prep, train=tape is not None)
+        if tape is not None:
+            tape.update(first_u8=first_u8)
+        return self._upper_part(xd, mr_d, first_u8, state_in, B, t, prep)
+
+    def _cnn_part(self, frames, t, prep: _Prepared, train: bool):
+        """frames [N, H, W, 3] (whole sequences of t frames) -> (xd bf16 [N, cnn_outsize], mr_d fp32 [N, 2]): the conv3d pre-stage (IDM),
+        the ImpalaCNN in frame chunks and the dense layer.  train: the training layout (`_cnn_chunk`); with a tape (self._tape) it also
+        records what the backward needs."""
+        cfg = self.cfg
+        N = frames.shape[0]
+        frame_shape = tuple(frames.shape[1:])
         Hf, Wf = cfg.final_hw
         C2 = cfg.chans[-1]
         # ---- ImpalaCNN in frame chunks (bounds the activation workspace), then ONE dense GEMM over all frames
-        cnn_out = torch.empty((N, Hf + 1, Wf + 1, C2), dtype=BF16, device=img.device)
+        cnn_out = torch.empty((N, Hf + 1, Wf + 1, C2), dtype=BF16, device=frames.device)
         mrs = []
         tape = self._tape
         # training forward: tape["recompute"] None keeps every stack's activations for the backward (one CNN pass per call); an integer
@@ -699,7 +845,7 @@ class MinecraftPolicy(nn.Module):
         for f0 in range(0, N, step):
             F_ = min(step, N - f0)
             chunk = frames[f0:f0 + F_] if cfg.conv3d_out is None else frames[f0:f0 + F_].view(F_ // t, t, *frame_shape)
-            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_], train=tape is not None, stacks=stacks,
+            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_], train=train, stacks=stacks,
                                     record_from=0 if tape is None else tape["stacks_from"])
             mrs.append(mr)
         mr_c = mrs[0] if len(mrs) == 1 else torch.cat(mrs, 0)
@@ -707,9 +853,15 @@ class MinecraftPolicy(nn.Module):
         xd, mr_d = self._linear(cnn_out.view(N, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
         if tape is not None:
             assert not (cnn_bwd and recompute is None and len(mrs) != 1), "the stored tape holds one CNN chunk (training._Trainer.check_call)"
-            tape.update(prep=prep, frames=frames, first_u8=first_u8, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d,
+            tape.update(prep=prep, frames=frames, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d,
                         cnn_chunks=[(f0, min(f0 + step, N)) for f0 in range(0, N, step)] if cnn_bwd else [])
-        del cnn_out
+        return xd, mr_d
+
+    def _upper_part(self, xd, mr_d, first_u8, state_in, B, t, prep: _Prepared):
+        """(xd, mr_d) of `_cnn_part` or of cached latents -> img_process.linear -> the transformer -> lastlayer -> final_ln:
+        (latent bf16 [N, h], latent fp32 (B, t, h), state_out).  Records into the tape (self._tape) when there is one."""
+        cfg = self.cfg
+        tape = self._tape
         self._tap("img_process.cnn.dense", xd)
         x, mr_x = self._linear(xd, prep.linear, cfg.hidsize, mr=mr_d, relu=1, want_stats=True)
         self._tap("img_process", x)
@@ -732,10 +884,11 @@ class MinecraftPolicy(nn.Module):
     def forward(self, ob, state_in, context):
         """lib/policy.py:193-218."""
         first = context["first"]
-        if _differentiable(self, ob["img"]):
-            (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
+        img = _ob_input(ob)
+        if _differentiable(self, img):
+            (latent,), state_out = _autograd_runner(self).run(img, first, state_in)
         else:
-            _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
+            _, latent, state_out = self._forward_impl(img, first, state_in)
         if self.single_output:
             return latent, state_out
         return (latent, latent), state_out
@@ -754,10 +907,11 @@ class InverseActionNet(MinecraftPolicy):
     def forward(self, ob, state_in, context):
         """lib/policy.py:374-392 -> ((pi_latent, None), state_out)."""
         first = context["first"]
-        if _differentiable(self, ob["img"]):
-            (latent,), state_out = _autograd_runner(self).run(ob["img"], first, state_in)
+        img = _ob_input(ob)
+        if _differentiable(self, img):
+            (latent,), state_out = _autograd_runner(self).run(img, first, state_in)
         else:
-            _, latent, state_out = self._forward_impl(ob["img"], first, state_in)
+            _, latent, state_out = self._forward_impl(img, first, state_in)
         return (latent, None), state_out
 
 
@@ -836,13 +990,25 @@ class _PolicyBase(nn.Module):
 
         An `img` that requires grad (a floating dtype on the uint8 scale, `frames_f32`) makes the forward differentiable even with every
         parameter frozen, and `loss.backward()` then writes `img.grad`; the trainable parameters' gradients are those of the same call
-        without it, bit for bit."""
+        without it, bit for bit.
+
+        The forward also takes cached latents, `{"img_latent": policy.encode(img)}`, with every parameter of the CNN part (`img_process.cnn.*`,
+        the IDM's `conv3d_layer.*`) frozen (ValueError otherwise, before any launch): no CNN runs, forward or backward, the gradients are those
+        of the same call from `img` with the CNN frozen, and the limits are `max_call_frames` / `max_call_batch`, T <= 128 for the IDM and
+        the bf16 mode; `recompute_frames` has nothing to recompute and is ignored for such a call.  Latents carry no graph (no image
+        gradient)."""
         recompute_frames = check_recompute_frames(recompute_frames)
         self._autograd = bool(on)
         self._state_grad = bool(on) and bool(state_grad)
         self._recompute_frames = recompute_frames if on else None
         self.net.set_autograd(on, state_grad=state_grad, recompute_frames=recompute_frames)
         return self
+
+    def encode(self, img) -> FrameLatents:
+        """`self.net.encode(img)`: the CNN part of the forward, once, for frames whose CNN output is used again (the epochs of a BC
+        fine-tune, the PPO epochs over one rollout, the frozen reference policy): `policy({"img_latent": lat}, first, state)` and the
+        trainers' `loss_and_grad(lat, ...)` then run the rest.  See `MinecraftPolicy.encode` and INTEGRATION.md, "cached latents"."""
+        return self.net.encode(img)
 
     def set_precision(self, precision: str):
         """"bf16" (default, production: bf16 operands, 1e-2 tolerance) or "fp32" (fp32-parity mode, precise.py: 1e-3 tolerance)."""
@@ -1147,12 +1313,13 @@ class MinecraftAgentPolicy(_PolicyBase):
             mask = obs.pop("mask", None)
         else:
             mask = None
-        if _differentiable(self, obs["img"]):
-            outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
+        img = _ob_input(obs)
+        if _differentiable(self, img):
+            outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
             pi_logits = OrderedDict(zip(self.head_specs, outs[:-1]))
             return (pi_logits, outs[-1], None), state_out
-        lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in)
-        B, t = obs["img"].shape[:2]
+        lat_bf16, _, state_out = self.net._forward_impl(img, first, state_in)
+        B, t = img.shape[:2]
         pi_logits, vpred = self._heads(lat_bf16, B, t, mask)
         return (pi_logits, vpred, None), state_out
 
@@ -1180,8 +1347,8 @@ class MinecraftAgentPolicy(_PolicyBase):
         return self.pi_head.kl_divergence(pd1, pd2)
 
     def get_output_for_observation(self, obs, state_in, first):
-        """lib/policy.py:287-305."""
-        obs = {k: v.unsqueeze(1) for k, v in obs.items()}
+        """lib/policy.py:287-305.  obs["img"] (B, H, W, 3) or obs["img_latent"], FrameLatents (B,)."""
+        obs = {k: _add_time(v) for k, v in obs.items()}
         first = first.unsqueeze(1)
         (pd, vpred, _), state_out = self(obs=obs, first=first, state_in=state_in)
         return pd, self.denormalize(vpred)[:, 0], state_out
@@ -1237,11 +1404,12 @@ class InverseActionPolicy(_PolicyBase):
             mask = obs.pop("mask", None)
         else:
             mask = None
-        if _differentiable(self, obs["img"]):
-            outs, state_out = _autograd_runner(self).run(obs["img"], first, state_in, mask)
+        img = _ob_input(obs)
+        if _differentiable(self, img):
+            outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
             return (OrderedDict(zip(self.head_specs, outs)), None, None), state_out
-        lat_bf16, _, state_out = self.net._forward_impl(obs["img"], first, state_in)
-        B, t = obs["img"].shape[:2]
+        lat_bf16, _, state_out = self.net._forward_impl(img, first, state_in)
+        B, t = img.shape[:2]
         pi_logits, _ = self._heads(lat_bf16, B, t, mask)
         return (pi_logits, None, None), state_out
 

@@ -45,7 +45,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops
-from .policy import BF16, F32, InverseActionPolicy, MinecraftAgentPolicy, _dense_from_zp
+from .policy import BF16, CNN_PREFIXES, F32, FrameLatents, InverseActionPolicy, MinecraftAgentPolicy, _dense_from_zp
 from .policy import _rot  # noqa: F401  (the dgrad weight layout lived here; code that imports it from this module keeps working)
 
 
@@ -252,13 +252,27 @@ class _Trainer:
         """The limits of one call, checked by every entry point before any launch so that a call that cannot finish accumulates nothing:
         the bf16 mode; for the IDM at most `IDMTrainer.max_t` frames per sequence; with the stored tape (recompute_frames None) and a
         backward that enters the CNN (`_grad_plan`, want_dimg: see there) at most `net.cnn_chunk_frames` (the IDM: `net.idm_chunk_frames`)
-        frames, the one CNN chunk the tape holds; otherwise `max_call_frames` frames and B <= `max_call_batch`."""
+        frames, the one CNN chunk the tape holds; otherwise `max_call_frames` frames and B <= `max_call_batch`.
+        From cached latents (`FrameLatents`, no CNN tape) `max_call_frames` and `max_call_batch` hold, and ValueError is raised for latents
+        the network cannot take (`MinecraftPolicy.check_latents`: shape, stale), latents that require grad, and a parameter of the CNN part
+        (`img_process.cnn.*`, `conv3d_layer.*`) that requires grad: it would get no gradient."""
         net = self.net
         B, t = img.shape[:2]
         if net.precision != "bf16":
             raise NotImplementedError("training and the differentiable forward run in the bf16 mode only (set_precision('bf16'))")
         if net.cfg.conv3d_out is not None and t > IDMTrainer.max_t:
             raise NotImplementedError(f"the IDM's backward takes at most {IDMTrainer.max_t} frames per sequence (got T = {t})")
+        if isinstance(img, FrameLatents):
+            if img.requires_grad:
+                raise ValueError("latents carry no autograd graph: there is no gradient wrt them (pass the frames for an image gradient)")
+            trainable = next((n for n, p in net.named_parameters() if p.requires_grad and n.startswith(CNN_PREFIXES)), None)
+            if trainable is not None:
+                raise ValueError(f"a call from latents trains nothing at or below img_process.cnn.dense, but {trainable} requires grad: "
+                                 "freeze the CNN part (requires_grad_(False)) or pass the frames")
+            net.check_latents(img)
+            if B * t > self.max_call_frames or B > self.max_call_batch:
+                raise NotImplementedError(f"at most {self.max_call_frames} frames and B <= {self.max_call_batch} per call (got B = {B}, T = {t})")
+            return
         if self.recompute_frames is None and self._grad_plan(want_dimg=want_dimg)["cnn"]:
             limit = net.cnn_chunk_frames if net.cfg.conv3d_out is None else net.idm_chunk_frames
             if B * t > limit:
@@ -361,8 +375,10 @@ class _Trainer:
         # again from the frames and the forward's weights, used, and dropped before the next chunk.  (No chunk when the CNN is frozen.)
         # The gradient wrt the CNN input (`_cnn_bwd`) is the image gradient for the agent's fused first conv, and for the IDM the gradient
         # wrt the conv3d output, which its own backward takes to the weights and, when wanted, to the image; each chunk writes its frames'.
-        frames = tape["frames"]
         chunks = tape["cnn_chunks"]
+        if not chunks:  # the CNN is frozen, or the call came from cached latents (no frames): the backward ends above the dense layer
+            return dmem
+        frames = tape["frames"]
         dimg = None
         if tape["want_dimg"] and len(chunks) > 1:
             dimg = torch.empty((frames.shape[0], *frames.shape[1:3], 3), dtype=F32, device=frames.device)
@@ -565,6 +581,11 @@ class BCTrainer(_Trainer):
     and the backward stops at the lowest unit that trains.  With the whole ImpalaCNN (`img_process.cnn.*`) frozen the forward keeps no
     CNN activation, so a call is bounded by `max_call_frames` instead of the stored tape, and `upper_grads_ready` fires at the end of the
     backward.  With nothing trainable the call returns the loss and state_out and runs no backward.
+
+    `img` may instead be cached latents (`FrameLatents`, `policy.encode(img)`, with the CNN part frozen): the call then runs no CNN, forward
+    or backward, and gives the loss, state_out and gradients of the same call from `img` with the CNN frozen, bit for bit.  Its limits are
+    `max_call_frames` and `max_call_batch`; `recompute_frames` has nothing to recompute and is ignored for such a call.  The same holds for
+    `RLTrainer` and `IDMTrainer` (see INTEGRATION.md, "cached latents").
     """
 
     def __init__(self, policy: MinecraftAgentPolicy, recompute_frames=None):
