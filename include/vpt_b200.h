@@ -290,6 +290,21 @@ int vpt_attention(const void* Q, const void* Kf, const void* Vf, const float* R,
                   const uint8_t* first, int64_t first_stride, const uint8_t* smask, void* out, int32_t B, int32_t t,
                   int32_t maxlen, int32_t heads, int32_t nbasis, int32_t causal, void* stream);
 
+/* The KV memory as a ring (policy.py RingState), for t = 1 rollout steps that update the state in place:
+ *   Kr, Vr bf16 [B][maxlen][h], smask u8 [B][maxlen]; [memory | chunk] key j (j in [0, maxlen]) is physical row (off + j) % maxlen,
+ *   so the step's own row (j = maxlen) is row `off`; off = ring_off[0], a device int32 in [0, maxlen) read by the kernels, so one captured
+ *   CUDA graph serves every step.
+ * vpt_ring_write     knew, vnew bf16 [B][h] -> ring row `off` of Kr / Vr; smask[b][off] = 1 and, where first[b], smask[b][j] = 0 for j != off
+ *                    (vpt_state_mask_update at t = 1).  Runs before the attention: row `off` held memory key j = 0, which t = 1 never reads.
+ * vpt_attention_ring vpt_attention (causal, t = 1) on the ring: the same keys, tiles and sums as the linear layout, so the same bits.
+ * vpt_ring_advance   ring_off[0] = (ring_off[0] + 1) % maxlen, once per step after the last layer. */
+int vpt_ring_write(const void* knew, const void* vnew, void* Kr, void* Vr, uint8_t* smask, const uint8_t* first, int64_t first_stride,
+                   const int32_t* ring_off, int32_t B, int32_t maxlen, int32_t h, void* stream);
+int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                       const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, void* out, int32_t B,
+                       int32_t maxlen, int32_t heads, int32_t nbasis, void* stream);
+int vpt_ring_advance(int32_t* ring_off, int32_t maxlen, void* stream);
+
 /* ----------------------------------------------------------------------------------------------------------
  * Action heads (lib/action_head.py:163-207)
  * -------------------------------------------------------------------------------------------------------- */

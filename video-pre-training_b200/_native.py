@@ -115,6 +115,10 @@ SIGNATURES = {
     "vpt_copy_rows2": (_I, [_P, _P, _I, _L, _L, _L, _P, _P, _I, _L, _L, _L, _I, _I, _I, _P]),
     "vpt_state_mask_update": (_I, [_P, _P, _L, _P, _I, _I, _I, _P]),
     "vpt_attention": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    # the KV memory as a ring (policy.py RingState, csrc/ring.cuh)
+    "vpt_ring_write": (_I, [_P, _P, _P, _P, _P, _P, _L, _P, _I, _I, _I, _P]),
+    "vpt_attention_ring": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "vpt_ring_advance": (_I, [_P, _I, _P]),
     "vpt_log_softmax": (_I, [_P, _L, _I, _I, _P, _L, _P]),
     "vpt_gumbel_argmax": (_I, [_P, _P, _P, _L, _I, _P]),
     "vpt_gather_logprob": (_I, [_P, _P, _P, _L, _I, _I, _P]),

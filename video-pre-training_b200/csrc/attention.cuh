@@ -45,11 +45,30 @@ __device__ __forceinline__ void load_tile_64x128(__nv_bfloat16* dst, const __nv_
     }
 }
 
+// Ring layout of the KV memory (t = 1 rollout steps, vpt_attention_ring): K / V are bf16 [B][maxlen][h] and smask u8 [B][maxlen] with
+// [memory | chunk] key j at physical row (off + j) % maxlen, so the new chunk row (j = maxlen) sits at `off`, where memory key j = 0 was
+// (outside the t = 1 band).  Only the row addresses change: the key order and tiling are those of the linear layout, so are the bits.
+__device__ __forceinline__ int ring_row(int row, int off, int maxlen) { return (off + row) % maxlen; }
+
+// load_tile_64x128 for a ring: memory-coordinate rows [row0, row0+64), zero beyond rows_total (tiles may wrap)
+__device__ __forceinline__ void load_tile_64x128_ring(__nv_bfloat16* dst, const __nv_bfloat16* src, long long ld, int row0, int rows_total,
+                                                      int col0, int off, int maxlen) {
+    for (int i = threadIdx.x; i < 64 * 16; i += kAttThreads) {
+        const int r = i >> 4, ch = i & 15;
+        __nv_bfloat16* d = dst + r * kAttPitch + ch * 8;
+        const int row = row0 + r;
+        if (row >= 0 && row < rows_total) cp_async16(d, src + (long long)ring_row(row, off, maxlen) * ld + col0 + ch * 8);
+        else *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
+    }
+}
+
+// RING: K / V / smask in the ring layout above, `off` read from ring_off[0] on the device (t = 1, causal)
+template <bool RING>
 __global__ void __launch_bounds__(kAttThreads) attention_kernel(
     const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __restrict__ Kf, const __nv_bfloat16* __restrict__ Vf,
     const float* __restrict__ R, long long ld_r, const float* __restrict__ b_nd, const uint8_t* __restrict__ first,
     long long first_stride, const uint8_t* __restrict__ smask, __nv_bfloat16* __restrict__ out, int t, int maxlen, int heads,
-    int nbasis, int causal) {
+    int nbasis, int causal, const int* __restrict__ ring_off) {
     pdl_sync();
     extern __shared__ __align__(16) uint8_t att_smem[];
     __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(att_smem);
@@ -65,13 +84,16 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
     const int T = maxlen + t;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
     const __nv_bfloat16* Qb = Q + (long long)b * t * h;
-    const __nv_bfloat16* Kb = Kf + (long long)b * T * h;
-    const __nv_bfloat16* Vb = Vf + (long long)b * T * h;
+    const int off = RING ? ring_off[0] : 0;
+    const long long kv_rows = RING ? maxlen : T;  // rows per batch row of K / V
+    const __nv_bfloat16* Kb = Kf + (long long)b * kv_rows * h;
+    const __nv_bfloat16* Vb = Vf + (long long)b * kv_rows * h;
 
     load_tile_64x128(Qs, Qb, h, q0, t, head * kAttD);
     if (causal && maxlen > 0) {
         const bool mem_ok = (first[(long long)b * first_stride] == 0) && (smask != nullptr);
-        for (int j = threadIdx.x; j < maxlen; j += kAttThreads) Ms[j] = mem_ok ? smask[(long long)b * maxlen + j] : 0;
+        for (int j = threadIdx.x; j < maxlen; j += kAttThreads)
+            Ms[j] = mem_ok ? smask[(long long)b * maxlen + (RING ? ring_row(j, off, maxlen) : j)] : 0;
         for (int i = threadIdx.x; i < nbasis * maxlen; i += kAttThreads) Bs[i] = __ldg(b_nd + i);
         for (int i = threadIdx.x; i < kAttBQ * nbasis; i += kAttThreads) {
             const int r = i / nbasis, n = i % nbasis;
@@ -119,8 +141,13 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
 
     for (int kb0 = j_lo; kb0 <= j_hi; kb0 += kAttBK) {
         __syncthreads();  // previous block's K/V fully consumed (also orders the Es writes before first use)
-        load_tile_64x128(Ks, Kb, h, kb0, T, head * kAttD);
-        load_tile_64x128(Vs, Vb, h, kb0, T, head * kAttD);
+        if (RING) {
+            load_tile_64x128_ring(Ks, Kb, h, kb0, T, head * kAttD, off, maxlen);
+            load_tile_64x128_ring(Vs, Vb, h, kb0, T, head * kAttD, off, maxlen);
+        } else {
+            load_tile_64x128(Ks, Kb, h, kb0, T, head * kAttD);
+            load_tile_64x128(Vs, Vb, h, kb0, T, head * kAttD);
+        }
         cp_async_wait_all();
         __syncthreads();
 
@@ -226,7 +253,13 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
 // attention_long.cuh: the causal forward for a KV memory whose bias table does not fit this kernel's shared memory
 int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
                        const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
-                       int nbasis, cudaStream_t stream);
+                       int nbasis, const int* ring_off, cudaStream_t stream);
+
+// shared memory of attention_kernel for a causal band of `maxlen` keys with `nb` basis rows (nb = 0: mask "none")
+inline size_t attention_smem(int maxlen, int nb) {
+    return (size_t)(kAttBQ + 2 * kAttBK) * kAttPitch * 2 + ((size_t)kAttBQ * maxlen + (size_t)nb * maxlen + (size_t)kAttBQ * nb) * 4 +
+           (size_t)((maxlen + 15) / 16 * 16) + 16;
+}
 
 }  // namespace vpt
 
@@ -239,22 +272,46 @@ extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, cons
     else VPT_CHECK(maxlen == 0, "vpt_attention: mask 'none' has no KV memory (maxlen must be 0)");
     VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention: grid too large");
     const int nb = causal ? nbasis : 0;
-    size_t smem = (size_t)(kAttBQ + 2 * kAttBK) * kAttPitch * 2 + ((size_t)kAttBQ * maxlen + (size_t)nb * maxlen + (size_t)kAttBQ * nb) * 4 +
-                  (size_t)((maxlen + 15) / 16 * 16) + 16;
+    const size_t smem = attention_smem(maxlen, nb);
     if (smem > 227 * 1024) {  // only a causal band can be this long (mask 'none' has no memory): tile it over keys
         return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf),
                                   reinterpret_cast<const __nv_bfloat16*>(Vf), R, ld_r, b_nd, first, first_stride, smask,
-                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, (cudaStream_t)stream);
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, nullptr, (cudaStream_t)stream);
     }
     static size_t attr = 0;
     if (smem > attr) {
-        VPT_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        VPT_CUDA(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     dim3 grid((t + kAttBQ - 1) / kAttBQ, heads, B);
-    launch_k(attention_kernel, dim3(grid), dim3(kAttThreads), smem, (cudaStream_t)stream, 
+    launch_k(attention_kernel<false>, dim3(grid), dim3(kAttThreads), smem, (cudaStream_t)stream, 
         reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf), reinterpret_cast<const __nv_bfloat16*>(Vf), R,
-        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), t, maxlen, heads, nb, causal);
+        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), t, maxlen, heads, nb, causal, (const int*)nullptr);
+    VPT_LAUNCH_CHECK();
+    return VPT_OK;
+}
+
+extern "C" int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                                  const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, void* out, int32_t B,
+                                  int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
+              "vpt_attention_ring: bad arguments");
+    VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring: grid too large");
+    const size_t smem = attention_smem(maxlen, nbasis);
+    if (smem > 227 * 1024) {
+        return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kr),
+                                  reinterpret_cast<const __nv_bfloat16*>(Vr), R, ld_r, b_nd, first, first_stride, smask,
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, 1, maxlen, heads, nbasis, ring_off, (cudaStream_t)stream);
+    }
+    static size_t attr = 0;
+    if (smem > attr) {
+        VPT_CUDA(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = smem;
+    }
+    launch_k(attention_kernel<true>, dim3(1, heads, B), dim3(kAttThreads), smem, (cudaStream_t)stream,
+        reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kr), reinterpret_cast<const __nv_bfloat16*>(Vr), R,
+        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), 1, maxlen, heads, nbasis, 1, (const int*)ring_off);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
 }

@@ -31,11 +31,13 @@ constexpr int kAlPo = kAttD + 4;                 // fp32 pitch of the partial ou
 constexpr int kAlKK = 64;                        // key offsets (rows kernel) / query offsets (keys, mem kernels) per staged tile
 constexpr int kAlStage = kAlKK + kAbRows - 1;    // rows staged per tile: the tile's span over the CTA's 16 queries / keys
 
+// RING: K / V / smask in the ring layout of attention.cuh (vpt_attention_ring), `off` read from ring_off[0] on the device
+template <bool RING>
 __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
     const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __restrict__ Kf, const __nv_bfloat16* __restrict__ Vf,
     const float* __restrict__ R, long long ld_r, const float* __restrict__ b_nd, const uint8_t* __restrict__ first,
     long long first_stride, const uint8_t* __restrict__ smask, __nv_bfloat16* __restrict__ out, int t, int maxlen, int heads,
-    int nbasis, int nsplit) {
+    int nbasis, int nsplit, const int* __restrict__ ring_off) {
     pdl_sync();
     extern __shared__ __align__(16) uint8_t al_smem[];
     __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(al_smem);
@@ -50,8 +52,10 @@ __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
     const int h = heads * kAttD;
     const int T = maxlen + t;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
-    const __nv_bfloat16* Kb = Kf + (long long)b * T * h;
-    const __nv_bfloat16* Vb = Vf + (long long)b * T * h;
+    const int off = RING ? ring_off[0] : 0;
+    const long long kv_rows = RING ? maxlen : T;  // rows per batch row of K / V
+    const __nv_bfloat16* Kb = Kf + (long long)b * kv_rows * h;
+    const __nv_bfloat16* Vb = Vf + (long long)b * kv_rows * h;
     const bool mem_ok = (first[(long long)b * first_stride] == 0) && (smask != nullptr);
 
     load_tile_64x128(Qs, Q + (long long)b * t * h, h, q0, t, head * kAttD);
@@ -90,8 +94,13 @@ __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
     for (int tile = split * per; tile < tile_end; ++tile) {
         const int kb0 = j_lo + tile * kAttBK;
         __syncthreads();  // previous tile's K / V / Bt / Ms fully consumed
-        load_tile_64x128(Ks, Kb, h, kb0, T, head * kAttD);
-        load_tile_64x128(Vs, Vb, h, kb0, T, head * kAttD);
+        if (RING) {
+            load_tile_64x128_ring(Ks, Kb, h, kb0, T, head * kAttD, off, maxlen);
+            load_tile_64x128_ring(Vs, Vb, h, kb0, T, head * kAttD, off, maxlen);
+        } else {
+            load_tile_64x128(Ks, Kb, h, kb0, T, head * kAttD);
+            load_tile_64x128(Vs, Vb, h, kb0, T, head * kAttD);
+        }
         const int dbase = maxlen + q0 - kb0 - (kAttBK - 1);  // distance of (query q0, key kb0 + 63)
         for (int x = threadIdx.x; x < kAlNb * kAlDist; x += kAttThreads) {
             const int n = x / kAlDist, c = x % kAlDist, d = dbase + c;
@@ -99,7 +108,7 @@ __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
         }
         if (threadIdx.x < kAttBK) {
             const int j = kb0 + threadIdx.x;
-            Ms[threadIdx.x] = (j >= maxlen) ? 1 : (mem_ok && smask[(long long)b * maxlen + j] != 0);
+            Ms[threadIdx.x] = (j >= maxlen) ? 1 : (mem_ok && smask[(long long)b * maxlen + (RING ? ring_row(j, off, maxlen) : j)] != 0);
         }
         cp_async_wait_all();
         __syncthreads();
@@ -537,13 +546,15 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_mem_long_kernel(const __n
 // ---------------------------------------------------------------------------------------------------------------------------------
 int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
                        const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
-                       int nbasis, cudaStream_t stream) {
+                       int nbasis, const int* ring_off, cudaStream_t stream) {
     VPT_CHECK(nbasis <= kAlNb, "vpt_attention: nbasis=%d > %d", nbasis, kAlNb);
     const size_t smem = (size_t)(kAttBQ + 2 * kAttBK) * kAttPitch * 2 + (size_t)(kAlNb * kAlDist + 2 * kAttBQ) * 4 + kAttBK;
-    static bool attr_set = false;
-    if (!attr_set) {
-        VPT_CUDA(cudaFuncSetAttribute(attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set = true;
+    const bool ring = ring_off != nullptr;
+    auto kernel = ring ? attention_long_kernel<true> : attention_long_kernel<false>;
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[ring]) {
+        VPT_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr_set[ring] = true;
     }
     const int nqb = (t + kAttBQ - 1) / kAttBQ;
     const long long ctas = (long long)nqb * heads * B;
@@ -552,8 +563,8 @@ int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __
     if (ctas < num_sms()) nsplit = (int)min((long long)min(kAlSplitMax, band_tiles), (num_sms() + ctas - 1) / ctas);
     dim3 grid(nqb * nsplit, heads, B);
     if (nsplit == 1) {
-        launch_k(attention_long_kernel, grid, dim3(kAttThreads), smem, stream, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen,
-                 heads, nbasis, 1);
+        launch_k(kernel, grid, dim3(kAttThreads), smem, stream, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen, heads, nbasis, 1,
+                 ring_off);
     } else {
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
@@ -568,8 +579,7 @@ int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;  // launched without PDL: pdl_sync() is then a no-op and the launch fully ordered
-        (void)cudaLaunchKernelEx(&cfg, attention_long_kernel, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen, heads, nbasis,
-                                 nsplit);
+        (void)cudaLaunchKernelEx(&cfg, kernel, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen, heads, nbasis, nsplit, ring_off);
     }
     VPT_LAUNCH_CHECK();
     return VPT_OK;

@@ -31,6 +31,7 @@ void set_error(const char* fmt, ...) {
 #include "attention_bwd.cuh"
 #include "attention_full_bwd.cuh"
 #include "attention_long.cuh"
+#include "ring.cuh"
 #include "idm_bwd.cuh"
 #include "rl_bwd.cuh"
 #include "log_softmax_bwd.cuh"

@@ -464,6 +464,114 @@ class FrameLatents:
         return FrameLatents(self.x.to(device, non_blocking=non_blocking), self.stats.to(device, non_blocking=non_blocking), self.token)
 
 
+class RingState:
+    """The recurrent state of `MinecraftAgentPolicy` as a ring that a t = 1 forward (`act`, `v`, `get_output_for_observation`, `forward`,
+    `GraphedAct(memory="ring")`) updates in place, instead of building a new state from a copy of the old one.  Per layer the KV memory
+    K / V is bf16 (B, maxlen, h) and the state mask bool (B, maxlen); memory row j (oldest first) is at physical row (off + j) % maxlen,
+    where `off` is one device int32 shared by the layers.  A step writes its K / V rows at `off`, attends, and advances `off`: nothing else
+    of the memory moves.  The step's results are those of the same step from `to_pytree()`, bit for bit: the pytree path rounds its fp32
+    state to bf16 before the attention reads it, and every row it stores came out of a bf16 GEMM.
+
+    The forward returns the RingState it was given, updated: copy it out with `to_pytree()` first to keep the old state."""
+
+    def __init__(self, k, v, mask, off):
+        self.k, self.v, self.mask, self.off = k, v, mask, off  # per layer: bf16 (B, maxlen, h) x 2, bool (B, maxlen); int32 (1,)
+
+    @staticmethod
+    def _net(policy):
+        net = getattr(policy, "net", policy)
+        if isinstance(net, InverseActionNet):
+            raise TypeError("the IDM has no KV memory across calls: RingState is for MinecraftAgentPolicy / MinecraftPolicy")
+        if not isinstance(net, MinecraftPolicy):
+            raise TypeError(f"RingState: expected a MinecraftAgentPolicy or MinecraftPolicy, got {type(policy).__name__}")
+        if net.cfg.maxlen == 0 or net.cfg.mask_style != "clipped_causal":
+            raise ValueError("RingState needs a KV memory: attention_memory_size > timesteps with the clipped_causal mask")
+        return net
+
+    @classmethod
+    def zeros(cls, policy, B: int) -> "RingState":
+        """The state of `policy.initial_state(B)` (empty memory, every mask bit clear) on the policy's device."""
+        net = cls._net(policy)
+        cfg, dev = net.cfg, net.final_ln.weight.device
+        L, maxlen, h = cfg.n_layers, cfg.maxlen, cfg.hidsize
+        k = torch.zeros((L, B, maxlen, h), dtype=BF16, device=dev)
+        v = torch.zeros((L, B, maxlen, h), dtype=BF16, device=dev)
+        mask = torch.zeros((L, B, maxlen), dtype=torch.bool, device=dev)
+        return cls(list(k.unbind(0)), list(v.unbind(0)), list(mask.unbind(0)), torch.zeros((1,), dtype=torch.int32, device=dev))
+
+    @classmethod
+    def from_pytree(cls, policy, state) -> "RingState":
+        """A ring holding the reference-format state `state` (`initial_state` / a `state_out`: per layer (mask (B, 1, maxlen) or None,
+        (K, V) (B, maxlen, h))); fp32 K / V are rounded to bf16 by the kernel, and so exactly as, the pytree forward rounds them."""
+        cls._net(policy)
+        ring = cls.zeros(policy, state[0][1][0].shape[0])
+        ring.load_(state)
+        return ring
+
+    @property
+    def batch_size(self):
+        return self.k[0].shape[0]
+
+    def load_(self, state):
+        """Copy `state` (a pytree as in `from_pytree`, or a RingState of the same shape) into this ring, in place."""
+        L, (B, maxlen, h) = len(self.k), self.k[0].shape
+        if isinstance(state, RingState):
+            if len(state.k) != L or state.k[0].shape != self.k[0].shape:
+                raise ValueError(f"RingState.load_: a ring of {len(state.k)} x {tuple(state.k[0].shape)} into one of {L} x {(B, maxlen, h)}")
+            for dst, src in zip(self.k + self.v + self.mask + [self.off], state.k + state.v + state.mask + [state.off]):
+                dst.copy_(src)
+            return self
+        if len(state) != L:
+            raise ValueError(f"RingState.load_: a state of {len(state)} layers into a ring of {L}")
+        for l, (m, (K, V)) in enumerate(state):
+            if tuple(K.shape) != (B, maxlen, h) or V.shape != K.shape:
+                raise ValueError(f"RingState.load_: layer {l} K / V {tuple(K.shape)} / {tuple(V.shape)} != {(B, maxlen, h)}")
+            if K.dtype not in (F32, BF16) or V.dtype not in (F32, BF16):
+                raise TypeError(f"RingState.load_: K / V must be float32 or bfloat16 (got {K.dtype}, {V.dtype})")
+            if m is None:
+                self.mask[l].zero_()  # lib/masked_attention.py:75-76: None == all-False
+            else:
+                self.mask[l].copy_(m.reshape(B, maxlen))
+            if K.stride() == V.stride() and K.dtype == V.dtype:
+                ops.copy_rows2(K, V, 0, self.k[l], self.v[l], 0, maxlen)
+            else:
+                ops.copy_rows(K, 0, self.k[l], 0, maxlen)
+                ops.copy_rows(V, 0, self.v[l], 0, maxlen)
+        self.off.zero_()
+        return self
+
+    def to_pytree(self):
+        """The reference-format state, a new list[(mask bool (B, 1, maxlen), (K, V) fp32 (B, maxlen, h))] with the oldest row first; after
+        a step it is the pytree forward's `state_out`, bit for bit.  Reads `off` back to the host (synchronises)."""
+        B, maxlen, h = self.k[0].shape
+        off = int(self.off.item())
+        out = []
+        for k, v, m in zip(self.k, self.v, self.mask):
+            K = torch.empty((B, maxlen, h), dtype=F32, device=k.device)
+            V = torch.empty_like(K)
+            ops.copy_rows2(k, v, off, K, V, 0, maxlen - off)
+            ops.copy_rows2(k, v, 0, K, V, maxlen - off, off)
+            out.append((torch.cat([m[:, off:], m[:, :off]], 1).unsqueeze(1), (K, V)))
+        return out
+
+
+def _check_ring_call(net, img, state_in, differentiable: bool):
+    """Raises, before any launch, for a forward call a RingState cannot serve."""
+    RingState._net(net)
+    if net.precision != "bf16":
+        raise NotImplementedError("RingState runs in the bf16 mode only (set_precision('bf16'))")
+    if differentiable or net._tape is not None:
+        raise ValueError("RingState is for inference: the differentiable forward and the trainers take the pytree state")
+    B, t = img.shape[:2]
+    if t != 1:
+        raise ValueError(f"RingState takes one frame per call (t = 1, got t = {t}): a chunk's rows would overwrite memory that its "
+                         "earlier frames still attend to")
+    cfg = net.cfg
+    if len(state_in.k) != cfg.n_layers or tuple(state_in.k[0].shape) != (B, cfg.maxlen, cfg.hidsize):
+        raise ValueError(f"RingState of {len(state_in.k)} x {tuple(state_in.k[0].shape)} for a call of {cfg.n_layers} x "
+                         f"{(B, cfg.maxlen, cfg.hidsize)}")
+
+
 def _ob_input(ob):
     """The network input of an observation dict: the frames `ob["img"]` or the latents `ob["img_latent"]` (exactly one of them)."""
     if LATENT_KEY not in ob:
@@ -683,16 +791,24 @@ class MinecraftPolicy(nn.Module):
         return out, mr_out
 
     def _block(self, l, x, mr_x, first_u8, state, B, t, prep: _Prepared, last: bool):
-        """lib/util.py:193-211: x_hat = LN(x); y = x_hat + Proj(Attn(x_hat)); z = y + mlp1(relu(mlp0(LN(y))))."""
+        """lib/util.py:193-211: x_hat = LN(x); y = x_hat + Proj(Attn(x_hat)); z = y + mlp1(relu(mlp0(LN(y)))).
+        state: the layer's (mask, (K, V)), or a RingState (t = 1), updated in place (returns None for the state)."""
         cfg, L = self.cfg, prep.layers[l]
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
         causal = cfg.mask_style == "clipped_causal"
-        state_mask, (mem_k, mem_v) = state
+        ring = state if isinstance(state, RingState) else None
         xhat, _, _ = ops.affine_norm(x, mr_x, L["ln_g"], L["ln_b"], rows_per_group=1)
         T = maxlen + t
-        full_k = torch.empty((B, T, h), dtype=BF16, device=x.device)
-        full_v = torch.empty((B, T, h), dtype=BF16, device=x.device)
-        if maxlen > 0:
+        if ring is not None:  # K / V of the step only (`seg` the identity): ring_write stores them in the ring
+            full_k = torch.empty((B, t, h), dtype=BF16, device=x.device)
+            full_v = torch.empty((B, t, h), dtype=BF16, device=x.device)
+            seg = (t, t, 0)
+        else:
+            state_mask, (mem_k, mem_v) = state
+            full_k = torch.empty((B, T, h), dtype=BF16, device=x.device)
+            full_v = torch.empty((B, T, h), dtype=BF16, device=x.device)
+            seg = (t, T, maxlen)
+        if maxlen > 0 and ring is None:
             if mem_k.shape != (B, maxlen, h):
                 raise AssertionError(f"KV memory shape {tuple(mem_k.shape)} != {(B, maxlen, h)}")
             if mem_k.stride() == mem_v.stride() and mem_k.dtype == mem_v.dtype:
@@ -709,20 +825,27 @@ class MinecraftPolicy(nn.Module):
                 R = torch.empty((B * t, NBASIS * heads), dtype=F32, device=x.device)
                 dsts.append((3 * h, R, NBASIS * heads, False))
             Wc, _, bc = L["qkvr"]
-            ops.gemm(xhat, Wc, q, B * t, Wc.shape[0], h, S2=bc, seg=(t, T, maxlen), dsts=dsts)
+            ops.gemm(xhat, Wc, q, B * t, Wc.shape[0], h, S2=bc, seg=seg, dsts=dsts)
         else:  # hidsize not a multiple of the N tile: four launches
             q, _ = self._linear(xhat, L["q"], h)
-            self._linear(xhat, L["k"], h, out=full_k, seg=(t, T, maxlen), ld_out=h)
-            self._linear(xhat, L["v"], h, out=full_v, seg=(t, T, maxlen), ld_out=h)
+            self._linear(xhat, L["k"], h, out=full_k, seg=seg, ld_out=h)
+            self._linear(xhat, L["v"], h, out=full_v, seg=seg, ld_out=h)
             if causal:
                 R, _ = self._linear(xhat, L["r"], NBASIS * heads, out_dtype=F32)
-        smask_u8 = state_mask.contiguous().view(torch.uint8) if state_mask is not None else None
-        a = ops.attention(q, full_k, full_v, R, L["b_nd"], first_u8, smask_u8, B, t, maxlen, heads, causal=causal)
-        # new state (lib/xf.py:380-381: last `maxlen` rows of full; lib/masked_attention.py:86-92)
-        new_k = torch.empty((B, maxlen, h), dtype=F32, device=x.device)
-        new_v = torch.empty((B, maxlen, h), dtype=F32, device=x.device)
-        ops.copy_rows2(full_k, full_v, T - maxlen, new_k, new_v, 0, maxlen)
-        new_mask = ops.state_mask_update(smask_u8, first_u8, t, maxlen) if causal else state_mask
+        if ring is not None:
+            # the step's rows go to ring slot `off` first: it held memory key 0, which a t = 1 query does not see
+            ops.ring_write(full_k, full_v, ring.k[l], ring.v[l], ring.mask[l], ring.off, first_u8)
+            a = ops.attention_ring(q, ring.k[l], ring.v[l], R, L["b_nd"], first_u8, ring.mask[l], ring.off, heads)
+            new_state = None
+        else:
+            smask_u8 = state_mask.contiguous().view(torch.uint8) if state_mask is not None else None
+            a = ops.attention(q, full_k, full_v, R, L["b_nd"], first_u8, smask_u8, B, t, maxlen, heads, causal=causal)
+            # new state (lib/xf.py:380-381: last `maxlen` rows of full; lib/masked_attention.py:86-92)
+            new_k = torch.empty((B, maxlen, h), dtype=F32, device=x.device)
+            new_v = torch.empty((B, maxlen, h), dtype=F32, device=x.device)
+            ops.copy_rows2(full_k, full_v, T - maxlen, new_k, new_v, 0, maxlen)
+            new_mask = ops.state_mask_update(smask_u8, first_u8, t, maxlen) if causal else state_mask
+            new_state = (new_mask, (new_k, new_v))
         y, mr_y = self._linear(a, L["proj"], h, residual=xhat, want_stats=True)
         self._tap(f"recurrent_layer.blocks.{l}.attn", y)
         hmid, _ = self._linear(y, L["mlp0"], h * cfg.pointwise_ratio, mr=mr_y, relu=1)
@@ -733,7 +856,7 @@ class MinecraftPolicy(nn.Module):
         if self._tape is not None:  # (None for a block below the backward's lowest unit)
             self._tape["blocks"].append(dict(x=x, mr_x=mr_x, xhat=xhat, q=q, full_k=full_k, full_v=full_v, R=R, smask=smask_u8, a=a, y=y,
                                              mr_y=mr_y, hmid=hmid, z=z, mr_z=mr_z) if l >= self._tape["blocks_from"] else None)
-        return z, mr_z, (new_mask, (new_k, new_v))
+        return z, mr_z, new_state
 
     # -- cached CNN latents -----------------------------------------------------------------------------------
     def _cnn_params(self):
@@ -792,8 +915,11 @@ class MinecraftPolicy(nn.Module):
         frame_shape = (cfg.img_shape[0], cfg.img_shape[1], 3)
         if not latents:
             assert tuple(img.shape[2:]) == frame_shape, f"img shape {tuple(img.shape[2:])} != {frame_shape}"
-        assert len(state_in) == cfg.n_layers, \
-            f"Length of state {len(state_in)} did not match length of blocks {cfg.n_layers}"  # lib/util.py:117-119
+        if isinstance(state_in, RingState):
+            _check_ring_call(self, img, state_in, differentiable=False)
+        else:
+            assert len(state_in) == cfg.n_layers, \
+                f"Length of state {len(state_in)} did not match length of blocks {cfg.n_layers}"  # lib/util.py:117-119
         if self.precision == "fp32":
             if self._tape is not None:
                 raise NotImplementedError("the BC step runs in the bf16 mode only")
@@ -868,10 +994,14 @@ class MinecraftPolicy(nn.Module):
         if tape is not None:
             tape.update(x0=x, mr_x0=mr_x)
         # ---- transformer
-        state_out = []
+        ring = isinstance(state_in, RingState)
+        state_out = state_in if ring else []
         for l in range(cfg.n_layers):
-            x, mr_x, s = self._block(l, x, mr_x, first_u8, state_in[l], B, t, prep, last=(l == cfg.n_layers - 1))
-            state_out.append(s)
+            x, mr_x, s = self._block(l, x, mr_x, first_u8, state_in if ring else state_in[l], B, t, prep, last=(l == cfg.n_layers - 1))
+            if not ring:
+                state_out.append(s)
+        if ring:  # every layer has written its row at `off`: the next step's oldest row is one further on
+            ops.ring_advance(state_in.off, cfg.maxlen)
         # x is relu(recurrent output) here
         if self.use_lastlayer:
             z_last, mr_zl = x, mr_x
@@ -885,6 +1015,8 @@ class MinecraftPolicy(nn.Module):
         """lib/policy.py:193-218."""
         first = context["first"]
         img = _ob_input(ob)
+        if isinstance(state_in, RingState):
+            _check_ring_call(self, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             (latent,), state_out = _autograd_runner(self).run(img, first, state_in)
         else:
@@ -908,6 +1040,8 @@ class InverseActionNet(MinecraftPolicy):
         """lib/policy.py:374-392 -> ((pi_latent, None), state_out)."""
         first = context["first"]
         img = _ob_input(ob)
+        if isinstance(state_in, RingState):
+            _check_ring_call(self, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             (latent,), state_out = _autograd_runner(self).run(img, first, state_in)
         else:
@@ -1314,6 +1448,8 @@ class MinecraftAgentPolicy(_PolicyBase):
         else:
             mask = None
         img = _ob_input(obs)
+        if isinstance(state_in, RingState):
+            _check_ring_call(self.net, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
             pi_logits = OrderedDict(zip(self.head_specs, outs[:-1]))
@@ -1372,11 +1508,11 @@ class MinecraftAgentPolicy(_PolicyBase):
         ac = {k: v[:, 0] for k, v in ac.items()}
         return ac, state_out, result
 
-    def make_graphed_act(self, batch_size: int, pdl: bool = False):
+    def make_graphed_act(self, batch_size: int, pdl: bool = False, memory: str = "pytree"):
         """Rollout-latency path (agent.py:190-206, SURVEY f-1): returns a callable with the signature of `act` whose whole
         step (forward + heads + sampling + log-prob + KV-memory roll) is ONE captured CUDA graph replay (pdl: captured with
-        programmatic dependent launch between its kernels -- bit-identical)."""
-        return GraphedAct(self, batch_size, pdl=pdl)
+        programmatic dependent launch between its kernels -- bit-identical; memory: see `GraphedAct`)."""
+        return GraphedAct(self, batch_size, pdl=pdl, memory=memory)
 
     @torch.no_grad()
     def v(self, obs, first, state_in):
@@ -1405,6 +1541,8 @@ class InverseActionPolicy(_PolicyBase):
         else:
             mask = None
         img = _ob_input(obs)
+        if isinstance(state_in, RingState):
+            _check_ring_call(self.net, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
             return (OrderedDict(zip(self.head_specs, outs)), None, None), state_out
@@ -1429,26 +1567,39 @@ class GraphedAct:
 
     The recurrent state lives in static buffers owned by the graph; the state object returned by a call is a handle to
     them (valid until the next call).  Passing any other state (e.g. `policy.initial_state(B)` after an episode reset)
-    copies it in.  Sampling uses torch's graph-safe Philox generator, i.e. the same `rand_like` draws as eager mode."""
+    copies it in.  Sampling uses torch's graph-safe Philox generator, i.e. the same `rand_like` draws as eager mode.
 
-    def __init__(self, policy: "MinecraftAgentPolicy", batch_size: int, pdl: bool = False):
+    memory="pytree" (default): the static state is the reference's list of (mask, (K, V)) fp32 and each step ends by copying the new
+    state over it.  memory="ring": the static state is a `RingState` that the step updates in place (no copy of the memory; half its
+    bytes); a pytree or another RingState passed in is copied into it, and every call returns that RingState."""
+
+    def __init__(self, policy: "MinecraftAgentPolicy", batch_size: int, pdl: bool = False, memory: str = "pytree"):
+        if memory not in ("pytree", "ring"):
+            raise ValueError(f"GraphedAct: memory must be 'pytree' or 'ring' (got {memory!r})")
         self.policy = policy
         self.pdl = pdl
+        self.memory = memory
         cfg = policy.net.cfg
         dev = policy.net.final_ln.weight.device
         B, self.B = batch_size, batch_size
         H, W = cfg.img_shape[0], cfg.img_shape[1]
         self.img = torch.zeros((B, H, W, 3), dtype=torch.uint8, device=dev)
         self.first = torch.zeros((B,), dtype=torch.bool, device=dev)
-        self.state = [(torch.zeros((B, 1, cfg.maxlen), dtype=torch.bool, device=dev),
-                       (torch.zeros((B, cfg.maxlen, cfg.hidsize), dtype=F32, device=dev),
-                        torch.zeros((B, cfg.maxlen, cfg.hidsize), dtype=F32, device=dev))) for _ in range(cfg.n_layers)]
+        if memory == "ring":
+            self.state = RingState.zeros(policy, B)
+        else:
+            self.state = [(torch.zeros((B, 1, cfg.maxlen), dtype=torch.bool, device=dev),
+                           (torch.zeros((B, cfg.maxlen, cfg.hidsize), dtype=F32, device=dev),
+                            torch.zeros((B, cfg.maxlen, cfg.hidsize), dtype=F32, device=dev))) for _ in range(cfg.n_layers)]
         self._held = self._layouts()
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):  # warm-up outside capture (lazy function attributes, allocator pools)
             for _ in range(2):
                 policy.act({"img": self.img}, self.first, self.state)
+            if memory == "ring":  # the warm-up stepped the ring in place: back to the empty state
+                for buf in self.state.k + self.state.v + self.state.mask + [self.state.off]:
+                    buf.zero_()
         torch.cuda.current_stream(dev).wait_stream(side)
         self.graphs = {}
 
@@ -1467,10 +1618,11 @@ class GraphedAct:
         try:
             with torch.cuda.graph(g):
                 ac, st, res = self.policy.act({"img": self.img}, self.first, self.state, stochastic=stochastic, return_pd=True)
-                for (m_in, (k_in, v_in)), (m_out, (k_out, v_out)) in zip(self.state, st):  # roll the state inside the graph
-                    m_in.copy_(m_out)
-                    if k_in.shape[1] > 0:
-                        ops.copy_rows2(k_out, v_out, 0, k_in, v_in, 0, k_in.shape[1])  # K and V in one launch
+                if self.memory == "pytree":
+                    for (m_in, (k_in, v_in)), (m_out, (k_out, v_out)) in zip(self.state, st):  # roll the state inside the graph
+                        m_in.copy_(m_out)
+                        if k_in.shape[1] > 0:
+                            ops.copy_rows2(k_out, v_out, 0, k_in, v_in, 0, k_in.shape[1])  # K and V in one launch
         finally:
             nat.lib().vpt_set_pdl(0)
         self.graphs[stochastic] = (g, ac, res)
@@ -1482,7 +1634,9 @@ class GraphedAct:
             raise NotImplementedError("GraphedAct: taken_action is only supported by the eager act()")
         self.img.copy_(obs["img"])
         self.first.copy_(first)
-        if state_in is not self.state:
+        if state_in is not self.state and self.memory == "ring":
+            self.state.load_(state_in)
+        elif state_in is not self.state:
             for (m_in, (k_in, v_in)), (m, (k, v)) in zip(self.state, state_in):
                 if m is None:
                     m_in.zero_()  # lib/masked_attention.py:75-76: None == all-False
