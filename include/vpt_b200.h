@@ -305,6 +305,21 @@ int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr, const floa
                        int32_t maxlen, int32_t heads, int32_t nbasis, void* stream);
 int vpt_ring_advance(int32_t* ring_off, int32_t maxlen, void* stream);
 
+/* A step of some of the ring's E environments (policy.py RingState.rows, asynchronous rollouts).  Two optional device arrays:
+ *   rows    int32 [B]: batch row b of the step (knew, vnew, Q, R, first, out) is ring row rows[b] (Kr, Vr, smask); rows[b] = -1 marks an
+ *           inert padding row, which reads and writes no ring memory and whose attention output is zero.  The non-negative entries are
+ *           distinct.  NULL: batch row b is ring row b.
+ *   row_off int32 [E], each in [0, maxlen): key j of ring row r is at physical row (off + row_off[r] + j) % maxlen.  NULL: all zeros.
+ * vpt_ring_write_rows / vpt_attention_ring_rows are vpt_ring_write / vpt_attention_ring with these; with both NULL they are the same calls.
+ * vpt_ring_advance_rows row_off[rows[i]] = (row_off[rows[i]] + 1) % maxlen for every rows[i] >= 0, after the last layer of a step of
+ *                       some environments (`off` stays). */
+int vpt_ring_write_rows(const void* knew, const void* vnew, void* Kr, void* Vr, uint8_t* smask, const uint8_t* first, int64_t first_stride,
+                        const int32_t* ring_off, const int32_t* rows, const int32_t* row_off, int32_t B, int32_t maxlen, int32_t h, void* stream);
+int vpt_attention_ring_rows(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                            const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, const int32_t* rows,
+                            const int32_t* row_off, void* out, int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream);
+int vpt_ring_advance_rows(int32_t* row_off, const int32_t* rows, int32_t B, int32_t maxlen, void* stream);
+
 /* ----------------------------------------------------------------------------------------------------------
  * Action heads (lib/action_head.py:163-207)
  * -------------------------------------------------------------------------------------------------------- */

@@ -119,6 +119,9 @@ SIGNATURES = {
     "vpt_ring_write": (_I, [_P, _P, _P, _P, _P, _P, _L, _P, _I, _I, _I, _P]),
     "vpt_attention_ring": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _I, _I, _I, _I, _P]),
     "vpt_ring_advance": (_I, [_P, _I, _P]),
+    "vpt_ring_write_rows": (_I, [_P, _P, _P, _P, _P, _P, _L, _P, _P, _P, _I, _I, _I, _P]),
+    "vpt_attention_ring_rows": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "vpt_ring_advance_rows": (_I, [_P, _P, _I, _I, _P]),
     "vpt_log_softmax": (_I, [_P, _L, _I, _I, _P, _L, _P]),
     "vpt_gumbel_argmax": (_I, [_P, _P, _P, _L, _I, _P]),
     "vpt_gather_logprob": (_I, [_P, _P, _P, _L, _I, _I, _P]),

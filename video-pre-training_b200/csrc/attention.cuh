@@ -50,6 +50,25 @@ __device__ __forceinline__ void load_tile_64x128(__nv_bfloat16* dst, const __nv_
 // (outside the t = 1 band).  Only the row addresses change: the key order and tiling are those of the linear layout, so are the bits.
 __device__ __forceinline__ int ring_row(int row, int off, int maxlen) { return (off + row) % maxlen; }
 
+// A step of some of the ring's environments (vpt_attention_ring_rows) adds two optional device arrays: `rows` int32 [B] maps batch row b
+// (Q, R, first, out) to ring row rows[b] (K, V, smask), rows[b] < 0 marking an inert padding row, and `row_off` int32 [E] adds a per-row
+// offset: key j of ring row r is at physical row (off + row_off[r] + j) % maxlen.  Null pointers: ring row b, offset `off`.
+// The ring row and offset of batch row b, or -1 for an inert row (RING only).
+__device__ __forceinline__ int ring_row_of(int b, const int* __restrict__ rows, const int* __restrict__ ring_off, const int* __restrict__ row_off,
+                                           int maxlen, int& off) {
+    const int r = rows ? rows[b] : b;
+    if (r >= 0) off = row_off ? (ring_off[0] + row_off[r]) % maxlen : ring_off[0];
+    return r;
+}
+
+// the output rows [q0, min(q0 + 64, t)) of one head of batch row b set to zero (an inert row of a ring step: no key is read)
+__device__ __forceinline__ void store_zero_rows(__nv_bfloat16* out, int b, int t, int q0, int h, int head) {
+    for (int i = threadIdx.x; i < kAttBQ * (kAttD / 8); i += kAttThreads) {
+        const int q = q0 + i / (kAttD / 8);
+        if (q < t) *reinterpret_cast<uint4*>(out + ((long long)b * t + q) * h + head * kAttD + (i % (kAttD / 8)) * 8) = make_uint4(0, 0, 0, 0);
+    }
+}
+
 // load_tile_64x128 for a ring: memory-coordinate rows [row0, row0+64), zero beyond rows_total (tiles may wrap)
 __device__ __forceinline__ void load_tile_64x128_ring(__nv_bfloat16* dst, const __nv_bfloat16* src, long long ld, int row0, int rows_total,
                                                       int col0, int off, int maxlen) {
@@ -62,13 +81,13 @@ __device__ __forceinline__ void load_tile_64x128_ring(__nv_bfloat16* dst, const 
     }
 }
 
-// RING: K / V / smask in the ring layout above, `off` read from ring_off[0] on the device (t = 1, causal)
+// RING: K / V / smask in the ring layout above, `off` read from ring_off[0] on the device, `rows` / `row_off` optional (t = 1, causal)
 template <bool RING>
 __global__ void __launch_bounds__(kAttThreads) attention_kernel(
     const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __restrict__ Kf, const __nv_bfloat16* __restrict__ Vf,
     const float* __restrict__ R, long long ld_r, const float* __restrict__ b_nd, const uint8_t* __restrict__ first,
     long long first_stride, const uint8_t* __restrict__ smask, __nv_bfloat16* __restrict__ out, int t, int maxlen, int heads,
-    int nbasis, int causal, const int* __restrict__ ring_off) {
+    int nbasis, int causal, const int* __restrict__ ring_off, const int* __restrict__ rows, const int* __restrict__ row_off) {
     pdl_sync();
     extern __shared__ __align__(16) uint8_t att_smem[];
     __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(att_smem);
@@ -84,16 +103,21 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
     const int T = maxlen + t;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
     const __nv_bfloat16* Qb = Q + (long long)b * t * h;
-    const int off = RING ? ring_off[0] : 0;
+    int off = 0;
+    const int rk = RING ? ring_row_of(b, rows, ring_off, row_off, maxlen, off) : b;  // row of K / V / smask
+    if (RING && rk < 0) {  // inert padding row (uniform over the CTA)
+        store_zero_rows(out, b, t, q0, h, head);
+        return;
+    }
     const long long kv_rows = RING ? maxlen : T;  // rows per batch row of K / V
-    const __nv_bfloat16* Kb = Kf + (long long)b * kv_rows * h;
-    const __nv_bfloat16* Vb = Vf + (long long)b * kv_rows * h;
+    const __nv_bfloat16* Kb = Kf + (long long)rk * kv_rows * h;
+    const __nv_bfloat16* Vb = Vf + (long long)rk * kv_rows * h;
 
     load_tile_64x128(Qs, Qb, h, q0, t, head * kAttD);
     if (causal && maxlen > 0) {
         const bool mem_ok = (first[(long long)b * first_stride] == 0) && (smask != nullptr);
         for (int j = threadIdx.x; j < maxlen; j += kAttThreads)
-            Ms[j] = mem_ok ? smask[(long long)b * maxlen + (RING ? ring_row(j, off, maxlen) : j)] : 0;
+            Ms[j] = mem_ok ? smask[(long long)rk * maxlen + (RING ? ring_row(j, off, maxlen) : j)] : 0;
         for (int i = threadIdx.x; i < nbasis * maxlen; i += kAttThreads) Bs[i] = __ldg(b_nd + i);
         for (int i = threadIdx.x; i < kAttBQ * nbasis; i += kAttThreads) {
             const int r = i / nbasis, n = i % nbasis;
@@ -253,7 +277,7 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
 // attention_long.cuh: the causal forward for a KV memory whose bias table does not fit this kernel's shared memory
 int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
                        const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
-                       int nbasis, const int* ring_off, cudaStream_t stream);
+                       int nbasis, const int* ring_off, const int* rows, const int* row_off, cudaStream_t stream);
 
 // shared memory of attention_kernel for a causal band of `maxlen` keys with `nb` basis rows (nb = 0: mask "none")
 inline size_t attention_smem(int maxlen, int nb) {
@@ -276,7 +300,7 @@ extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, cons
     if (smem > 227 * 1024) {  // only a causal band can be this long (mask 'none' has no memory): tile it over keys
         return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf),
                                   reinterpret_cast<const __nv_bfloat16*>(Vf), R, ld_r, b_nd, first, first_stride, smask,
-                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, nullptr, (cudaStream_t)stream);
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, nullptr, nullptr, nullptr, (cudaStream_t)stream);
     }
     static size_t attr = 0;
     if (smem > attr) {
@@ -286,23 +310,22 @@ extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, cons
     dim3 grid((t + kAttBQ - 1) / kAttBQ, heads, B);
     launch_k(attention_kernel<false>, dim3(grid), dim3(kAttThreads), smem, (cudaStream_t)stream, 
         reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf), reinterpret_cast<const __nv_bfloat16*>(Vf), R,
-        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), t, maxlen, heads, nb, causal, (const int*)nullptr);
+        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), t, maxlen, heads, nb, causal, (const int*)nullptr,
+        (const int*)nullptr, (const int*)nullptr);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
 }
 
-extern "C" int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
-                                  const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, void* out, int32_t B,
-                                  int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
-    using namespace vpt;
-    VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
-              "vpt_attention_ring: bad arguments");
-    VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring: grid too large");
+namespace vpt {
+
+int attention_ring(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
+                   int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, const int32_t* rows, const int32_t* row_off, void* out,
+                   int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
     const size_t smem = attention_smem(maxlen, nbasis);
     if (smem > 227 * 1024) {
         return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kr),
                                   reinterpret_cast<const __nv_bfloat16*>(Vr), R, ld_r, b_nd, first, first_stride, smask,
-                                  reinterpret_cast<__nv_bfloat16*>(out), B, 1, maxlen, heads, nbasis, ring_off, (cudaStream_t)stream);
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, 1, maxlen, heads, nbasis, ring_off, rows, row_off, (cudaStream_t)stream);
     }
     static size_t attr = 0;
     if (smem > attr) {
@@ -311,7 +334,30 @@ extern "C" int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr,
     }
     launch_k(attention_kernel<true>, dim3(1, heads, B), dim3(kAttThreads), smem, (cudaStream_t)stream,
         reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kr), reinterpret_cast<const __nv_bfloat16*>(Vr), R,
-        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), 1, maxlen, heads, nbasis, 1, (const int*)ring_off);
+        ld_r, b_nd, first, first_stride, smask, reinterpret_cast<__nv_bfloat16*>(out), 1, maxlen, heads, nbasis, 1, (const int*)ring_off,
+        (const int*)rows, (const int*)row_off);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
+}
+
+}  // namespace vpt
+
+extern "C" int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                                  const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, void* out, int32_t B,
+                                  int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
+              "vpt_attention_ring: bad arguments");
+    VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring: grid too large");
+    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, nullptr, nullptr, out, B, maxlen, heads, nbasis, stream);
+}
+
+extern "C" int vpt_attention_ring_rows(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                                       const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, const int32_t* rows,
+                                       const int32_t* row_off, void* out, int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
+              "vpt_attention_ring_rows: bad arguments");
+    VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring_rows: grid too large");
+    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, rows, row_off, out, B, maxlen, heads, nbasis, stream);
 }

@@ -31,13 +31,14 @@ constexpr int kAlPo = kAttD + 4;                 // fp32 pitch of the partial ou
 constexpr int kAlKK = 64;                        // key offsets (rows kernel) / query offsets (keys, mem kernels) per staged tile
 constexpr int kAlStage = kAlKK + kAbRows - 1;    // rows staged per tile: the tile's span over the CTA's 16 queries / keys
 
-// RING: K / V / smask in the ring layout of attention.cuh (vpt_attention_ring), `off` read from ring_off[0] on the device
+// RING: K / V / smask in the ring layout of attention.cuh (vpt_attention_ring), `off` read from ring_off[0] on the device, `rows` /
+// `row_off` optional (vpt_attention_ring_rows)
 template <bool RING>
 __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
     const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __restrict__ Kf, const __nv_bfloat16* __restrict__ Vf,
     const float* __restrict__ R, long long ld_r, const float* __restrict__ b_nd, const uint8_t* __restrict__ first,
     long long first_stride, const uint8_t* __restrict__ smask, __nv_bfloat16* __restrict__ out, int t, int maxlen, int heads,
-    int nbasis, int nsplit, const int* __restrict__ ring_off) {
+    int nbasis, int nsplit, const int* __restrict__ ring_off, const int* __restrict__ rows, const int* __restrict__ row_off) {
     pdl_sync();
     extern __shared__ __align__(16) uint8_t al_smem[];
     __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(al_smem);
@@ -52,10 +53,15 @@ __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
     const int h = heads * kAttD;
     const int T = maxlen + t;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
-    const int off = RING ? ring_off[0] : 0;
+    int off = 0;
+    const int rk = RING ? ring_row_of(b, rows, ring_off, row_off, maxlen, off) : b;  // row of K / V / smask
+    if (RING && rk < 0) {  // inert padding row: every CTA of the cluster shares b, so all leave before the first cluster barrier
+        if (split == 0) store_zero_rows(out, b, t, q0, h, head);
+        return;
+    }
     const long long kv_rows = RING ? maxlen : T;  // rows per batch row of K / V
-    const __nv_bfloat16* Kb = Kf + (long long)b * kv_rows * h;
-    const __nv_bfloat16* Vb = Vf + (long long)b * kv_rows * h;
+    const __nv_bfloat16* Kb = Kf + (long long)rk * kv_rows * h;
+    const __nv_bfloat16* Vb = Vf + (long long)rk * kv_rows * h;
     const bool mem_ok = (first[(long long)b * first_stride] == 0) && (smask != nullptr);
 
     load_tile_64x128(Qs, Q + (long long)b * t * h, h, q0, t, head * kAttD);
@@ -108,7 +114,7 @@ __global__ void __launch_bounds__(kAttThreads) attention_long_kernel(
         }
         if (threadIdx.x < kAttBK) {
             const int j = kb0 + threadIdx.x;
-            Ms[threadIdx.x] = (j >= maxlen) ? 1 : (mem_ok && smask[(long long)b * maxlen + (RING ? ring_row(j, off, maxlen) : j)] != 0);
+            Ms[threadIdx.x] = (j >= maxlen) ? 1 : (mem_ok && smask[(long long)rk * maxlen + (RING ? ring_row(j, off, maxlen) : j)] != 0);
         }
         cp_async_wait_all();
         __syncthreads();
@@ -546,7 +552,7 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_mem_long_kernel(const __n
 // ---------------------------------------------------------------------------------------------------------------------------------
 int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
                        const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
-                       int nbasis, const int* ring_off, cudaStream_t stream) {
+                       int nbasis, const int* ring_off, const int* rows, const int* row_off, cudaStream_t stream) {
     VPT_CHECK(nbasis <= kAlNb, "vpt_attention: nbasis=%d > %d", nbasis, kAlNb);
     const size_t smem = (size_t)(kAttBQ + 2 * kAttBK) * kAttPitch * 2 + (size_t)(kAlNb * kAlDist + 2 * kAttBQ) * 4 + kAttBK;
     const bool ring = ring_off != nullptr;
@@ -564,7 +570,7 @@ int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __
     dim3 grid(nqb * nsplit, heads, B);
     if (nsplit == 1) {
         launch_k(kernel, grid, dim3(kAttThreads), smem, stream, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen, heads, nbasis, 1,
-                 ring_off);
+                 ring_off, rows, row_off);
     } else {
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
@@ -579,7 +585,8 @@ int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;  // launched without PDL: pdl_sync() is then a no-op and the launch fully ordered
-        (void)cudaLaunchKernelEx(&cfg, kernel, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen, heads, nbasis, nsplit, ring_off);
+        (void)cudaLaunchKernelEx(&cfg, kernel, Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, t, maxlen, heads, nbasis, nsplit, ring_off,
+                                 rows, row_off);
     }
     VPT_LAUNCH_CHECK();
     return VPT_OK;

@@ -548,7 +548,7 @@ from .ops_dist import (head_entropy, head_entropy_bwd, head_kl, head_kl_bwd,  # 
                        rl_head_bwd_ent)
 from .ops_bptt import attention_bwd_state  # noqa: E402,F401  (gradients through the KV memory, csrc/attention_bwd.cuh)
 from .ops_pixel import conv3d_t5_dimg, firstconv_dimg  # noqa: E402,F401  (image gradients, csrc/firstconv_bwd.cuh, csrc/idm_bwd.cuh)
-from .ops_ring import attention_ring, ring_advance, ring_write  # noqa: E402,F401  (the KV memory as a ring, csrc/ring.cuh)
+from .ops_ring import attention_ring, ring_advance, ring_advance_rows, ring_write  # noqa: E402,F401  (the KV memory as a ring, csrc/ring.cuh)
 
 
 # ---- on-device action codec (csrc/codec.cuh) -----------------------------------------------------------------------------

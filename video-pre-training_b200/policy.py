@@ -472,10 +472,16 @@ class RingState:
     of the memory moves.  The step's results are those of the same step from `to_pytree()`, bit for bit: the pytree path rounds its fp32
     state to bf16 before the attention reads it, and every row it stores came out of a bf16 GEMM.
 
-    The forward returns the RingState it was given, updated: copy it out with `to_pytree()` first to keep the old state."""
+    The forward returns the RingState it was given, updated: copy it out with `to_pytree()` first to keep the old state.
 
-    def __init__(self, k, v, mask, off):
-        self.k, self.v, self.mask, self.off = k, v, mask, off  # per layer: bf16 (B, maxlen, h) x 2, bool (B, maxlen); int32 (1,)
+    Asynchronous rollouts step some of the ring's environments at a time through a view, `ring.rows(idx)` (`RingRows`).  They need one
+    offset per environment: `row_off`, None (all zeros) until the first call that needs it allocates a device int32 (E,); memory row j of
+    environment e is then at physical row (off + row_off[e] + j) % maxlen.  A step of the whole ring advances `off`, a step of a view
+    advances `row_off` of the rows it stepped."""
+
+    def __init__(self, k, v, mask, off, row_off=None):
+        self.k, self.v, self.mask, self.off = k, v, mask, off  # per layer: bf16 (E, maxlen, h) x 2, bool (E, maxlen); int32 (1,)
+        self.row_off = row_off  # None or int32 (E,), each in [0, maxlen)
 
     @staticmethod
     def _net(policy):
@@ -512,14 +518,43 @@ class RingState:
     def batch_size(self):
         return self.k[0].shape[0]
 
+    def _alloc_row_off(self):
+        if self.row_off is None:
+            self.row_off = torch.zeros((self.batch_size,), dtype=torch.int32, device=self.off.device)
+        return self.row_off
+
+    def rows(self, idx) -> "RingRows":
+        """A view of the environments `idx` (a 1-D integer sequence, CPU or CUDA tensor) for a t = 1 step of those only: row i of the
+        call's obs and `first` is environment idx[i]'s next frame, and -1 marks an inert padding row.  Validated here, on the host (a CUDA
+        `idx` is copied back once); raises ValueError for an entry outside [-1, E) or an environment listed twice."""
+        host = idx.detach().to("cpu") if torch.is_tensor(idx) else torch.as_tensor(idx)
+        if host.dim() != 1 or host.numel() == 0 or host.dtype.is_floating_point or host.dtype.is_complex or host.dtype == torch.bool:
+            raise ValueError(f"RingState.rows: idx must be a non-empty 1-D integer sequence (got {host.dtype} {tuple(host.shape)})")
+        E = self.batch_size
+        envs = host.tolist()
+        bad = [e for e in envs if not -1 <= e < E]
+        if bad:
+            raise ValueError(f"RingState.rows: rows {bad} are outside the ring's {E} environments (or -1 for padding)")
+        real = [e for e in envs if e >= 0]
+        if len(set(real)) != len(real):
+            raise ValueError(f"RingState.rows: an environment is listed twice in {envs}")
+        return RingRows(self, torch.tensor(envs, dtype=torch.int32).to(self.off.device, non_blocking=True), envs)
+
     def load_(self, state):
-        """Copy `state` (a pytree as in `from_pytree`, or a RingState of the same shape) into this ring, in place."""
+        """Copy `state` (a pytree as in `from_pytree`, or a RingState of the same shape) into this ring, in place.  A pytree is written at
+        rotation 0 (`row_off` zeroed); a ring's `row_off` is copied."""
         L, (B, maxlen, h) = len(self.k), self.k[0].shape
+        if isinstance(state, RingRows):
+            raise ValueError("RingState.load_: a view of a ring; load its `to_pytree()`, or use `view.load_` to write into a view")
         if isinstance(state, RingState):
             if len(state.k) != L or state.k[0].shape != self.k[0].shape:
                 raise ValueError(f"RingState.load_: a ring of {len(state.k)} x {tuple(state.k[0].shape)} into one of {L} x {(B, maxlen, h)}")
             for dst, src in zip(self.k + self.v + self.mask + [self.off], state.k + state.v + state.mask + [state.off]):
                 dst.copy_(src)
+            if state.row_off is not None:
+                self._alloc_row_off().copy_(state.row_off)
+            elif self.row_off is not None:
+                self.row_off.zero_()
             return self
         if len(state) != L:
             raise ValueError(f"RingState.load_: a state of {len(state)} layers into a ring of {L}")
@@ -538,12 +573,30 @@ class RingState:
                 ops.copy_rows(K, 0, self.k[l], 0, maxlen)
                 ops.copy_rows(V, 0, self.v[l], 0, maxlen)
         self.off.zero_()
+        if self.row_off is not None:
+            self.row_off.zero_()
         return self
+
+    def _gather(self, sel):
+        """The reference-format state of the ring rows `sel` (a device int64 vector), each rotated by its own offset (bf16 -> fp32 is exact)."""
+        maxlen, h = self.k[0].shape[1:]
+        shift = self.off if self.row_off is None else self.off + self.row_off[sel]
+        phys = ((shift.long()[:, None] + torch.arange(maxlen, device=sel.device)) % maxlen).expand(sel.numel(), maxlen)
+        idx = phys[:, :, None].expand(-1, -1, h)
+        out = []
+        for k, v, m in zip(self.k, self.v, self.mask):
+            K = k.index_select(0, sel).gather(1, idx).float()
+            V = v.index_select(0, sel).gather(1, idx).float()
+            out.append((m.index_select(0, sel).gather(1, phys).unsqueeze(1), (K, V)))
+        return out
 
     def to_pytree(self):
         """The reference-format state, a new list[(mask bool (B, 1, maxlen), (K, V) fp32 (B, maxlen, h))] with the oldest row first; after
-        a step it is the pytree forward's `state_out`, bit for bit.  Reads `off` back to the host (synchronises)."""
+        a step it is the pytree forward's `state_out`, bit for bit.  Reads `off` back to the host (synchronises) unless `row_off` is
+        allocated: each environment is then rotated by its own offset on the device."""
         B, maxlen, h = self.k[0].shape
+        if self.row_off is not None:
+            return self._gather(torch.arange(B, device=self.off.device))
         off = int(self.off.item())
         out = []
         for k, v, m in zip(self.k, self.v, self.mask):
@@ -555,8 +608,66 @@ class RingState:
         return out
 
 
+class RingRows:
+    """A view of some environments of a `RingState` (`ring.rows(idx)`), accepted wherever a RingState is: a t = 1 step of environments
+    idx[0], idx[1], ... (row i of obs and `first`), which updates their memory and their `row_off` in place and returns the same view.
+    Every other environment is untouched.  A -1 entry is an inert padding row: it reads and writes no ring memory, its attention output
+    is zero, and its outputs (actions, log-probs, vpred, pd) are finite and meaningless.
+
+    `idx` is a device int32 copy of the environments (`envs`, host ints); `GraphedAct(..., envs=E)` replays one graph over its own views."""
+
+    def __init__(self, ring: RingState, idx, envs):
+        self.ring, self.idx, self.envs = ring, idx, envs
+
+    def __len__(self):
+        return len(self.envs)
+
+    @property
+    def batch_size(self):
+        return len(self.envs)
+
+    def _sel(self, what):
+        if any(e < 0 for e in self.envs):
+            raise ValueError(f"RingRows.{what}: the view has inert (-1) rows")
+        return self.idx.long()
+
+    def to_pytree(self):
+        """The listed environments' reference-format state, in `idx` order (as `RingState.to_pytree`; no -1 entry)."""
+        return self.ring._gather(self._sel("to_pytree"))
+
+    def load_(self, state):
+        """Write `state`, a reference-format state of len(idx) rows, into the listed environments only (no -1 entry).  Each is stored at
+        rotation 0 with row_off[e] = -off mod maxlen; fp32 K / V are rounded to bf16 as the pytree forward rounds them."""
+        ring = self.ring
+        sel = self._sel("load_")
+        L, (E, maxlen, h) = len(ring.k), ring.k[0].shape
+        n = len(self)
+        if isinstance(state, (RingState, RingRows)):
+            raise ValueError("RingRows.load_ takes a reference-format state (a ring's `to_pytree()`)")
+        if len(state) != L:
+            raise ValueError(f"RingRows.load_: a state of {len(state)} layers into a ring of {L}")
+        for l, (m, (K, V)) in enumerate(state):
+            if tuple(K.shape) != (n, maxlen, h) or V.shape != K.shape:
+                raise ValueError(f"RingRows.load_: layer {l} K / V {tuple(K.shape)} / {tuple(V.shape)} != {(n, maxlen, h)}")
+            if K.dtype not in (F32, BF16) or V.dtype not in (F32, BF16):
+                raise TypeError(f"RingRows.load_: K / V must be float32 or bfloat16 (got {K.dtype}, {V.dtype})")
+        for l, (m, (K, V)) in enumerate(state):
+            ring.k[l].index_copy_(0, sel, K.to(device=sel.device, dtype=BF16))
+            ring.v[l].index_copy_(0, sel, V.to(device=sel.device, dtype=BF16))
+            if m is None:
+                ring.mask[l].index_fill_(0, sel, False)  # lib/masked_attention.py:75-76: None == all-False
+            else:
+                ring.mask[l].index_copy_(0, sel, m.reshape(n, maxlen).to(device=sel.device, dtype=torch.bool))
+        rot0 = ((maxlen - ring.off) % maxlen).to(torch.int32)  # off + row_off[e] = 0 (mod maxlen): memory row j at physical row j
+        ring._alloc_row_off().index_copy_(0, sel, rot0.expand(n).contiguous())
+        return self
+
+
+_RING_STATES = (RingState, RingRows)
+
+
 def _check_ring_call(net, img, state_in, differentiable: bool):
-    """Raises, before any launch, for a forward call a RingState cannot serve."""
+    """Raises, before any launch, for a forward call a RingState (or a view of one) cannot serve."""
     RingState._net(net)
     if net.precision != "bf16":
         raise NotImplementedError("RingState runs in the bf16 mode only (set_precision('bf16'))")
@@ -566,10 +677,16 @@ def _check_ring_call(net, img, state_in, differentiable: bool):
     if t != 1:
         raise ValueError(f"RingState takes one frame per call (t = 1, got t = {t}): a chunk's rows would overwrite memory that its "
                          "earlier frames still attend to")
+    ring, E = state_in, B
+    if isinstance(state_in, RingRows):
+        if len(state_in) != B:
+            raise ValueError(f"a view of {len(state_in)} ring rows for a call of B = {B}")
+        ring = state_in.ring
+        E = ring.batch_size
     cfg = net.cfg
-    if len(state_in.k) != cfg.n_layers or tuple(state_in.k[0].shape) != (B, cfg.maxlen, cfg.hidsize):
-        raise ValueError(f"RingState of {len(state_in.k)} x {tuple(state_in.k[0].shape)} for a call of {cfg.n_layers} x "
-                         f"{(B, cfg.maxlen, cfg.hidsize)}")
+    if len(ring.k) != cfg.n_layers or tuple(ring.k[0].shape) != (E, cfg.maxlen, cfg.hidsize):
+        raise ValueError(f"RingState of {len(ring.k)} x {tuple(ring.k[0].shape)} for a call of {cfg.n_layers} x "
+                         f"{(E, cfg.maxlen, cfg.hidsize)}")
 
 
 def _ob_input(ob):
@@ -792,11 +909,11 @@ class MinecraftPolicy(nn.Module):
 
     def _block(self, l, x, mr_x, first_u8, state, B, t, prep: _Prepared, last: bool):
         """lib/util.py:193-211: x_hat = LN(x); y = x_hat + Proj(Attn(x_hat)); z = y + mlp1(relu(mlp0(LN(y)))).
-        state: the layer's (mask, (K, V)), or a RingState (t = 1), updated in place (returns None for the state)."""
+        state: the layer's (mask, (K, V)), or a RingState or RingRows (t = 1), updated in place (returns None for the state)."""
         cfg, L = self.cfg, prep.layers[l]
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
         causal = cfg.mask_style == "clipped_causal"
-        ring = state if isinstance(state, RingState) else None
+        ring = state if isinstance(state, _RING_STATES) else None
         xhat, _, _ = ops.affine_norm(x, mr_x, L["ln_g"], L["ln_b"], rows_per_group=1)
         T = maxlen + t
         if ring is not None:  # K / V of the step only (`seg` the identity): ring_write stores them in the ring
@@ -833,9 +950,15 @@ class MinecraftPolicy(nn.Module):
             if causal:
                 R, _ = self._linear(xhat, L["r"], NBASIS * heads, out_dtype=F32)
         if ring is not None:
-            # the step's rows go to ring slot `off` first: it held memory key 0, which a t = 1 query does not see
-            ops.ring_write(full_k, full_v, ring.k[l], ring.v[l], ring.mask[l], ring.off, first_u8)
-            a = ops.attention_ring(q, ring.k[l], ring.v[l], R, L["b_nd"], first_u8, ring.mask[l], ring.off, heads)
+            # a view steps some environments: batch row b is ring row idx[b] (-1: an inert row)
+            rr, rows = (ring.ring, ring.idx) if isinstance(ring, RingRows) else (ring, None)
+            # the step's rows go to their ring slot first: it held memory key 0, which a t = 1 query does not see
+            if rr.row_off is None:  # every row at `off`
+                ops.ring_write(full_k, full_v, rr.k[l], rr.v[l], rr.mask[l], rr.off, first_u8)
+                a = ops.attention_ring(q, rr.k[l], rr.v[l], R, L["b_nd"], first_u8, rr.mask[l], rr.off, heads)
+            else:
+                ops.ring_write(full_k, full_v, rr.k[l], rr.v[l], rr.mask[l], rr.off, first_u8, rows=rows, row_off=rr.row_off)
+                a = ops.attention_ring(q, rr.k[l], rr.v[l], R, L["b_nd"], first_u8, rr.mask[l], rr.off, heads, rows=rows, row_off=rr.row_off)
             new_state = None
         else:
             smask_u8 = state_mask.contiguous().view(torch.uint8) if state_mask is not None else None
@@ -915,8 +1038,10 @@ class MinecraftPolicy(nn.Module):
         frame_shape = (cfg.img_shape[0], cfg.img_shape[1], 3)
         if not latents:
             assert tuple(img.shape[2:]) == frame_shape, f"img shape {tuple(img.shape[2:])} != {frame_shape}"
-        if isinstance(state_in, RingState):
+        if isinstance(state_in, _RING_STATES):
             _check_ring_call(self, img, state_in, differentiable=False)
+            if isinstance(state_in, RingRows):
+                state_in.ring._alloc_row_off()  # (the first step of a view: every row's offset starts at 0)
         else:
             assert len(state_in) == cfg.n_layers, \
                 f"Length of state {len(state_in)} did not match length of blocks {cfg.n_layers}"  # lib/util.py:117-119
@@ -994,13 +1119,16 @@ class MinecraftPolicy(nn.Module):
         if tape is not None:
             tape.update(x0=x, mr_x0=mr_x)
         # ---- transformer
-        ring = isinstance(state_in, RingState)
+        ring = isinstance(state_in, _RING_STATES)
         state_out = state_in if ring else []
         for l in range(cfg.n_layers):
             x, mr_x, s = self._block(l, x, mr_x, first_u8, state_in if ring else state_in[l], B, t, prep, last=(l == cfg.n_layers - 1))
             if not ring:
                 state_out.append(s)
-        if ring:  # every layer has written its row at `off`: the next step's oldest row is one further on
+        # every layer has written its row at its slot: the next step's oldest row is one further on
+        if isinstance(state_in, RingRows):
+            ops.ring_advance_rows(state_in.ring.row_off, state_in.idx, cfg.maxlen)
+        elif ring:
             ops.ring_advance(state_in.off, cfg.maxlen)
         # x is relu(recurrent output) here
         if self.use_lastlayer:
@@ -1015,7 +1143,7 @@ class MinecraftPolicy(nn.Module):
         """lib/policy.py:193-218."""
         first = context["first"]
         img = _ob_input(ob)
-        if isinstance(state_in, RingState):
+        if isinstance(state_in, _RING_STATES):
             _check_ring_call(self, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             (latent,), state_out = _autograd_runner(self).run(img, first, state_in)
@@ -1040,7 +1168,7 @@ class InverseActionNet(MinecraftPolicy):
         """lib/policy.py:374-392 -> ((pi_latent, None), state_out)."""
         first = context["first"]
         img = _ob_input(ob)
-        if isinstance(state_in, RingState):
+        if isinstance(state_in, _RING_STATES):
             _check_ring_call(self, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             (latent,), state_out = _autograd_runner(self).run(img, first, state_in)
@@ -1448,7 +1576,7 @@ class MinecraftAgentPolicy(_PolicyBase):
         else:
             mask = None
         img = _ob_input(obs)
-        if isinstance(state_in, RingState):
+        if isinstance(state_in, _RING_STATES):
             _check_ring_call(self.net, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
@@ -1508,11 +1636,11 @@ class MinecraftAgentPolicy(_PolicyBase):
         ac = {k: v[:, 0] for k, v in ac.items()}
         return ac, state_out, result
 
-    def make_graphed_act(self, batch_size: int, pdl: bool = False, memory: str = "pytree"):
+    def make_graphed_act(self, batch_size: int, pdl: bool = False, memory: str = "pytree", envs: Optional[int] = None):
         """Rollout-latency path (agent.py:190-206, SURVEY f-1): returns a callable with the signature of `act` whose whole
         step (forward + heads + sampling + log-prob + KV-memory roll) is ONE captured CUDA graph replay (pdl: captured with
-        programmatic dependent launch between its kernels -- bit-identical; memory: see `GraphedAct`)."""
-        return GraphedAct(self, batch_size, pdl=pdl, memory=memory)
+        programmatic dependent launch between its kernels -- bit-identical; memory, envs: see `GraphedAct`)."""
+        return GraphedAct(self, batch_size, pdl=pdl, memory=memory, envs=envs)
 
     @torch.no_grad()
     def v(self, obs, first, state_in):
@@ -1541,7 +1669,7 @@ class InverseActionPolicy(_PolicyBase):
         else:
             mask = None
         img = _ob_input(obs)
-        if isinstance(state_in, RingState):
+        if isinstance(state_in, _RING_STATES):
             _check_ring_call(self.net, img, state_in, _differentiable(self, img))
         if _differentiable(self, img):
             outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
@@ -1571,21 +1699,36 @@ class GraphedAct:
 
     memory="pytree" (default): the static state is the reference's list of (mask, (K, V)) fp32 and each step ends by copying the new
     state over it.  memory="ring": the static state is a `RingState` that the step updates in place (no copy of the memory; half its
-    bytes); a pytree or another RingState passed in is copied into it, and every call returns that RingState."""
+    bytes); a pytree or another RingState passed in is copied into it, and every call returns that RingState.
 
-    def __init__(self, policy: "MinecraftAgentPolicy", batch_size: int, pdl: bool = False, memory: str = "pytree"):
+    envs=E (with memory="ring"): asynchronous rollouts.  `state` is a RingState of E environments, and a call steps any k of them,
+    1 <= k <= batch_size: `step(obs_k, first_k, step.state.rows(idx))` with len(idx) = k.  The call pads its static buffers to batch_size
+    rows with inert rows (-1, zero frames, first False), so one graph per `stochastic` serves every subset without a host sync, and
+    returns the view with the first k rows of the outputs.  It takes only views of its own `state`: install a state with
+    `step.state.load_(...)` or `step.state.rows(idx).load_(...)`."""
+
+    def __init__(self, policy: "MinecraftAgentPolicy", batch_size: int, pdl: bool = False, memory: str = "pytree",
+                 envs: Optional[int] = None):
         if memory not in ("pytree", "ring"):
             raise ValueError(f"GraphedAct: memory must be 'pytree' or 'ring' (got {memory!r})")
+        if envs is not None and (memory != "ring" or envs < 1):
+            raise ValueError(f"GraphedAct: envs={envs} needs memory='ring' and at least one environment")
         self.policy = policy
         self.pdl = pdl
         self.memory = memory
+        self.envs = envs
         cfg = policy.net.cfg
         dev = policy.net.final_ln.weight.device
         B, self.B = batch_size, batch_size
         H, W = cfg.img_shape[0], cfg.img_shape[1]
         self.img = torch.zeros((B, H, W, 3), dtype=torch.uint8, device=dev)
         self.first = torch.zeros((B,), dtype=torch.bool, device=dev)
-        if memory == "ring":
+        if envs is not None:
+            self.state = RingState.zeros(policy, envs)
+            self.state._alloc_row_off()
+            self.idx = torch.full((B,), -1, dtype=torch.int32, device=dev)
+            self._view = RingRows(self.state, self.idx, [-1] * B)  # what the graph steps: the rows in self.idx
+        elif memory == "ring":
             self.state = RingState.zeros(policy, B)
         else:
             self.state = [(torch.zeros((B, 1, cfg.maxlen), dtype=torch.bool, device=dev),
@@ -1596,8 +1739,8 @@ class GraphedAct:
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):  # warm-up outside capture (lazy function attributes, allocator pools)
             for _ in range(2):
-                policy.act({"img": self.img}, self.first, self.state)
-            if memory == "ring":  # the warm-up stepped the ring in place: back to the empty state
+                policy.act({"img": self.img}, self.first, self.state if envs is None else self._view)  # (a view: inert rows only)
+            if memory == "ring" and envs is None:  # the warm-up stepped the ring in place: back to the empty state
                 for buf in self.state.k + self.state.v + self.state.mask + [self.state.off]:
                     buf.zero_()
         torch.cuda.current_stream(dev).wait_stream(side)
@@ -1617,7 +1760,8 @@ class GraphedAct:
         nat.lib().vpt_set_pdl(1 if self.pdl else 0)
         try:
             with torch.cuda.graph(g):
-                ac, st, res = self.policy.act({"img": self.img}, self.first, self.state, stochastic=stochastic, return_pd=True)
+                state = self.state if self.envs is None else self._view
+                ac, st, res = self.policy.act({"img": self.img}, self.first, state, stochastic=stochastic, return_pd=True)
                 if self.memory == "pytree":
                     for (m_in, (k_in, v_in)), (m_out, (k_out, v_out)) in zip(self.state, st):  # roll the state inside the graph
                         m_in.copy_(m_out)
@@ -1625,13 +1769,53 @@ class GraphedAct:
                             ops.copy_rows2(k_out, v_out, 0, k_in, v_in, 0, k_in.shape[1])  # K and V in one launch
         finally:
             nat.lib().vpt_set_pdl(0)
-        self.graphs[stochastic] = (g, ac, res)
-        return self.graphs[stochastic]
+        self.graphs[self._key(stochastic)] = (g, ac, res)
+        return self.graphs[self._key(stochastic)]
+
+    def _replay(self, stochastic: bool):
+        held = self._layouts()
+        if any(a is not b for a, b in zip(held, self._held)):  # a copy was rebuilt since capture (a load, an optimizer step): re-capture
+            self.graphs = {}
+            self._held = held
+        g, ac, res = self.graphs.get(self._key(stochastic)) or self._capture(stochastic)
+        g.replay()
+        return ac, res
+
+    def _key(self, stochastic: bool):
+        # a ring given per-row offsets (copied in from a ring that has them) runs other kernels than the graph captured without them
+        return stochastic, self.memory == "ring" and self.state.row_off is not None
+
+    def _call_rows(self, obs, first, view, stochastic: bool, return_pd: bool):
+        """envs=E: step the k environments of `view` as rows 0..k-1 of the graph, inert rows after them."""
+        if not isinstance(view, RingRows) or view.ring is not self.state:
+            raise ValueError("GraphedAct(envs=E) steps views of its own ring, `step.state.rows(idx)`; install other states with "
+                             "`step.state.load_` or `step.state.rows(idx).load_`")
+        k, B = len(view), self.B
+        if k > B:
+            raise ValueError(f"GraphedAct: a view of {k} rows for a graph of batch size {B}")
+        if obs["img"].shape[0] != k or first.shape[0] != k:
+            raise ValueError(f"GraphedAct: {obs['img'].shape[0]} frames and {first.shape[0]} `first` flags for a view of {k} rows")
+        self.idx[:k].copy_(view.idx)
+        self.img[:k].copy_(obs["img"])
+        self.first[:k].copy_(first)
+        if k < B:
+            self.idx[k:].fill_(-1)
+            self.img[k:].zero_()
+            self.first[k:].zero_()
+        ac, res = self._replay(stochastic)
+        out = {"log_prob": res["log_prob"][:k], "vpred": res["vpred"][:k]}
+        if return_pd:
+            out["pd"] = {n: x[:k] for n, x in res["pd"].items()}
+        return {n: x[:k] for n, x in ac.items()}, view, out
 
     @torch.no_grad()
     def __call__(self, obs, first, state_in, stochastic: bool = True, taken_action=None, return_pd: bool = False):
         if taken_action is not None:
             raise NotImplementedError("GraphedAct: taken_action is only supported by the eager act()")
+        if self.envs is not None:
+            return self._call_rows(obs, first, state_in, stochastic, return_pd)
+        if isinstance(state_in, RingRows):
+            raise ValueError("GraphedAct: a view of a ring needs GraphedAct(..., memory='ring', envs=E)")
         self.img.copy_(obs["img"])
         self.first.copy_(first)
         if state_in is not self.state and self.memory == "ring":
@@ -1644,12 +1828,7 @@ class GraphedAct:
                     m_in.copy_(m)
                 k_in.copy_(k)
                 v_in.copy_(v)
-        held = self._layouts()
-        if any(a is not b for a, b in zip(held, self._held)):  # a copy was rebuilt since capture (a load, an optimizer step): re-capture
-            self.graphs = {}
-            self._held = held
-        g, ac, res = self.graphs.get(stochastic) or self._capture(stochastic)
-        g.replay()
+        ac, res = self._replay(stochastic)
         out = {"log_prob": res["log_prob"], "vpred": res["vpred"]}
         if return_pd:
             out["pd"] = res["pd"]

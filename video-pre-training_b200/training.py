@@ -45,7 +45,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops
-from .policy import BF16, CNN_PREFIXES, F32, FrameLatents, InverseActionPolicy, MinecraftAgentPolicy, RingState, _dense_from_zp
+from .policy import BF16, CNN_PREFIXES, F32, FrameLatents, InverseActionPolicy, MinecraftAgentPolicy, RingRows, RingState, _dense_from_zp
 from .policy import _rot  # noqa: F401  (the dgrad weight layout lived here; code that imports it from this module keeps working)
 
 
@@ -286,7 +286,7 @@ class _Trainer:
         The tape also holds the kernel-layout weights the forward used (`prep`) and those the backward will use (`wts`, `heads_t`), and
         the backward's `_grad_plan` (want_dmem, want_dimg: see there).  The caller has checked the call's limits (`check_call`)."""
         net, pol = self.net, self.policy
-        if isinstance(state_in, RingState):
+        if isinstance(state_in, (RingState, RingRows)):
             raise ValueError("RingState is for inference: the trainers and the differentiable forward take the pytree state")
         tape = self._grad_plan(want_dmem, want_dimg)
         if pol is not None:
