@@ -22,7 +22,7 @@ import fwd_refs as Rf
 from test_gpu_backward_shapes import Guarded, _run_twice, check_bf16, check_sum
 from test_gpu_long_attention import fwd_ref as attention_ref
 from video_pre_training_b200 import _native as nat
-from video_pre_training_b200 import ops
+from video_pre_training_b200 import ops, ops_ring
 from video_pre_training_b200.policy import NBASIS, _dense_from_zp
 
 pytestmark = pytest.mark.gpu
@@ -91,16 +91,64 @@ def peak_memory(request):
 
 
 def chunks(s):
-    """the production chunk and a ragged last chunk (N = chunk + 200 frames; the IDM cuts whole 128-frame sequences: 512 + 256)"""
-    return (s["chunk"], 256) if s["conv3d"] else (s["chunk"], 200)
+    """the production chunk, a ragged last chunk (N = chunk + 200 frames; the IDM cuts whole 128-frame sequences: 512 + 256) and the
+    small calls (`small_counts`)"""
+    return ((s["chunk"], 256) if s["conv3d"] else (s["chunk"], 200)) + tuple(small_counts(s))
+
+
+def pool_parts(Fn, H, W, Cc):
+    """statistics partials per frame of vpt_maxpool3s2 on a [Fn, H, W, Cc] input, with the per-channel partials where ops.maxpool3s2 asks
+    for them"""
+    return lib().vpt_pool_chan_parts(Fn, H, W, Cc) if with_chan(Cc) else lib().vpt_pool_stat_parts(Fn, H, W, Cc)
+
+
+def plan_probes(s):
+    """{op: Fn -> statistics partials per frame} of the CNN ops whose launch plan follows the frame count: the blocks' convolutions
+    (64-column weight tiles for a few frames) and the pools of stacks 1 and 2 (more blocks per frame)"""
+    probes = {}
+    for i, sh in enumerate(s["stacks"]):
+        H, W, Cc = sh["H"], sh["W"], sh["C"]
+        probes[f"stack {i} block conv"] = lambda Fn, H=H, W=W, Cc=Cc: conv_parts(Fn, H // 2, W // 2, Cc)
+        if not sh["fused_first"]:
+            probes[f"stack {i} maxpool3s2"] = lambda Fn, H=H, W=W, Cc=Cc: pool_parts(Fn, H, W, Cc)
+    return probes
+
+
+def last_small(probe, chunk):
+    """the largest frame count whose partial count differs from the production chunk's (None: every count takes the chunk's plan)"""
+    at_chunk = probe(chunk)
+    return max((Fn for Fn in range(1, chunk) if probe(Fn) != at_chunk), default=None)
+
+
+def small_counts(s):
+    """1, 3, 8 and 9 frames, and for each op of `plan_probes` the last count of its small-call plan and the first of the batch plan
+    (derived from the C ABI, so the cases follow the kernels when the thresholds move)"""
+    counts = {1, 3, 8, 9}
+    for probe in plan_probes(s).values():
+        last = last_small(probe, s["chunk"])
+        if last is not None:
+            counts |= {last, last + 1}
+    return sorted(counts)
+
+
+def check_plan(s, op, Fn):
+    """prints the plan a call of Fn frames takes (its partials per frame beside the production chunk's) and asserts it at the op's own
+    boundary: the small-call plan at the last count that takes it, the batch plan one frame later"""
+    probe = plan_probes(s)[op]
+    P, P0, last = probe(Fn), probe(s["chunk"]), last_small(probe, s["chunk"])
+    print(f"{op} F={Fn}: {'small-call' if P != P0 else 'batch'} plan, {P} partials per frame ({P0} at the production chunk)")
+    assert Fn != last or P != P0, (op, Fn)
+    assert last is None or Fn != last + 1 or P == P0, (op, Fn)
 
 
 def frame_kind(f, Fn):
+    if Fn < 5:  # every kind that fits: the last frame near-constant from 3 frames on, a single frame DC-shifted (as edge_rows' single row)
+        return "const" if (f == Fn - 1 and Fn >= 3) else "dc" if (f % 2 == 1 or Fn == 1) else "randn"
     return "const" if f == Fn - 1 else "dc" if (f % 2 == 1 or f == Fn - 2) else "randn"
 
 
 def sel_frames(Fn):
-    return sorted({0, 1, Fn // 2, Fn - 2, Fn - 1})
+    return sorted({f for f in (0, 1, Fn // 2, Fn - 2, Fn - 1) if 0 <= f < Fn})
 
 
 def fill(t, seed, relu=False):
@@ -207,6 +255,13 @@ def with_chan(Cc):
     return Cc >= 8 and 256 % (Cc // 8) == 0
 
 
+def chan_sums(y_zp, parts):
+    """per-channel (sum, sumsq) partials of the interior of ZP y, fp32 [F][parts][C][2]: float64 sums over `parts` runs of pixels, each
+    rounded once (the shape norm2_fold reads, whatever kernel made them)"""
+    yi = y_zp[:, :-1, :-1, :].to(F64).flatten(1, 2)
+    return torch.stack([torch.stack([b.sum(1), (b * b).sum(1)], -1) for b in yi.tensor_split(parts, 1)], 1).float()
+
+
 def in_chunks(fn, x, n=64):
     return torch.cat([fn(x[i:i + n]) for i in range(0, x.shape[0], n)])
 
@@ -277,7 +332,8 @@ def test_stack_firstconv_and_pool(model):
             check_frames(f"{w} stack {i} firstconv F={Fn}", full, Rf.conv(x[idx], sd, p + ".firstconv"), idx, CONV_FLOOR)
             del xb, x
             chan = with_chan(Cc)
-            P = lib().vpt_pool_chan_parts(Fn, H, W, Cc) if chan else lib().vpt_pool_stat_parts(Fn, H, W, Cc)
+            P = pool_parts(Fn, H, W, Cc)
+            check_plan(s, f"stack {i} maxpool3s2", Fn)
             yb, y = guarded_zp(Fn, H // 2, W // 2, Cc)
             pb, cb = Guarded(Fn * P * 2), Guarded(Fn * P * Cc * 2 if chan else 4)
 
@@ -317,8 +373,13 @@ def test_block0_with_the_stack_norm_folded(model):
         for Fn in chunks(s):
             yb, y1 = guarded_zp(Fn, H, W, Cc)
             fill(y1, 200 + i, relu=True)
-            NP = H // 8
-            chan = in_chunks(lambda v: Rf.chan_sums(v, NP), y1)
+            # as many partials as the producer hands norm2_fold at this frame count: one per 8 x 8 tile from the fused first conv, the
+            # pool's blocks per frame otherwise (more of them for a few frames)
+            NP = lib().vpt_firstconv_stat_parts(Fn, sh["H"], sh["W"], Cc) // Cc if sh["fused_first"] else pool_parts(Fn, sh["H"], sh["W"], Cc)
+            if not sh["fused_first"]:
+                check_plan(s, f"stack {i} maxpool3s2", Fn)
+            print(f"{w} stack {i} norm2_fold F={Fn}: {NP} per-channel partials per frame")
+            chan = in_chunks(lambda v: chan_sums(v, NP), y1)
             bufs = [Guarded(Fn * 2), Guarded(Fn * 9 * Cc), Guarded(Fn * Cc), Guarded(Fn * Cc)]
             mrE, Ef, rs, rb = bufs[0].t.view(Fn, 2), bufs[1].t.view(Fn, 9, Cc), bufs[2].t.view(Fn, Cc), bufs[3].t.view(Fn, Cc)
 
@@ -342,6 +403,7 @@ def test_block0_with_the_stack_norm_folded(model):
             assert e <= FOLD_REL
             hb, hmid = guarded_zp(Fn, H, W, Cc)
             pb = conv_part_buf(Fn, H, W, Cc)
+            check_plan(s, f"stack {i} block conv", Fn)
             res = {}
 
             def conv0():
@@ -409,6 +471,7 @@ def test_block1_and_the_training_layout(model):
             Wb, S1, S2 = st["convs"][2]
             hb, hmid = guarded_zp(Fn, H, W, Cc)
             pb = conv_part_buf(Fn, H, W, Cc)
+            check_plan(s, f"stack {i} block conv", Fn)
             res = {}
 
             def conv0():
@@ -459,7 +522,7 @@ def test_block1_and_the_training_layout(model):
 
 
 def test_idm_conv3d_pre_stage(model):
-    """vpt_conv3d_t5 at B x T = 4 x 128 (and 2 x 128), 128 x 128 px, C = 128 against float64 conv3d_stage, on the frames at both ends of
+    """vpt_conv3d_t5 at B x T = 4 x 128 (and 2 x 128, and one sequence of each small count), 128 x 128 px, C = 128 against float64 conv3d_stage, on the frames at both ends of
     every sequence (the clipped time window) and one in the middle"""
     w, s, pol, sd, prep = model
     if s["conv3d"] is None:
@@ -468,7 +531,7 @@ def test_idm_conv3d_pre_stage(model):
     Cc, T = s["conv3d"], s["t"]
     w3, b3 = prep.conv3d
     for Fn in chunks(s):
-        B = Fn // T
+        B, T = (Fn // s["t"], s["t"]) if Fn % s["t"] == 0 else (1, Fn)  # a few frames: one short sequence
         img = torch.randint(0, 256, (B, T, H, W, 3), dtype=torch.uint8, generator=torch.Generator(device=DEV).manual_seed(Fn), device=DEV)
         img[-1, -3:] = 100 + img[-1, -3:] // 32  # nearly flat last frames
         P = lib().vpt_conv3d_stat_parts(H, W, Cc)
@@ -486,7 +549,7 @@ def test_idm_conv3d_pre_stage(model):
         mr = ops.stats_finalize(pb.t.view(Fn, P, 2), Fn, P, H * W * Cc)
         got, ref, fr = [], [], []
         for b in range(B):
-            for t in (0, 1, T // 2, T - 2, T - 1):
+            for t in sorted({t for t in (0, 1, T // 2, T - 2, T - 1) if 0 <= t < T}):
                 lo, hi = max(0, t - 2), min(T, t + 3)
                 ref.append(Rf.conv3d(img[b:b + 1, lo:hi], sd, "conv3d_layer")[t - lo])
                 fr.append(b * T + t)
@@ -516,9 +579,36 @@ def guarded_rows(M, N, dtype=BF16, ld=None):
     return b, b.t.view(M, ld or N)
 
 
+ROWS = [2048, 1096, 64, 9, 8, 3, 1]  # the tensor-core kernel from 9 rows (partial M tiles but at 2048), weight streaming up to 8
+
+
+def check_gemm_plan(name, M, part):
+    """the GEMM kernel a call of M rows ran, read from the statistics partials [M][P][2] (P >= 2) it wrote with stat_mode=1: the
+    weight-streaming kernel's row pass puts each row's whole (sum, sumsq) in slot 0 and zeros in the others, the tensor-core kernel one
+    partial per 64-column half of its N tiles.  It must be the weight-streaming kernel up to 8 rows and the tensor-core kernel above."""
+    assert part.shape[1] >= 2
+    streamed = bool((part[:, 1:] == 0).all())
+    print(f"{name}: {'gemv_small_kernel' if streamed else 'gemm_tc_kernel'} ({part.shape[1]} partials per row)")
+    assert streamed == (M <= 8), name
+
+
+def plan_partials(x, Wb, M, N, K, **kw):
+    """The statistics partials of a sibling of a GEMM call that writes none (the heads, the fused QKVR): the same x, weights, M, N and K
+    into a scratch output, with stat_mode=1 partials and without destination segments.  vpt_gemm_bf16 picks its kernel by M and K alone
+    for such calls (csrc/gemv_small.cuh, `try_launch_gemv_small`), so the sibling runs the call's kernel (`check_gemm_plan`)."""
+    P = ops.gemm_stat_parts(N)
+    ld = kw.pop("ld_out", N)
+    out = torch.empty((M, ld), dtype=F32, device=DEV)
+    part = torch.empty((M, P, 2), dtype=F32, device=DEV)
+    ops.gemm(x, Wb, out, M, N, K, ld_out=ld, stat_part=part, stat_mode=1, **kw)
+    torch.cuda.synchronize()
+    nat.device_check()
+    return part
+
+
 def _linear_case(name, x, fold, N, ref, *, mr=None, relu=0, residual=None, flat_floor=LIN_FLOOR):
     """one vpt_gemm_bf16 call with stat_mode=1 partials into guarded buffers: run twice, output against `ref`, statistics against float64
-    LayerNorm statistics of the stored output"""
+    LayerNorm statistics of the stored output, and the kernel it ran (`check_gemm_plan`)"""
     M, K = x.shape
     Wb, S1, S2 = fold
     P = ops.gemm_stat_parts(N)
@@ -537,6 +627,7 @@ def _linear_case(name, x, fold, N, ref, *, mr=None, relu=0, residual=None, flat_
 
     _run_twice(name, call)
     assert all_finite(out) and all_finite(pb.t)
+    check_gemm_plan(name, M, pb.t.view(M, P, 2))
     kinds = ["const" if (r == M - 1 and M > 1) else "dc" if (r % 2 == 1 or M == 1) else "randn" for r in range(M)]
     for k in dict.fromkeys(kinds):
         j = [r for r in range(M) if kinds[r] == k]
@@ -544,11 +635,11 @@ def _linear_case(name, x, fold, N, ref, *, mr=None, relu=0, residual=None, flat_
     check_stats(f"{name} (mean, rstd)", res["mr"], Rf.stats(out))
 
 
-@pytest.mark.parametrize("M", [2048, 8, 1])
+@pytest.mark.parametrize("M", ROWS)
 def test_linear_folds(model, M):
     """dense (ZP rows, zero weight columns at the pads), linear, mlp0 (LayerNorm fold, ReLU), mlp1 (residual; relu=2 on the last block),
     proj (residual = x_hat) and lastlayer through vpt_gemm_bf16 against float64 fanin_linear / F.linear: M = 2048 on the tensor-core
-    kernel, M = 1 and 8 on the small-M streaming kernel of rollout"""
+    kernel, M = 1096, 64 and 9 on its partial M tiles (many-environment rollouts), M = 1, 3 and 8 on the small-M streaming kernel"""
     w, s, pol, sd, prep = model
     cfg = s["cfg"]
     Hf, Wf, C2, kd = s["dense"]
@@ -579,7 +670,7 @@ def test_linear_folds(model, M):
     nat.device_check()
 
 
-@pytest.mark.parametrize("M", [2048, 8, 1])
+@pytest.mark.parametrize("M", ROWS)
 def test_heads_and_log_softmax(model, M):
     """the heads GEMM (out_scale = 1 / temperature, fp32 out, ragged N, ld > N: the columns beyond N stay NaN) against float64
     F.linear / temperature, then vpt_log_softmax of every head (each of the IDM's sub-actions) reading the raw logits between NaN guard
@@ -603,6 +694,7 @@ def test_heads_and_log_softmax(model, M):
         return [raw[:, :N].clone()], [rb]
 
     _run_twice(f"{w} heads GEMM M={M} N={N} ld={ld}", heads)
+    check_gemm_plan(f"{w} heads GEMM M={M}", M, plan_partials(lat, Wb, M, N, s["h"], S2=S2, out_scale=1.0 / temp, ld_out=ld))
     assert all_finite(raw[:, :N])
     check_sum(f"{w} heads logits M={M}", raw[:, :N], ref, scale, HEAD_ELEM, HEAD_L2)
     for name, c0, n, cnt in s["head_cols"]:
@@ -626,42 +718,51 @@ def test_heads_and_log_softmax(model, M):
 # attention block: fused QKVR, KV memory copies, attention
 # ---------------------------------------------------------------------------------------------------------------------
 def test_fused_qkvr(model):
-    """the Q | K | V | R GEMM with column segments (policy.py, `_block`) at B = 16 (IDM: 4), t = 128: K / V land in the rows of full_k /
-    full_v after the memory rows (untouched, NaN), R in fp32 with a row pitch wider than its columns (untouched, NaN); against four float64
-    F.linear"""
+    """the Q | K | V | R GEMM with column segments (policy.py, `_block`) at B = 16 (IDM: 4), t = 128, and for the policies at the
+    rollout rows (B, t) = (1, 1), (8, 1) (the weight-streaming kernel), (9, 1) and (64, 1) (partial M tiles), each in the pytree layout
+    and the ring layout: K / V land in the rows of full_k / full_v after the memory rows (untouched, NaN), or in (B, 1, h) step rows for
+    the ring (`seg` the identity); R in fp32 with a row pitch wider than its columns (untouched, NaN); against four float64 F.linear"""
     w, s, pol, sd, prep = model
-    h, heads, maxlen, t = s["h"], s["heads"], s["maxlen"], s["t"]
-    B = 4 if s["conv3d"] else 16
-    T, M = maxlen + t, B * t
+    h, heads, maxlen = s["h"], s["heads"], s["maxlen"]
     o = "recurrent_layer.blocks.0.r.orc_block"
     Wc, _, bc = prep.layers[0]["qkvr"]
     assert Wc.shape[0] == s["qkvr"]
-    xhat = edge_rows(M, h, 8)
     nr = NBASIS * heads if s["causal"] else 0
     ldr = nr + 8
-    qb, q = guarded_rows(M, h)
-    kb, vb = Guarded(B * T * h, BF16), Guarded(B * T * h, BF16)
-    fk, fv = kb.t.view(B, T, h), vb.t.view(B, T, h)
-    Rb, R = guarded_rows(M, ldr, F32)
-    dsts = [(0, q, h, False), (h, fk, h, True), (2 * h, fv, h, True)] + ([(3 * h, R, ldr, False)] if nr else [])
+    cases = [(4 if s["conv3d"] else 16, s["t"], "pytree")]
+    if s["causal"]:
+        cases += [(B, 1, layout) for B in (1, 8, 9, 64) for layout in ("pytree", "ring")]
+    for B, t, layout in cases:
+        M = B * t
+        mem = maxlen if layout == "pytree" else 0  # memory rows before the step's K / V rows
+        T = mem + t
+        name = f"{w} fused qkvr B={B} t={t} {layout} layout"
+        xhat = edge_rows(M, h, 8 if t > 1 else 8 + M)
+        qb, q = guarded_rows(M, h)
+        kb, vb = Guarded(B * T * h, BF16), Guarded(B * T * h, BF16)
+        fk, fv = kb.t.view(B, T, h), vb.t.view(B, T, h)
+        Rb, R = guarded_rows(M, ldr, F32)
+        dsts = [(0, q, h, False), (h, fk, h, True), (2 * h, fv, h, True)] + ([(3 * h, R, ldr, False)] if nr else [])
 
-    def call():
-        refill(qb, kb, vb, Rb)
-        ops.gemm(xhat, Wc, q, M, Wc.shape[0], h, S2=bc, seg=(t, T, maxlen), dsts=dsts)
-        for full in (fk, fv):
-            assert (full[:, :maxlen].view(torch.int16) == -1).all(), "wrote into the memory rows"
-        assert (R[:, nr:].view(torch.int32) == -1).all(), "wrote beyond the R columns"
-        return [q.clone(), fk[:, maxlen:].clone(), fv[:, maxlen:].clone(), R[:, :nr].clone()], [qb, kb, vb, Rb]
+        def call():
+            refill(qb, kb, vb, Rb)
+            ops.gemm(xhat, Wc, q, M, Wc.shape[0], h, S2=bc, seg=(t, T, mem), dsts=dsts)
+            for full in (fk, fv):
+                assert (full[:, :mem].view(torch.int16) == -1).all(), "wrote into the memory rows"
+            assert (R[:, nr:].view(torch.int32) == -1).all(), "wrote beyond the R columns"
+            return [q.clone(), fk[:, mem:].clone(), fv[:, mem:].clone(), R[:, :nr].clone()], [qb, kb, vb, Rb]
 
-    _run_twice(f"{w} fused qkvr B={B} t={t} maxlen={maxlen}", call)
-    refs = [Rf.plain_linear(xhat, sd, o + ".q_layer"), Rf.plain_linear(xhat, sd, o + ".k_layer", bias=False),
-            Rf.plain_linear(xhat, sd, o + ".v_layer", bias=False)]
-    for name, got, ref in zip("qkv", (q, fk[:, maxlen:].reshape(M, h), fv[:, maxlen:].reshape(M, h)), refs):
-        check_bf16(f"{w} fused qkvr {name}", got, ref, LIN_FLOOR)
-    if nr:
-        ref = Rf.plain_linear(xhat, sd, o + ".r_layer")
-        Wr = sd[o + ".r_layer.weight"]
-        check_sum(f"{w} fused qkvr R (fp32)", R[:, :nr], ref, xhat.to(F64).abs() @ Wr.abs().T + sd[o + ".r_layer.bias"].abs(), HEAD_ELEM, HEAD_L2)
+        _run_twice(name, call)
+        check_gemm_plan(name, M, plan_partials(xhat, Wc, M, Wc.shape[0], h, S2=bc))
+        refs = [Rf.plain_linear(xhat, sd, o + ".q_layer"), Rf.plain_linear(xhat, sd, o + ".k_layer", bias=False),
+                Rf.plain_linear(xhat, sd, o + ".v_layer", bias=False)]
+        for c, got, ref in zip("qkv", (q, fk[:, mem:].reshape(M, h), fv[:, mem:].reshape(M, h)), refs):
+            check_bf16(f"{name} {c}", got, ref, LIN_FLOOR)
+        if nr:
+            ref = Rf.plain_linear(xhat, sd, o + ".r_layer")
+            Wr = sd[o + ".r_layer.weight"]
+            check_sum(f"{name} R (fp32)", R[:, :nr], ref, xhat.to(F64).abs() @ Wr.abs().T + sd[o + ".r_layer.bias"].abs(), HEAD_ELEM, HEAD_L2)
+        del qb, kb, vb, Rb, q, fk, fv, R
 
 
 def test_copy_rows2(model):
@@ -756,3 +857,53 @@ def test_attention(model, t):
     check_bf16(f"{w} attention heads={heads} t={t}", out, ref, ATTN_FLOOR)
     if causal:
         check_bf16(f"{w} attention heads={heads} t={t} [row with its memory fully masked]", out[3 * t:4 * t], ref[3 * t:4 * t], ATTN_FLOOR)
+    if causal and t == 1:
+        _ring_rows_case(w, x, out, B, maxlen, heads, g)
+
+
+def _ring_rows_case(w, x, lin_out, B, maxlen, heads, g):
+    """The same step on a ring (`vpt_ring_write_rows`, then `vpt_attention_ring_rows`) at a random `off`, random per-environment
+    `row_off` and batch rows mapped to a permutation of E = B + 3 environments, three of them inert (-1): every other row equals the
+    linear layout's row bit for bit, inert rows are zero, and environments no row lists keep every byte."""
+    h = x["Q"].shape[1]
+    E = B + 3
+    rows = torch.randperm(E, generator=torch.Generator().manual_seed(11))[:B].to(torch.int32)
+    rows[[2, 7, B - 1]] = -1
+    off = torch.randint(0, maxlen, (1,), generator=g, device=DEV, dtype=torch.int32)
+    row_off = torch.randint(0, maxlen, (E,), generator=g, device=DEV, dtype=torch.int32)
+    kb, vb, mb = Guarded(E * maxlen * h, BF16), Guarded(E * maxlen * h, BF16), Guarded(E * maxlen, torch.uint8)
+    kr, vr, mask = kb.t.view(E, maxlen, h), vb.t.view(E, maxlen, h), mb.t.view(E, maxlen)
+    rows_d = rows.to(DEV)
+    # memory key j of the batch row b listed at ring row r sits at (off + row_off[r] + j) % maxlen; unlisted rows hold randn
+    k0 = torch.randn((E, maxlen, h), generator=g, device=DEV).to(BF16)
+    v0 = torch.randn((E, maxlen, h), generator=g, device=DEV).to(BF16)
+    m0 = (torch.rand((E, maxlen), generator=g, device=DEV) > 0.5).to(torch.uint8)
+    for b in range(B):
+        r = int(rows[b])
+        if r >= 0:
+            slot = (off + row_off[r] + torch.arange(maxlen, device=DEV)) % maxlen
+            k0[r, slot], v0[r, slot], m0[r, slot] = x["Kf"][b, :maxlen], x["Vf"][b, :maxlen], x["smask_u8"][b]
+    k_new, v_new = x["Kf"][:, maxlen].contiguous(), x["Vf"][:, maxlen].contiguous()
+    ob = Guarded(B * h, BF16)
+
+    def call():
+        kr.copy_(k0)
+        vr.copy_(v0)
+        mask.copy_(m0)
+        ob.raw.fill_(0xFF)
+        ops_ring.ring_write(k_new, v_new, kr, vr, mask, off, x["first_u8"], rows=rows_d, row_off=row_off)
+        nat.check(lib().vpt_attention_ring_rows(x["Q"].data_ptr(), kr.data_ptr(), vr.data_ptr(), x["R"].data_ptr(), x["R"].stride(0),
+                                                x["b_nd"].data_ptr(), x["first_u8"].data_ptr(), x["first_u8"].stride(0), mask.data_ptr(),
+                                                off.data_ptr(), rows_d.data_ptr(), row_off.data_ptr(), ob.ptr(), B, maxlen, heads,
+                                                x["b_nd"].shape[0], stream()), "vpt_attention_ring_rows")
+        return [ob.t.clone(), kr.clone(), vr.clone(), mask.clone()], [kb, vb, mb, ob]
+
+    _run_twice(f"{w} attention_ring_rows heads={heads} B={B} E={E}", call)
+    out = ob.t.view(B, h)
+    real = rows >= 0
+    bad = (out[real] != lin_out[real]).sum().item()
+    print(f"{w} attention_ring_rows heads={heads} B={B} E={E}: mismatches against the linear layout {bad}, "
+          f"nonzero values in the {int((~real).sum())} inert rows {int((out[~real] != 0).sum())} (bound 0)")
+    assert bad == 0 and bool((out[~real] == 0).all())
+    unlisted = sorted(set(range(E)) - set(rows[real].tolist()))
+    assert unlisted and all(torch.equal(a[unlisted], b[unlisted]) for a, b in ((kr, k0), (vr, v0), (mask, m0))), "an unlisted environment changed"

@@ -135,6 +135,14 @@ def test_inference_from_latents():
         assert torch.equal(k0, k1) and torch.equal(v0, v1)
 
 
+def _same_latents(part, ref, label):
+    nat.device_check()
+    dx = (part.x.float() - ref.x.float()).abs().max().item()
+    ds = (part.stats - ref.stats).abs().max().item()
+    print(f"{label}: max |dx| {dx:.3e}, max |dstats| {ds:.3e}")
+    assert torch.equal(part.x, ref.x) and torch.equal(part.stats, ref.stats), label
+
+
 def test_latent_rows_do_not_depend_on_the_encoded_batch():
     """`encode` of a slice against the slice of a whole encoding: the 2x agent over B = 16 against B = 3 and 5 (rows of frames the
     convolution tiles differently), the 4x IDM over B = 4 against B = 1 (re-batched along B only)."""
@@ -146,9 +154,49 @@ def test_latent_rows_do_not_depend_on_the_encoded_batch():
     img_i = torch.randint(0, 256, (4, 128, 128, 128, 3), dtype=torch.uint8, generator=torch.Generator().manual_seed(5)).cuda()
     cases.append((idm, img_i, idm.encode(img_i), (slice(2, 3),)))
     for mod, frames, enc, sl in cases:
-        part, ref = mod.encode(frames[sl]), enc[sl]
-        nat.device_check()
-        dx = (part.x.float() - ref.x.float()).abs().max().item()
-        ds = (part.stats - ref.stats).abs().max().item()
-        print(f"{type(mod).__name__} encode{sl} against the slice of the whole encoding: max |dx| {dx:.3e}, max |dstats| {ds:.3e}")
-        assert torch.equal(part.x, ref.x) and torch.equal(part.stats, ref.stats), sl
+        _same_latents(mod.encode(frames[sl]), enc[sl], f"{type(mod).__name__} encode{sl} against the slice of the whole encoding")
+
+
+@pytest.mark.parametrize("width", ["2x", "1x"])
+def test_latents_of_a_few_frames_do_not_depend_on_the_encoded_batch(width):
+    """A few frames take other launch plans in the CNN (narrow weight tiles, more pool blocks: other statistics partials) and in `dense`
+    (the weight-streaming GEMM up to 8 rows); `encode` pads them to the count from which every plan is the full chunk's.  Every slice
+    length from 1 frame to one past that count, against the same rows of a 2 x 48-frame encoding, and a call whose last 2048-frame chunk
+    holds 2 frames (B = 2, T = 1025), whose frames copy two of its first chunk."""
+    pol = _policy(width)
+    g = torch.Generator().manual_seed(6)
+    img = torch.randint(0, 256, (2, 48, 128, 128, 3), dtype=torch.uint8, generator=g).cuda()
+    whole = pol.encode(img)
+    n = pol.net._batch_plan_frames(1)
+    print(f"{width}: encode pads a chunk to {n} frames")
+    assert 17 <= n < 48
+    for L in range(1, n + 2):
+        t0 = (5 * L) % (48 - L)
+        _same_latents(pol.encode(img[1:2, t0:t0 + L]), whole[1:2, t0:t0 + L], f"{width} encode of {L} frames")
+    long = torch.randint(0, 256, (2, 1025, 128, 128, 3), dtype=torch.uint8, generator=g).cuda()
+    long[1, 1023:1025] = long[0, 0:2]
+    lat = pol.encode(long)
+    _same_latents(lat[1, 1023:1025], lat[0, 0:2], f"{width} B=2 T=1025: the 2 frames of the last chunk against the same frames in the first")
+
+
+def test_idm_latents_of_short_sequences_do_not_depend_on_the_encoded_batch():
+    """The IDM re-batched along B at T = 8: every B of 1 .. 4 sequences against the rows of one 6 x 8 encoding (the IDM pads whole
+    zero sequences)."""
+    idm = _idm()
+    img = torch.randint(0, 256, (6, 8, 128, 128, 3), dtype=torch.uint8, generator=torch.Generator().manual_seed(7)).cuda()
+    whole = idm.encode(img)
+    for b0, b1 in ((0, 1), (3, 4), (1, 3), (2, 5), (5, 6)):
+        _same_latents(idm.encode(img[b0:b1]), whole[b0:b1], f"IDM encode of B={b1 - b0} T=8 sequences")
+
+
+def test_2x_frozen_cnn_step_of_four_frames_from_sliced_latents():
+    """A frozen-CNN BC step at B = 1, T = 4 from latents sliced out of a 2 x 32-frame encoding: the step from the frames, bit for bit."""
+    pol = _policy()
+    _freeze_cnn(pol)
+    img, _, actions = _frames(torch.Generator().manual_seed(8), 2, 32)
+    lat = pol.encode(img)[1:2, 9:13]
+    img, first = img[1:2, 9:13].contiguous(), torch.zeros(1, 4, dtype=torch.bool).cuda()
+    actions = {k: a[1:2, 9:13].contiguous() for k, a in actions.items()}
+    tr = BCTrainer(pol)
+    _same(_step(pol, tr, lat, first, actions), _step(pol, tr, img, first, actions))
+    print("2x frozen-CNN BC step B=1 T=4: from sliced latents == from frames, bit for bit")

@@ -1,6 +1,7 @@
 """Tensor-level wrappers of the C ABI: torch tensors in, torch tensors out, everything enqueued on torch's current
 CUDA stream.  torch is used for device memory and streams only -- all arithmetic happens in libvpt_b200.so."""
 import ctypes as C
+import functools
 
 import torch
 
@@ -78,6 +79,29 @@ def set_default_cluster(cs):
 
 def gemm_stat_parts(N):
     return nat.lib().vpt_gemm_stat_parts(N)
+
+
+@functools.lru_cache(maxsize=None)
+def cnn_batch_plan_frames(stacks, chunk):
+    """The smallest frame count from which every convolution and pool of an ImpalaCNN runs the launch plan it has at `chunk` frames.
+    stacks: ((H, W, C), ...), each stack's input size and channels.  A few frames take plans with narrower weight tiles or more pool
+    blocks, and so more statistics partials per frame, summed in another order.  The count is at least 9: the `dense` GEMM streams
+    its weights for up to 8 rows, with its own summation order."""
+    lib = nat.lib()
+    probes = []
+    for H, W, Cc in stacks:
+        pool = lib.vpt_pool_chan_parts if Cc >= 8 and 256 % (Cc // 8) == 0 else lib.vpt_pool_stat_parts
+        probes += [lambda F_, H=H, W=W, Cc=Cc: lib.vpt_conv_zp_stat_parts(F_, H, W, Cc),  # the stack's first convolution
+                   lambda F_, H=H, W=W, Cc=Cc: lib.vpt_conv_zp_stat_parts(F_, H // 2, W // 2, Cc),  # the blocks' convolutions
+                   lambda F_, H=H, W=W, Cc=Cc, pool=pool: pool(F_, H, W, Cc)]
+    first = 9
+    for p in probes:
+        at_chunk = p(chunk)
+        F_ = chunk - 1
+        while F_ >= first and p(F_) == at_chunk:
+            F_ -= 1
+        first = max(first, F_ + 1)
+    return first
 
 
 def stats_finalize(part, G, n_per_group, count, eps=1e-5):

@@ -1070,6 +1070,20 @@ class MinecraftPolicy(nn.Module):
             tape.update(first_u8=first_u8)
         return self._upper_part(xd, mr_d, first_u8, state_in, B, t, prep)
 
+    def _batch_plan_frames(self, t):
+        """Frames per CNN chunk from which every launch plan of this net's CNN is the one of a full chunk (`ops.cnn_batch_plan_frames`);
+        the IDM's: whole sequences of t frames."""
+        cfg = self.cfg
+        H, W = cfg.img_shape[0], cfg.img_shape[1]
+        stacks = []
+        for c in cfg.chans:
+            stacks.append((H, W, c))
+            H, W = H // 2, W // 2
+        if cfg.conv3d_out is None:
+            return ops.cnn_batch_plan_frames(tuple(stacks), self.cnn_chunk_frames)
+        n = ops.cnn_batch_plan_frames(tuple(stacks), max(t, self.idm_chunk_frames // t * t))
+        return -(-n // t) * t
+
     def _cnn_part(self, frames, t, prep: _Prepared, train: bool):
         """frames [N, H, W, 3] (whole sequences of t frames) -> (xd bf16 [N, cnn_outsize], mr_d fp32 [N, 2]): the conv3d pre-stage (IDM),
         the ImpalaCNN in frame chunks and the dense layer.  train: the training layout (`_cnn_chunk`); with a tape (self._tape) it also
@@ -1080,7 +1094,6 @@ class MinecraftPolicy(nn.Module):
         Hf, Wf = cfg.final_hw
         C2 = cfg.chans[-1]
         # ---- ImpalaCNN in frame chunks (bounds the activation workspace), then ONE dense GEMM over all frames
-        cnn_out = torch.empty((N, Hf + 1, Wf + 1, C2), dtype=BF16, device=frames.device)
         mrs = []
         tape = self._tape
         # training forward: tape["recompute"] None keeps every stack's activations for the backward (one CNN pass per call); an integer
@@ -1093,15 +1106,31 @@ class MinecraftPolicy(nn.Module):
             step = self.cnn_chunk_frames if recompute is None else min(recompute, self.cnn_chunk_frames)
         else:  # chunks of whole sequences; the IDM's 128-channel full-resolution stage is ~13 MiB/frame
             step = max(1, (self.idm_chunk_frames if recompute is None else min(recompute, self.idm_chunk_frames)) // t) * t
+        # Latents promise a frame's output independent of its batch.  The convolutions and pools pick their launch plan by the chunk's
+        # frame count, and `dense` by its row count, and a few frames take plans that sum in another order.  So the training layout
+        # without a CNN tape (`encode`, a trainer with the CNN frozen) runs a short chunk padded with zero frames (the IDM: zero
+        # sequences) up to the count from which every plan is the one of a full chunk, and drops the padded rows after `dense`.
+        pad = self._batch_plan_frames(t) if train and not cnn_bwd else 0
+        step = max(step, pad)  # (only the last chunk can be short)
+        f_last = (N - 1) // step * step
+        Nr = f_last + max(N - f_last, pad)  # rows of cnn_out and of the dense GEMM
+        cnn_out = torch.empty((Nr, Hf + 1, Wf + 1, C2), dtype=BF16, device=frames.device)
         for f0 in range(0, N, step):
             F_ = min(step, N - f0)
-            chunk = frames[f0:f0 + F_] if cfg.conv3d_out is None else frames[f0:f0 + F_].view(F_ // t, t, *frame_shape)
-            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + F_], train=train, stacks=stacks,
+            Fr = min(step, Nr - f0)
+            chunk = frames[f0:f0 + F_]
+            if Fr > F_:
+                chunk = torch.cat([chunk, chunk.new_zeros((Fr - F_, *frame_shape))])
+            if cfg.conv3d_out is not None:
+                chunk = chunk.view(Fr // t, t, *frame_shape)
+            _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + Fr], train=train, stacks=stacks,
                                     record_from=0 if tape is None else tape["stacks_from"])
             mrs.append(mr)
         mr_c = mrs[0] if len(mrs) == 1 else torch.cat(mrs, 0)
         Kd = (Hf + 1) * (Wf + 1) * C2  # ZP rows flattened; the zero row / column meets zero weight columns
-        xd, mr_d = self._linear(cnn_out.view(N, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
+        xd, mr_d = self._linear(cnn_out.view(Nr, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
+        if Nr > N:
+            cnn_out, mr_c, xd, mr_d = cnn_out[:N], mr_c[:N], xd[:N], mr_d[:N]
         if tape is not None:
             assert not (cnn_bwd and recompute is None and len(mrs) != 1), "the stored tape holds one CNN chunk (training._Trainer.check_call)"
             tape.update(prep=prep, frames=frames, cnn_out=cnn_out, mr_c=mr_c, xd=xd, mr_d=mr_d,
