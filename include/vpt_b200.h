@@ -91,6 +91,11 @@ typedef struct vpt_gemm_args {
 } vpt_gemm_args;
 
 int vpt_gemm_bf16(const vpt_gemm_args* args, void* stream);
+/* Batch-invariant inference: vpt_gemm_bf16 on the weight-streaming kernel at any M.  Each row is computed exactly as an M = 1 call of
+ * vpt_gemm_bf16 computes it (same K split, lane-to-K mapping and combine order, which depend on N, K and the SM count only), over
+ * ceil(M / 8) row groups that each stream the weights (for M <= 8: the very launch vpt_gemm_bf16 makes).  Same epilogue contract.  Refused (VPT_ERR_ARG): conv, K % 8 != 0, stat_mode 2,
+ * statistics together with dst segments, M > 524280. */
+int vpt_gemm_bf16_rowwise(const vpt_gemm_args* args, void* stream);
 /* Cluster size used when vpt_gemm_args.cluster == 0 (tuning knob; 1, 2 or 4; initial value 1). */
 int vpt_set_default_cluster(int32_t cluster);
 /* Hardware experiment hook used by tools/desc_experiment.py (A rows loaded `shift` rows early, wgmma descriptor start
@@ -134,6 +139,9 @@ typedef struct vpt_conv_zp_args {
 } vpt_conv_zp_args;
 
 int vpt_conv3x3_zp(const vpt_conv_zp_args* args, void* stream);
+/* vpt_conv3x3_zp running, for any F, the launch plan it picks for plan_frames frames (the weight-tile width, hence stat_part's layout
+ * [rows][vpt_conv_zp_stat_parts(plan_frames, ...)]).  vpt_conv3x3_zp is the plan_frames = F case.  Batch-invariant inference passes 1. */
+int vpt_conv3x3_zp_plan(const vpt_conv_zp_args* args, int32_t plan_frames, void* stream);
 /* Kernel-variant knob kept for ABI compatibility: this build has a single convolution kernel, so bits 0..3 and 8 have no effect;
  * bits 4..7 select the epilogue timing experiment of tools/conv_bench.py (0 = off). */
 int vpt_set_conv_pair_mode(int32_t on);
@@ -226,6 +234,10 @@ int vpt_maxpool3s2(const void* in, void* out, float* stat_part, float* chan_part
                    void* stream);  /* chan_part: NULL or float2 [F][P][C] per-channel partials (needs C/8 | 256); with chan_part BOTH partial
                                       buffers hold P = vpt_pool_chan_parts(F, H, W, C) entries per frame instead of vpt_pool_stat_parts */
 int vpt_pool_chan_parts(int32_t F, int32_t H, int32_t W, int32_t C);
+/* vpt_maxpool3s2 with the blocks per frame (= partials per frame: vpt_pool_stat_parts / vpt_pool_chan_parts(plan_frames, H, W, C)) of a
+ * call of plan_frames frames, for any F.  vpt_maxpool3s2 is the plan_frames = F case. */
+int vpt_maxpool3s2_plan(const void* in, void* out, float* stat_part, float* chan_part, int32_t F, int32_t H, int32_t W, int32_t C, int32_t zp,
+                        int32_t plan_frames, void* stream);
 /* Two-norm composition: the post-pool GroupNorm `n` (lib/impala_cnn.py:119) is not run as a pass; its effect is folded into the two
  * consumers of x0 = n(y1): block 0's conv0 (input y1, weights W*gamma0*gamma_n, per-frame table Ef) and conv1 (residual y1 with a
  * per-frame affine).  From the per-channel (sum, sumsq) partials of y1 [F][NP][C] (vpt_firstconv_pool / vpt_maxpool3s2), gamma_n / beta_n
@@ -320,6 +332,23 @@ int vpt_attention_ring_rows(const void* Q, const void* Kr, const void* Vr, const
                             const int32_t* row_off, void* out, int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream);
 int vpt_ring_advance_rows(int32_t* row_off, const int32_t* rows, int32_t B, int32_t maxlen, void* stream);
 
+/* Batch-invariant inference.  The _plan variants of the attention run the long band's t = 1 cluster split that a call of plan_batch rows
+ * picks (it is the only batch-dependent choice of the causal attention; attention_kernel runs one CTA per (query block, head, row)).  The
+ * calls without _plan are the plan_batch = B case; vpt_attention_ring_rows_plan takes NULL rows / row_off like vpt_attention_ring_rows.
+ * vpt_ring_noise_keys  sampling keys of a ring step: keys int64 [B][2], keys[b] = (r, steps[r]) for batch row b of environment r (rows[b],
+ *                      or b if rows is NULL), then steps[r] += 1; an inert row (rows[b] < 0) gets (-1, 0).  steps int64 [E]. */
+int vpt_attention_plan(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
+                       int64_t first_stride, const uint8_t* smask, void* out, int32_t B, int32_t t, int32_t maxlen, int32_t heads, int32_t nbasis,
+                       int32_t causal, int32_t plan_batch, void* stream);
+int vpt_attention_ring_plan(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                            const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, void* out, int32_t B,
+                            int32_t maxlen, int32_t heads, int32_t nbasis, int32_t plan_batch, void* stream);
+int vpt_attention_ring_rows_plan(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                                 const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, const int32_t* rows,
+                                 const int32_t* row_off, void* out, int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, int32_t plan_batch,
+                                 void* stream);
+int vpt_ring_noise_keys(int64_t* steps, const int32_t* rows, int64_t* keys, int32_t B, void* stream);
+
 /* ----------------------------------------------------------------------------------------------------------
  * Action heads (lib/action_head.py:163-207)
  * -------------------------------------------------------------------------------------------------------- */
@@ -328,6 +357,11 @@ int vpt_log_softmax(const float* in, int64_t ld_in, int32_t col0, int32_t n, flo
 /* idx[r] = argmax_j(logits[r][j] - log(-log(u[r][j]))) with u==1 -> 0.999; u == NULL -> plain argmax (deterministic).
  * Ties resolve to the lowest index (torch.argmax). */
 int vpt_gumbel_argmax(const float* logits, const float* u, int64_t* idx, int64_t rows, int32_t n, void* stream);
+/* Gumbel-max with counter-based noise: keys int64 [rows][2] = (stream, step).  Row r's uniform for column j is word j % 4 of the
+ * Philox4x32-10 block of counter (j / 4, head, stream, step) (low 32 bits of stream and step) under key (seed low 32 bits, seed high 32
+ * bits), u = ((x >> 9) + 0.5) * 2^-23, exact in fp32 and in [2^-24, 1 - 2^-24]; idx[r] = argmax_j(logits[r][j] - log(-log(u))) in fp32, ties to the lowest index. */
+int vpt_gumbel_argmax_keyed(const float* logits, const int64_t* keys, uint64_t seed, int32_t head, int64_t* idx, int64_t rows, int32_t n,
+                            void* stream);
 /* lp[r] (+)= logits[r][idx[r]]   (lib/action_head.py:176-184) */
 int vpt_gather_logprob(const float* logits, const int64_t* idx, float* lp, int64_t rows, int32_t n, int32_t accumulate,
                        void* stream);

@@ -78,9 +78,11 @@ SIGNATURES = {
     "vpt_device_error": (_I, []),
     "vpt_num_sms": (_I, []),
     "vpt_gemm_bf16": (_I, [C.POINTER(GemmArgs), _P]),
+    "vpt_gemm_bf16_rowwise": (_I, [C.POINTER(GemmArgs), _P]),
     "vpt_gemm_stat_parts": (_I, [_I]),
     "vpt_set_default_cluster": (_I, [_I]),
     "vpt_conv3x3_zp": (_I, [C.POINTER(ConvZpArgs), _P]),
+    "vpt_conv3x3_zp_plan": (_I, [C.POINTER(ConvZpArgs), _I, _P]),
     "vpt_conv_zp_stat_parts": (_I, [_I, _I, _I, _I]),
     "vpt_conv_zp_t_stat_floats": (_L, [_I, _I, _I, _I]),
     "vpt_conv_zp_t_stats_finalize": (_I, [_P, _P, _I, _I, _I, _F, _P]),
@@ -104,6 +106,7 @@ SIGNATURES = {
     "vpt_codec_from_env": (_I, [_P, _P, _P, _I, _P, _L, _L, _P, _P]),
     "vpt_conv3d_stat_parts": (_I, [_I, _I, _I]),
     "vpt_maxpool3s2": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vpt_maxpool3s2_plan": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "vpt_norm2_fold": (_I, [_P, _I, _I, _L, _P, _P, _P, _P, _P, _P, _I, _F, _P, _P, _P, _P, _L, _P]),
     "vpt_pool_stat_parts": (_I, [_I, _I, _I, _I]),
     "vpt_pool_chan_parts": (_I, [_I, _I, _I, _I]),
@@ -122,8 +125,14 @@ SIGNATURES = {
     "vpt_ring_write_rows": (_I, [_P, _P, _P, _P, _P, _P, _L, _P, _P, _P, _I, _I, _I, _P]),
     "vpt_attention_ring_rows": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "vpt_ring_advance_rows": (_I, [_P, _P, _I, _I, _P]),
+    # batch-invariant inference (policy.py set_batch_invariant)
+    "vpt_attention_plan": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "vpt_attention_ring_plan": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vpt_attention_ring_rows_plan": (_I, [_P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vpt_ring_noise_keys": (_I, [_P, _P, _P, _I, _P]),
     "vpt_log_softmax": (_I, [_P, _L, _I, _I, _P, _L, _P]),
     "vpt_gumbel_argmax": (_I, [_P, _P, _P, _L, _I, _P]),
+    "vpt_gumbel_argmax_keyed": (_I, [_P, _P, C.c_uint64, _I, _P, _L, _I, _P]),
     "vpt_gather_logprob": (_I, [_P, _P, _P, _L, _I, _I, _P]),
     "vpt_resize_bilinear_u8": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "vpt_composite_cursor_u8": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),

@@ -277,7 +277,7 @@ __global__ void __launch_bounds__(kAttThreads) attention_kernel(
 // attention_long.cuh: the causal forward for a KV memory whose bias table does not fit this kernel's shared memory
 int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
                        const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
-                       int nbasis, const int* ring_off, const int* rows, const int* row_off, cudaStream_t stream);
+                       int nbasis, const int* ring_off, const int* rows, const int* row_off, int plan_B, cudaStream_t stream);
 
 // shared memory of attention_kernel for a causal band of `maxlen` keys with `nb` basis rows (nb = 0: mask "none")
 inline size_t attention_smem(int maxlen, int nb) {
@@ -287,10 +287,13 @@ inline size_t attention_smem(int maxlen, int nb) {
 
 }  // namespace vpt
 
-extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
-                             const uint8_t* first, int64_t first_stride, const uint8_t* smask, void* out, int32_t B, int32_t t,
-                             int32_t maxlen, int32_t heads, int32_t nbasis, int32_t causal, void* stream) {
+// plan_batch: the batch size whose launch plan (the long band's cluster split) the call runs; vpt_attention passes B.  attention_kernel
+// itself has no batch-dependent choice: one CTA per (query block, head, batch row).
+extern "C" int vpt_attention_plan(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
+                                  const uint8_t* first, int64_t first_stride, const uint8_t* smask, void* out, int32_t B, int32_t t,
+                                  int32_t maxlen, int32_t heads, int32_t nbasis, int32_t causal, int32_t plan_batch, void* stream) {
     using namespace vpt;
+    VPT_CHECK(plan_batch > 0, "vpt_attention_plan: plan_batch=%d must be > 0", plan_batch);
     VPT_CHECK(Q && Kf && Vf && out && B > 0 && t > 0 && heads > 0 && maxlen >= 0, "vpt_attention: bad arguments");
     if (causal) VPT_CHECK(maxlen > 0 && R && b_nd && first && nbasis > 0, "vpt_attention: causal mode needs maxlen > 0, R, b_nd, first");
     else VPT_CHECK(maxlen == 0, "vpt_attention: mask 'none' has no KV memory (maxlen must be 0)");
@@ -300,7 +303,7 @@ extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, cons
     if (smem > 227 * 1024) {  // only a causal band can be this long (mask 'none' has no memory): tile it over keys
         return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kf),
                                   reinterpret_cast<const __nv_bfloat16*>(Vf), R, ld_r, b_nd, first, first_stride, smask,
-                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, t, maxlen, heads, nb, nullptr, nullptr, nullptr, plan_batch, (cudaStream_t)stream);
     }
     static size_t attr = 0;
     if (smem > attr) {
@@ -316,16 +319,23 @@ extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, cons
     return VPT_OK;
 }
 
+extern "C" int vpt_attention(const void* Q, const void* Kf, const void* Vf, const float* R, int64_t ld_r, const float* b_nd,
+                             const uint8_t* first, int64_t first_stride, const uint8_t* smask, void* out, int32_t B, int32_t t,
+                             int32_t maxlen, int32_t heads, int32_t nbasis, int32_t causal, void* stream) {
+    return vpt_attention_plan(Q, Kf, Vf, R, ld_r, b_nd, first, first_stride, smask, out, B, t, maxlen, heads, nbasis, causal, B, stream);
+}
+
 namespace vpt {
 
 int attention_ring(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd, const uint8_t* first,
                    int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, const int32_t* rows, const int32_t* row_off, void* out,
-                   int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, void* stream) {
+                   int32_t B, int32_t maxlen, int32_t heads, int32_t nbasis, int32_t plan_B, void* stream) {
+    VPT_CHECK(plan_B > 0, "vpt_attention_ring_plan: plan_batch=%d must be > 0", plan_B);
     const size_t smem = attention_smem(maxlen, nbasis);
     if (smem > 227 * 1024) {
         return attention_long_fwd(reinterpret_cast<const __nv_bfloat16*>(Q), reinterpret_cast<const __nv_bfloat16*>(Kr),
                                   reinterpret_cast<const __nv_bfloat16*>(Vr), R, ld_r, b_nd, first, first_stride, smask,
-                                  reinterpret_cast<__nv_bfloat16*>(out), B, 1, maxlen, heads, nbasis, ring_off, rows, row_off, (cudaStream_t)stream);
+                                  reinterpret_cast<__nv_bfloat16*>(out), B, 1, maxlen, heads, nbasis, ring_off, rows, row_off, plan_B, (cudaStream_t)stream);
     }
     static size_t attr = 0;
     if (smem > attr) {
@@ -349,7 +359,7 @@ extern "C" int vpt_attention_ring(const void* Q, const void* Kr, const void* Vr,
     VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
               "vpt_attention_ring: bad arguments");
     VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring: grid too large");
-    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, nullptr, nullptr, out, B, maxlen, heads, nbasis, stream);
+    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, nullptr, nullptr, out, B, maxlen, heads, nbasis, B, stream);
 }
 
 extern "C" int vpt_attention_ring_rows(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
@@ -359,5 +369,29 @@ extern "C" int vpt_attention_ring_rows(const void* Q, const void* Kr, const void
     VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
               "vpt_attention_ring_rows: bad arguments");
     VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring_rows: grid too large");
-    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, rows, row_off, out, B, maxlen, heads, nbasis, stream);
+    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, rows, row_off, out, B, maxlen, heads, nbasis, B, stream);
+}
+
+// vpt_attention_ring / vpt_attention_ring_rows (rows may be null) with the long band's cluster split of plan_batch rows
+extern "C" int vpt_attention_ring_plan(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                                       const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off, void* out, int32_t B,
+                                       int32_t maxlen, int32_t heads, int32_t nbasis, int32_t plan_batch, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
+              "vpt_attention_ring_plan: bad arguments");
+    VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring_plan: grid too large");
+    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, nullptr, nullptr, out, B, maxlen, heads, nbasis, plan_batch,
+                          stream);
+}
+
+extern "C" int vpt_attention_ring_rows_plan(const void* Q, const void* Kr, const void* Vr, const float* R, int64_t ld_r, const float* b_nd,
+                                            const uint8_t* first, int64_t first_stride, const uint8_t* smask, const int32_t* ring_off,
+                                            const int32_t* rows, const int32_t* row_off, void* out, int32_t B, int32_t maxlen, int32_t heads,
+                                            int32_t nbasis, int32_t plan_batch, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(Q && Kr && Vr && R && b_nd && first && smask && ring_off && out && B > 0 && maxlen > 0 && heads > 0 && nbasis > 0,
+              "vpt_attention_ring_rows_plan: bad arguments");
+    VPT_CHECK(B <= 65535 && heads <= 65535, "vpt_attention_ring_rows_plan: grid too large");
+    return attention_ring(Q, Kr, Vr, R, ld_r, b_nd, first, first_stride, smask, ring_off, rows, row_off, out, B, maxlen, heads, nbasis, plan_batch,
+                          stream);
 }

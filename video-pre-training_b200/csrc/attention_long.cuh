@@ -552,7 +552,7 @@ __global__ void __launch_bounds__(kAbThreads) attn_bwd_mem_long_kernel(const __n
 // ---------------------------------------------------------------------------------------------------------------------------------
 int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __nv_bfloat16* Vf, const float* R, long long ld_r, const float* b_nd,
                        const uint8_t* first, long long first_stride, const uint8_t* smask, __nv_bfloat16* out, int B, int t, int maxlen, int heads,
-                       int nbasis, const int* ring_off, const int* rows, const int* row_off, cudaStream_t stream) {
+                       int nbasis, const int* ring_off, const int* rows, const int* row_off, int plan_B, cudaStream_t stream) {
     VPT_CHECK(nbasis <= kAlNb, "vpt_attention: nbasis=%d > %d", nbasis, kAlNb);
     const size_t smem = (size_t)(kAttBQ + 2 * kAttBK) * kAttPitch * 2 + (size_t)(kAlNb * kAlDist + 2 * kAttBQ) * 4 + kAttBK;
     const bool ring = ring_off != nullptr;
@@ -563,7 +563,9 @@ int attention_long_fwd(const __nv_bfloat16* Q, const __nv_bfloat16* Kf, const __
         attr_set[ring] = true;
     }
     const int nqb = (t + kAttBQ - 1) / kAttBQ;
-    const long long ctas = (long long)nqb * heads * B;
+    // few CTAs: split each query block's key band over a cluster.  The split is chosen for plan_B rows (B, or 1 for the batch-invariant
+    // plan); it fixes the order in which a row's partial softmax sums meet
+    const long long ctas = (long long)nqb * heads * plan_B;
     const int band_tiles = (maxlen + kAttBQ - 1 + kAttBK - 1) / kAttBK;  // most key tiles of one query block
     int nsplit = 1;
     if (ctas < num_sms()) nsplit = (int)min((long long)min(kAlSplitMax, band_tiles), (num_sms() + ctas - 1) / ctas);

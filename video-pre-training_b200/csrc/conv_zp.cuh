@@ -458,8 +458,9 @@ static inline void conv_zp_block_n(long long Q, int N, int* bn, int* nt) {
 }
 }  // namespace vpt
 
-extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
-    using namespace vpt;
+namespace vpt {
+// plan_frames: the frame count whose launch plan (weight-tile width, hence the statistics partial layout) the call runs
+static int conv3x3_zp_launch(const vpt_conv_zp_args* a, int plan_frames, void* stream) {
     VPT_CHECK(a && a->x && a->w && a->out, "vpt_conv3x3_zp: null operand");
     const int H = a->H, W = a->W, C = a->Cin, N = a->Cout;
     VPT_CHECK(a->F > 0 && H >= 2 && W >= 2 && C > 0 && C % 64 == 0 && N > 0 && N % 16 == 0,
@@ -474,7 +475,8 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
     p.Q = (long long)a->F * p.FS;
     VPT_CHECK(p.Q <= 2147483647LL - kBlockM, "vpt_conv3x3_zp: too many rows for 32-bit row indices and TMA coordinates");
     p.N = N; p.cin = C; p.cin_blocks = C / 64;
-    conv_zp_block_n(p.Q, N, &p.block_n, &p.num_n_tiles);
+    VPT_CHECK(plan_frames > 0, "vpt_conv3x3_zp_plan: plan_frames=%d must be > 0", plan_frames);
+    conv_zp_block_n((long long)plan_frames * p.FS, N, &p.block_n, &p.num_n_tiles);
     p.num_m_tiles = (p.Q + kBlockM - 1) / kBlockM;
     const int span = kBlockM + 2 * (p.Wp + 1);
     p.a_boxes = (span + 255) / 256;
@@ -532,6 +534,16 @@ extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
         launch_k(conv3x3_zp_kernel<128>, dim3((unsigned)grid), dim3(kCzThreads), smem_bytes, (cudaStream_t)stream, tmA, tmB, p);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
+}
+}  // namespace vpt
+
+extern "C" int vpt_conv3x3_zp(const vpt_conv_zp_args* a, void* stream) {
+    return vpt::conv3x3_zp_launch(a, a ? a->F : 1, stream);
+}
+
+// The plan of `plan_frames` frames at any F: each output row (and its statistics partials) is computed as in a call of plan_frames frames.
+extern "C" int vpt_conv3x3_zp_plan(const vpt_conv_zp_args* a, int32_t plan_frames, void* stream) {
+    return vpt::conv3x3_zp_launch(a, plan_frames, stream);
 }
 
 // Kernel-variant knobs of the C ABI.  This build has one convolution kernel (no CTA-pair or operand-swapped variant), so only the

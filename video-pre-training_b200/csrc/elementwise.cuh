@@ -539,14 +539,16 @@ extern "C" int vpt_norm2_fold(const float* chan_part, int32_t NP, int32_t C, int
     return VPT_OK;
 }
 
-extern "C" int vpt_maxpool3s2(const void* in, void* out, float* stat_part, float* chan_part, int32_t F, int32_t H, int32_t W, int32_t C, int32_t zp,
-                              void* stream) {
+// plan_frames: the frame count whose blocks per frame (= statistics partials per frame) the call runs; vpt_maxpool3s2 passes F
+extern "C" int vpt_maxpool3s2_plan(const void* in, void* out, float* stat_part, float* chan_part, int32_t F, int32_t H, int32_t W, int32_t C,
+                                   int32_t zp, int32_t plan_frames, void* stream) {
     using namespace vpt;
     VPT_CHECK(in && out && F > 0, "vpt_maxpool3s2: null argument");
     VPT_CHECK(!chan_part || (C >= 8 && 256 % (C / 8) == 0), "vpt_maxpool3s2: per-channel partials need C/8 to divide 256 (C=%d)", C);
     VPT_CHECK(H % 2 == 0 && W % 2 == 0 && C % 8 == 0, "vpt_maxpool3s2: need even H, W and C %% 8 == 0 (H=%d W=%d C=%d)", H, W, C);
     VPT_CHECK(F <= 65535, "vpt_maxpool3s2: at most 65535 frames per call (got %d)", F);
-    dim3 grid(chan_part ? vpt_pool_chan_parts(F, H, W, C) : vpt_pool_stat_parts(F, H, W, C), F);
+    VPT_CHECK(plan_frames > 0, "vpt_maxpool3s2_plan: plan_frames=%d must be > 0", plan_frames);
+    dim3 grid(chan_part ? vpt_pool_chan_parts(plan_frames, H, W, C) : vpt_pool_stat_parts(plan_frames, H, W, C), F);
     if (chan_part)
         launch_k(maxpool3s2_kernel<true>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out),
                                                                       reinterpret_cast<float2*>(stat_part), reinterpret_cast<float2*>(chan_part), H, W, C / 8, zp ? 1 : 0);
@@ -555,6 +557,11 @@ extern "C" int vpt_maxpool3s2(const void* in, void* out, float* stat_part, float
                                                                        reinterpret_cast<float2*>(stat_part), nullptr, H, W, C / 8, zp ? 1 : 0);
     VPT_LAUNCH_CHECK();
     return VPT_OK;
+}
+
+extern "C" int vpt_maxpool3s2(const void* in, void* out, float* stat_part, float* chan_part, int32_t F, int32_t H, int32_t W, int32_t C, int32_t zp,
+                              void* stream) {
+    return vpt_maxpool3s2_plan(in, out, stat_part, chan_part, F, H, W, C, zp, F, stream);
 }
 
 extern "C" int vpt_norm_stat_parts(int32_t rows_per_group, int32_t C) {

@@ -32,13 +32,17 @@ __device__ __forceinline__ uint4 ld_stream16(const uint4* p, uint64_t pol) {
 
 // kWpc warps share one output column (each streams a contiguous 1/kWpc of the K range; partial sums meet in shared memory): used when
 // N is small, so that the layer still has thousands of 16-byte loads in flight per SM (N = 256, K = 73984 `dense`: 32 CTAs otherwise).
-template <int kWpc>
+// kGroups: blockIdx.y picks a group of kGsMaxM rows (the any-M launch); without it the one group is rows 0..M-1 and the code is the M <= 8
+// launch's as it always was.  A row's sum is the same either way.
+template <int kWpc, bool kGroups>
 __global__ void __launch_bounds__(kGsThreads) gemv_small_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __restrict__ W,
                                                                   const GemmParams p) {
     pdl_sync();
     __shared__ float s_part[kGsThreads / 32][kGsMaxM];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int M = p.M, K8 = p.K >> 3;
+    const int m0 = kGroups ? blockIdx.y * kGsMaxM : 0;
+    const int M = kGroups ? min(p.M - m0, kGsMaxM) : p.M, K8 = p.K >> 3;
+    if (kGroups) A += (size_t)m0 * p.K;
     const uint64_t pol = l2_evict_first_policy();
     constexpr int kCols = (kGsThreads / 32) / kWpc;  // output columns per CTA
     const int kpart = warp % kWpc;
@@ -98,9 +102,10 @@ __global__ void __launch_bounds__(kGsThreads) gemv_small_kernel(const __nv_bfloa
 #pragma unroll
             for (int m = 0; m < kGsMaxM; ++m) {
                 if (m >= M) continue;
+                const int mg = m0 + m;
                 float ga = 1.f, gb = 0.f;
                 if (p.mr) {
-                    const int g = m / p.rows_per_group;
+                    const int g = mg / p.rows_per_group;
                     const float mean = __ldg(p.mr + 2 * g), rstd = __ldg(p.mr + 2 * g + 1);
                     ga = rstd;
                     gb = rstd * mean;
@@ -108,8 +113,8 @@ __global__ void __launch_bounds__(kGsThreads) gemv_small_kernel(const __nv_bfloa
                 float v = fmaf(ga, acc[m], fmaf(-gb, s1, s2));
                 if (p.relu == 1) v = fmaxf(v, 0.f);
                 if (p.residual) {
-                    v += p.residual_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)m * p.ld_res + n]
-                                        : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)m * p.ld_res + n]);
+                    v += p.residual_f32 ? reinterpret_cast<const float*>(p.residual)[(size_t)mg * p.ld_res + n]
+                                        : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[(size_t)mg * p.ld_res + n]);
                 }
                 if (p.relu == 2) v = fmaxf(v, 0.f);
                 v *= p.out_scale;
@@ -125,8 +130,8 @@ __global__ void __launch_bounds__(kGsThreads) gemv_small_kernel(const __nv_bfloa
                     d_out = p.dst_out[sg]; d_ld = p.dst_ld[sg]; d_f32 = p.dst_f32[sg]; d_col0 = p.dst_n0[sg];
                     d_remap = d_remap && p.dst_remap[sg] != 0;
                 }
-                long long orow = m;
-                if (d_remap) orow = (long long)(m / p.seg_len) * p.seg_stride + p.seg_off + (m % p.seg_len);
+                long long orow = mg;
+                if (d_remap) orow = (long long)(mg / p.seg_len) * p.seg_stride + p.seg_off + (mg % p.seg_len);
                 if (d_f32) reinterpret_cast<float*>(d_out)[(size_t)orow * d_ld + (n - d_col0)] = v;
                 else reinterpret_cast<__nv_bfloat16*>(d_out)[(size_t)orow * d_ld + (n - d_col0)] = __float2bfloat16_rn(v);
             }
@@ -154,9 +159,14 @@ __global__ void __launch_bounds__(256) row_stats_small_kernel(const GemmParams p
     for (int i = 1 + threadIdx.x; i < P; i += blockDim.x) sp[i] = make_float2(0.f, 0.f);
 }
 
-// returns VPT_OK after launching, or 1 if this shape is not handled here (caller falls through to the tensor-core kernel)
-static int try_launch_gemv_small(const vpt_gemm_args* a, void* stream) {
-    if (a->conv || a->M > kGsMaxM || (a->K & 7) != 0 || (a->stat_part && a->stat_mode != 1) || (a->ndst > 0 && a->stat_part)) return 1;
+static bool gemv_small_shape_ok(const vpt_gemm_args* a) {
+    return !a->conv && (a->K & 7) == 0 && !(a->stat_part && a->stat_mode != 1) && !(a->ndst > 0 && a->stat_part);
+}
+
+// Launches the weight-streaming kernel over ceil(M / 8) groups of rows.  Every row gets the accumulation order of the M <= 8 launch
+// (the K split, lane-to-K mapping and combine order come from N, K and the SM count only), so its result does not depend on M.
+template <bool kGroups>
+static int launch_gemv_small(const vpt_gemm_args* a, void* stream) {
     GemmParams p;
     memset(&p, 0, sizeof(p));
     p.M = a->M; p.N = a->N; p.K = a->K;
@@ -178,11 +188,12 @@ static int try_launch_gemv_small(const vpt_gemm_args* a, void* stream) {
     const bool split = a->N < 4 * num_sms() * (kGsThreads / 32) / 8 && a->K >= 2048;
     int grid = split ? a->N : (a->N + kGsThreads / 32 - 1) / (kGsThreads / 32);
     if (grid > 8 * 148) grid = 8 * 148;
+    const int groups = (a->M + kGsMaxM - 1) / kGsMaxM;
     if (split)
-        launch_k(gemv_small_kernel<kGsThreads / 32>, dim3(grid), dim3(kGsThreads), 0, (cudaStream_t)stream, reinterpret_cast<const __nv_bfloat16*>(a->A),
+        launch_k(gemv_small_kernel<kGsThreads / 32, kGroups>, dim3(grid, groups), dim3(kGsThreads), 0, (cudaStream_t)stream, reinterpret_cast<const __nv_bfloat16*>(a->A),
                                                                                           reinterpret_cast<const __nv_bfloat16*>(a->B), p);
     else
-        launch_k(gemv_small_kernel<1>, dim3(grid), dim3(kGsThreads), 0, (cudaStream_t)stream, reinterpret_cast<const __nv_bfloat16*>(a->A),
+        launch_k(gemv_small_kernel<1, kGroups>, dim3(grid, groups), dim3(kGsThreads), 0, (cudaStream_t)stream, reinterpret_cast<const __nv_bfloat16*>(a->A),
                                                                             reinterpret_cast<const __nv_bfloat16*>(a->B), p);
     VPT_LAUNCH_CHECK();
     if (a->stat_part) {
@@ -192,6 +203,28 @@ static int try_launch_gemv_small(const vpt_gemm_args* a, void* stream) {
     return VPT_OK;
 }
 
+// returns VPT_OK after launching, or 1 if this shape is not handled here (caller falls through to the tensor-core kernel)
+static int try_launch_gemv_small(const vpt_gemm_args* a, void* stream) {
+    if (a->M > kGsMaxM || !gemv_small_shape_ok(a)) return 1;
+    return launch_gemv_small<false>(a, stream);
+}
+
 int try_launch_gemv_small_fwd(const vpt_gemm_args* a, void* stream) { return try_launch_gemv_small(a, stream); }
 
 }  // namespace vpt
+
+// The weight-streaming kernel at any M (batch-invariant inference): each row is computed as the M = 1 launch computes it.  Shapes the
+// kernel does not take (conv, K % 8 != 0, stat_mode 2, destination segments with statistics) are refused, not sent elsewhere.
+extern "C" int vpt_gemm_bf16_rowwise(const vpt_gemm_args* a, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(a != nullptr && a->A && a->B && a->out, "vpt_gemm_bf16_rowwise: null operand");
+    VPT_CHECK(a->M > 0 && a->N > 0 && a->K > 0, "vpt_gemm_bf16_rowwise: bad shape M=%d N=%d K=%d", a->M, a->N, a->K);
+    VPT_CHECK(((uintptr_t)a->A & 15) == 0 && ((uintptr_t)a->B & 15) == 0, "vpt_gemm_bf16_rowwise: A/B must be 16-byte aligned");
+    VPT_CHECK(a->mr == nullptr || a->rows_per_group > 0, "vpt_gemm_bf16_rowwise: rows_per_group must be > 0 with mr");
+    VPT_CHECK(!(a->mr && !a->S1), "vpt_gemm_bf16_rowwise: mr given without S1");
+    VPT_CHECK(gemv_small_shape_ok(a), "vpt_gemm_bf16_rowwise: no conv, K %% 8 == 0 (K=%d), statistics in stat_mode 1 and not with dst segments",
+              a->K);
+    VPT_CHECK((a->M + kGsMaxM - 1) / kGsMaxM <= 65535, "vpt_gemm_bf16_rowwise: M=%d exceeds %d rows", a->M, 65535 * kGsMaxM);
+    // up to 8 rows: the M <= 8 launch itself (one group, the same kernel as vpt_gemm_bf16 runs there)
+    return a->M <= kGsMaxM ? launch_gemv_small<false>(a, stream) : launch_gemv_small<true>(a, stream);
+}

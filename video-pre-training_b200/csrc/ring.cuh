@@ -93,3 +93,32 @@ extern "C" int vpt_ring_advance_rows(int32_t* row_off, const int32_t* rows, int3
     VPT_LAUNCH_CHECK();
     return VPT_OK;
 }
+
+namespace vpt {
+// the sampling keys of a step of a ring (batch-invariant mode): keys[b] = (r, steps[r]) for batch row b of environment r, then steps[r] += 1;
+// an inert row (r < 0) gets (-1, 0) and advances nothing.  The rows are distinct: no two threads share an entry.
+__global__ void ring_noise_keys_kernel(long long* __restrict__ steps, const int* __restrict__ rows, long long* __restrict__ keys, int B) {
+    pdl_sync();
+    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
+        const int r = rows ? rows[b] : b;
+        if (r < 0) {
+            keys[2 * b] = -1;
+            keys[2 * b + 1] = 0;
+            continue;
+        }
+        const long long s = steps[r];
+        keys[2 * b] = r;
+        keys[2 * b + 1] = s;
+        steps[r] = s + 1;
+    }
+}
+}  // namespace vpt
+
+extern "C" int vpt_ring_noise_keys(int64_t* steps, const int32_t* rows, int64_t* keys, int32_t B, void* stream) {
+    using namespace vpt;
+    VPT_CHECK(steps && keys && B > 0, "vpt_ring_noise_keys: bad arguments");
+    launch_k(ring_noise_keys_kernel, dim3((B + 255) / 256), dim3(256), 0, (cudaStream_t)stream, reinterpret_cast<long long*>(steps), (const int*)rows,
+             reinterpret_cast<long long*>(keys), (int)B);
+    VPT_LAUNCH_CHECK();
+    return VPT_OK;
+}

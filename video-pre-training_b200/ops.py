@@ -42,6 +42,22 @@ def gemm(A, Bw, out, M, N, K, *, conv=None, mr=None, rows_per_group=1, S1=None, 
          residual=None, ld_out=None, seg=None, stat_part=None, stat_mode=0, cluster=0, dsts=None):
     """out = epilogue(A @ Bw^T); see struct vpt_gemm_args.  dsts: up to 4 column segments [(n0, tensor, ld, remap)] with their own
     destination buffer (then `out` is only used for its device / may be the first segment's tensor)."""
+    a = _gemm_args(A, Bw, out, M, N, K, conv=conv, mr=mr, rows_per_group=rows_per_group, S1=S1, S2=S2, relu=relu, out_scale=out_scale,
+                   residual=residual, ld_out=ld_out, seg=seg, stat_part=stat_part, stat_mode=stat_mode, cluster=cluster, dsts=dsts)
+    prof = GEMM_PROFILE
+    if prof is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    nat.check(nat.lib().vpt_gemm_bf16(C.byref(a), _stream()), "vpt_gemm_bf16")
+    if prof is not None:
+        e1.record()
+        prof.append((e0, e1, 2.0 * M * N * K, "conv" if conv is not None else "linear", (M, N, K)))
+    _count()
+    return out
+
+
+def _gemm_args(A, Bw, out, M, N, K, *, conv, mr, rows_per_group, S1, S2, relu, out_scale, residual, ld_out, seg, stat_part, stat_mode, cluster,
+               dsts):
     _cuda(A, Bw, out)
     a = nat.GemmArgs()
     a.A, a.B, a.M, a.N, a.K = _p(A), _p(Bw), M, N, K
@@ -61,16 +77,7 @@ def gemm(A, Bw, out, M, N, K, *, conv=None, mr=None, rows_per_group=1, S1=None, 
         for i, (n0, t, ld, remap) in enumerate(dsts):
             _cuda(t)
             a.dst_n0[i], a.dst_out[i], a.dst_ld[i], a.dst_f32[i], a.dst_remap[i] = n0, _p(t), ld, int(t.dtype == F32), int(remap)
-    prof = GEMM_PROFILE
-    if prof is not None:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-    nat.check(nat.lib().vpt_gemm_bf16(C.byref(a), _stream()), "vpt_gemm_bf16")
-    if prof is not None:
-        e1.record()
-        prof.append((e0, e1, 2.0 * M * N * K, "conv" if conv is not None else "linear", (M, N, K)))
-    _count()
-    return out
+    return a
 
 
 def set_default_cluster(cs):
@@ -114,22 +121,8 @@ def stats_finalize(part, G, n_per_group, count, eps=1e-5):
 def conv3x3_zp(x, Wb, H, W, *, mr=None, S1=None, S2=None, relu=1, residual=None, want_stats=True, out=None, Ef=None, res_scale=None,
                res_shift=None):
     """GroupNorm(1)->conv3x3->ReLU[+residual] on a ZP tensor x bf16 [F,H+1,W+1,Cin]; returns (ZP out, per-frame (mean, rstd))."""
-    _cuda(x, Wb)
-    F_, Cin = x.shape[0], x.shape[3]
-    Cout = Wb.shape[0]
-    assert tuple(x.shape[1:3]) == (H + 1, W + 1) and Wb.shape[1] == 9 * Cin
-    if out is None:
-        out = torch.empty((F_, H + 1, W + 1, Cout), dtype=BF16, device=x.device)
-    assert out.is_contiguous() and tuple(out.shape) == (F_, H + 1, W + 1, Cout)
-    P = nat.lib().vpt_conv_zp_stat_parts(F_, H, W, Cout)
-    tfl = nat.lib().vpt_conv_zp_t_stat_floats(F_, H, W, Cout)  # > 0: the swapped kernel's fragment epilogue (per-tile partials)
-    part = None
-    if want_stats:
-        part = torch.empty((tfl,) if tfl > 0 else (F_ * (H + 1) * (W + 1), P, 2), dtype=F32, device=x.device)
-    a = nat.ConvZpArgs()
-    a.x, a.w, a.F, a.H, a.W, a.Cin, a.Cout = _p(x), _p(Wb), F_, H, W, Cin, Cout
-    a.mr, a.S1, a.S2, a.relu, a.residual, a.out, a.stat_part = _p(mr), _p(S1), _p(S2), relu, _p(residual), _p(out), _p(part)
-    a.Ef, a.res_scale, a.res_shift = _p(Ef), _p(res_scale), _p(res_shift)  # two-norm composition (vpt_norm2_fold)
+    a, out, part, P, tfl = _conv_zp_args(x, Wb, H, W, mr, S1, S2, relu, residual, want_stats, out, Ef, res_scale, res_shift, x.shape[0])
+    F_, Cin, Cout = x.shape[0], x.shape[3], Wb.shape[0]
     prof = GEMM_PROFILE
     if prof is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -147,6 +140,28 @@ def conv3x3_zp(x, Wb, H, W, *, mr=None, S1=None, S2=None, relu=1, residual=None,
     elif want_stats:
         mr_out = stats_finalize(part, F_, (H + 1) * (W + 1) * P, H * W * Cout)
     return out, mr_out
+
+
+def _conv_zp_args(x, Wb, H, W, mr, S1, S2, relu, residual, want_stats, out, Ef, res_scale, res_shift, plan_frames):
+    """-> (vpt_conv_zp_args, out, the statistics partials or None, partials per row, fragment-partial floats) of a call whose launch
+    plan is that of `plan_frames` frames."""
+    _cuda(x, Wb)
+    F_, Cin = x.shape[0], x.shape[3]
+    Cout = Wb.shape[0]
+    assert tuple(x.shape[1:3]) == (H + 1, W + 1) and Wb.shape[1] == 9 * Cin
+    if out is None:
+        out = torch.empty((F_, H + 1, W + 1, Cout), dtype=BF16, device=x.device)
+    assert out.is_contiguous() and tuple(out.shape) == (F_, H + 1, W + 1, Cout)
+    P = nat.lib().vpt_conv_zp_stat_parts(plan_frames, H, W, Cout)
+    tfl = nat.lib().vpt_conv_zp_t_stat_floats(F_, H, W, Cout)  # > 0: the swapped kernel's fragment epilogue (per-tile partials)
+    part = None
+    if want_stats:
+        part = torch.empty((tfl,) if tfl > 0 else (F_ * (H + 1) * (W + 1), P, 2), dtype=F32, device=x.device)
+    a = nat.ConvZpArgs()
+    a.x, a.w, a.F, a.H, a.W, a.Cin, a.Cout = _p(x), _p(Wb), F_, H, W, Cin, Cout
+    a.mr, a.S1, a.S2, a.relu, a.residual, a.out, a.stat_part = _p(mr), _p(S1), _p(S2), relu, _p(residual), _p(out), _p(part)
+    a.Ef, a.res_scale, a.res_shift = _p(Ef), _p(res_scale), _p(res_shift)  # two-norm composition (vpt_norm2_fold)
+    return a, out, part, P, tfl
 
 
 def _frames_f32(img, what):
@@ -246,15 +261,24 @@ def attention_f32(q, full_k, full_v, R, b_nd, first_u8, smask_u8, B, t, maxlen, 
 def maxpool3s2(x, zp=True, want_chan=False):
     """bf16 [F,H,W,C] (>= 0) -> (bf16 [F,H/2,W/2,C], per-frame (mean, rstd)); with zp both tensors are ZP ([F,H+1,W+1,C]).
     want_chan: also the per-channel (sum, sumsq) partials [F, NP, C, 2] of the pooled tensor (None when C/8 does not divide 256)."""
+    return _maxpool3s2(x, zp, want_chan, None)
+
+
+def _maxpool3s2(x, zp, want_chan, plan_frames):
+    """maxpool3s2 with the blocks per frame of a call of plan_frames frames (None: the call's own)."""
     _cuda(x)
     z = int(zp)
     F_, H, W, Cc = x.shape[0], x.shape[1] - z, x.shape[2] - z, x.shape[3]
     out = torch.empty((F_, H // 2 + z, W // 2 + z, Cc), dtype=BF16, device=x.device)
     with_chan = want_chan and Cc >= 8 and 256 % (Cc // 8) == 0
-    P = nat.lib().vpt_pool_chan_parts(F_, H, W, Cc) if with_chan else nat.lib().vpt_pool_stat_parts(F_, H, W, Cc)
+    Fp = F_ if plan_frames is None else plan_frames
+    P = nat.lib().vpt_pool_chan_parts(Fp, H, W, Cc) if with_chan else nat.lib().vpt_pool_stat_parts(Fp, H, W, Cc)
     part = torch.empty((F_, P, 2), dtype=F32, device=x.device)
     chan = torch.empty((F_, P, Cc, 2), dtype=F32, device=x.device) if with_chan else None
-    nat.check(nat.lib().vpt_maxpool3s2(_p(x), _p(out), _p(part), _p(chan), F_, H, W, Cc, z, _stream()), "vpt_maxpool3s2")
+    if plan_frames is None:
+        nat.check(nat.lib().vpt_maxpool3s2(_p(x), _p(out), _p(part), _p(chan), F_, H, W, Cc, z, _stream()), "vpt_maxpool3s2")
+    else:
+        nat.check(nat.lib().vpt_maxpool3s2_plan(_p(x), _p(out), _p(part), _p(chan), F_, H, W, Cc, z, plan_frames, _stream()), "vpt_maxpool3s2_plan")
     _count()
     mr = stats_finalize(part, F_, P, (H // 2) * (W // 2) * Cc)
     return (out, mr, chan) if want_chan else (out, mr)
@@ -345,12 +369,20 @@ def state_mask_update(mask_in, first_u8, t, maxlen):
 
 
 def attention(Q, Kf, Vf, R, b_nd, first_u8, smask, B, t, maxlen, heads, causal=True):
+    return _attention(Q, Kf, Vf, R, b_nd, first_u8, smask, B, t, maxlen, heads, causal, None)
+
+
+def _attention(Q, Kf, Vf, R, b_nd, first_u8, smask, B, t, maxlen, heads, causal, plan_batch):
+    """attention with the launch plan of a call of plan_batch rows (None: the call's own)."""
     _cuda(Q, Kf, Vf)
     out = torch.empty_like(Q)
     nbasis = b_nd.shape[0] if (causal and b_nd is not None) else 0
-    nat.check(nat.lib().vpt_attention(_p(Q), _p(Kf), _p(Vf), _p(R), R.stride(-2) if R is not None else 0, _p(b_nd),
-                                      _p(first_u8), first_u8.stride(0) if first_u8 is not None else 0, _p(smask), _p(out), B, t,
-                                      maxlen, heads, nbasis, int(causal), _stream()), "vpt_attention")
+    args = (_p(Q), _p(Kf), _p(Vf), _p(R), R.stride(-2) if R is not None else 0, _p(b_nd), _p(first_u8), first_u8.stride(0) if first_u8 is not None else 0,
+            _p(smask), _p(out), B, t, maxlen, heads, nbasis, int(causal))
+    if plan_batch is None:
+        nat.check(nat.lib().vpt_attention(*args, _stream()), "vpt_attention")
+    else:
+        nat.check(nat.lib().vpt_attention_plan(*args, plan_batch, _stream()), "vpt_attention_plan")
     _count()
     return out
 
@@ -572,7 +604,8 @@ from .ops_dist import (head_entropy, head_entropy_bwd, head_kl, head_kl_bwd,  # 
                        rl_head_bwd_ent)
 from .ops_bptt import attention_bwd_state  # noqa: E402,F401  (gradients through the KV memory, csrc/attention_bwd.cuh)
 from .ops_pixel import conv3d_t5_dimg, firstconv_dimg  # noqa: E402,F401  (image gradients, csrc/firstconv_bwd.cuh, csrc/idm_bwd.cuh)
-from .ops_ring import attention_ring, ring_advance, ring_advance_rows, ring_write  # noqa: E402,F401  (the KV memory as a ring, csrc/ring.cuh)
+from .ops_ring import attention_ring, attention_ring_plan, ring_advance, ring_advance_rows, ring_noise_keys, ring_write  # noqa: E402,F401  (the KV memory as a ring, csrc/ring.cuh)
+from .ops_invariant import attention_plan, conv3x3_zp_plan, gemm_rowwise, gumbel_argmax_keyed, maxpool3s2_plan  # noqa: E402,F401  (batch-invariant mode)
 
 
 # ---- on-device action codec (csrc/codec.cuh) -----------------------------------------------------------------------------

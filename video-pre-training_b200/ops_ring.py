@@ -52,6 +52,15 @@ def ring_write(knew, vnew, k, v, mask, off, first_u8, rows=None, row_off=None):
 def attention_ring(Q, k, v, R, b_nd, first_u8, mask, off, heads, rows=None, row_off=None):
     """`ops.attention` (causal, t = 1) with the KV memory and the step's own row read from the ring (after `ring_write`): Q bf16 [B, h].
     With `rows`, batch row b (Q, R, first, out) attends over ring row rows[b]; an inert row's output is zero."""
+    return _attention_ring(Q, k, v, R, b_nd, first_u8, mask, off, heads, rows, row_off, None)
+
+
+def attention_ring_plan(Q, k, v, R, b_nd, first_u8, mask, off, heads, rows=None, row_off=None, plan_batch=1):
+    """`attention_ring` with the long band's cluster split of a call of `plan_batch` rows (the batch-invariant mode)."""
+    return _attention_ring(Q, k, v, R, b_nd, first_u8, mask, off, heads, rows, row_off, plan_batch)
+
+
+def _attention_ring(Q, k, v, R, b_nd, first_u8, mask, off, heads, rows, row_off, plan_batch):
     ops._cuda(Q, k, v, R, b_nd, first_u8, mask, off, rows, row_off)
     E, maxlen, h = k.shape
     _ring("attention_ring", k, v, mask, off, E, maxlen, h)
@@ -59,7 +68,15 @@ def attention_ring(Q, k, v, R, b_nd, first_u8, mask, off, heads, rows=None, row_
     if Q.dtype != BF16 or Q.numel() != B * h or not Q.is_contiguous():
         raise ValueError(f"attention_ring: Q must be contiguous bf16 with {B} rows of {h} (one step; got {Q.dtype} {tuple(Q.shape)})")
     out = torch.empty_like(Q)
-    if rows is None and row_off is None:
+    if plan_batch is not None and rows is None and row_off is None:
+        nat.check(nat.lib().vpt_attention_ring_plan(ops._p(Q), ops._p(k), ops._p(v), ops._p(R), R.stride(-2), ops._p(b_nd), ops._p(first_u8),
+                                                    first_u8.stride(0), ops._p(mask), ops._p(off), ops._p(out), B, maxlen, heads, b_nd.shape[0],
+                                                    plan_batch, ops._stream()), "vpt_attention_ring_plan")
+    elif plan_batch is not None:
+        nat.check(nat.lib().vpt_attention_ring_rows_plan(ops._p(Q), ops._p(k), ops._p(v), ops._p(R), R.stride(-2), ops._p(b_nd), ops._p(first_u8),
+                                                         first_u8.stride(0), ops._p(mask), ops._p(off), ops._p(rows), ops._p(row_off), ops._p(out),
+                                                         B, maxlen, heads, b_nd.shape[0], plan_batch, ops._stream()), "vpt_attention_ring_rows_plan")
+    elif rows is None and row_off is None:
         nat.check(nat.lib().vpt_attention_ring(ops._p(Q), ops._p(k), ops._p(v), ops._p(R), R.stride(-2), ops._p(b_nd), ops._p(first_u8),
                                                first_u8.stride(0), ops._p(mask), ops._p(off), ops._p(out), B, maxlen, heads, b_nd.shape[0],
                                                ops._stream()), "vpt_attention_ring")
@@ -87,3 +104,17 @@ def ring_advance_rows(row_off, rows, maxlen):
         raise ValueError(f"ring_advance_rows: row_off must be a contiguous int32 vector (got {row_off.dtype} {tuple(row_off.shape)})")
     nat.check(nat.lib().vpt_ring_advance_rows(ops._p(row_off), ops._p(rows), rows.numel(), maxlen, ops._stream()), "vpt_ring_advance_rows")
     ops._count()
+
+
+def ring_noise_keys(steps, rows, B):
+    """The sampling keys of a step of B batch rows (batch-invariant mode): int64 [B, 2], row b = (r, steps[r]) for its environment r =
+    rows[b] (r = b without `rows`), then steps[r] += 1 on the device; an inert row (rows[b] = -1) gets (-1, 0) and advances nothing."""
+    ops._cuda(steps, rows)
+    if steps.dtype != torch.int64 or steps.dim() != 1 or not steps.is_contiguous():
+        raise ValueError(f"ring_noise_keys: steps must be a contiguous int64 vector (got {steps.dtype} {tuple(steps.shape)})")
+    if rows is not None:
+        B = _rows("ring_noise_keys", rows, None, 0)
+    keys = torch.empty((B, 2), dtype=torch.int64, device=steps.device)
+    nat.check(nat.lib().vpt_ring_noise_keys(ops._p(steps), ops._p(rows), ops._p(keys), B, ops._stream()), "vpt_ring_noise_keys")
+    ops._count()
+    return keys

@@ -477,11 +477,17 @@ class RingState:
     Asynchronous rollouts step some of the ring's environments at a time through a view, `ring.rows(idx)` (`RingRows`).  They need one
     offset per environment: `row_off`, None (all zeros) until the first call that needs it allocates a device int32 (E,); memory row j of
     environment e is then at physical row (off + row_off[e] + j) % maxlen.  A step of the whole ring advances `off`, a step of a view
-    advances `row_off` of the rows it stepped."""
+    advances `row_off` of the rows it stepped.
+
+    In the batch-invariant mode (`MinecraftAgentPolicy.set_batch_invariant`) `act` samples environment e's step with the noise key
+    (stream e, step steps[e]): `steps` is None until the first such `act` allocates a device int64 (E,) of zeros, and each such `act`
+    advances it, on the device, for the environments it stepped (never for an inert row).  `to_pytree` / `load_` leave it alone; set it in
+    place (`ring.steps[e] = s`) to replay environment e from its step s."""
 
     def __init__(self, k, v, mask, off, row_off=None):
         self.k, self.v, self.mask, self.off = k, v, mask, off  # per layer: bf16 (E, maxlen, h) x 2, bool (E, maxlen); int32 (1,)
         self.row_off = row_off  # None or int32 (E,), each in [0, maxlen)
+        self.steps = None  # None or int64 (E,): the batch-invariant mode's per-environment sampling step
 
     @staticmethod
     def _net(policy):
@@ -522,6 +528,11 @@ class RingState:
         if self.row_off is None:
             self.row_off = torch.zeros((self.batch_size,), dtype=torch.int32, device=self.off.device)
         return self.row_off
+
+    def _alloc_steps(self):
+        if self.steps is None:
+            self.steps = torch.zeros((self.batch_size,), dtype=torch.int64, device=self.off.device)
+        return self.steps
 
     def rows(self, idx) -> "RingRows":
         """A view of the environments `idx` (a 1-D integer sequence, CPU or CUDA tensor) for a t = 1 step of those only: row i of the
@@ -822,13 +833,18 @@ class MinecraftPolicy(nn.Module):
     # -- CNN -----------------------------------------------------------------------------------------------
     # Activations are kept in the "ZP" layout [F][H+1][W+1][C] (zero last row / column; include/vpt_b200.h): it lets the
     # conv kernel address every 3x3 neighbour linearly and reuse one shared-memory input span for all nine taps.
-    def _cnn_chunk(self, img, prep: _Prepared, out, pfx="img_process.cnn", train=False, stacks=None, record_from=0):
+    def _cnn_chunk(self, img, prep: _Prepared, out, pfx="img_process.cnn", train=False, stacks=None, record_from=0, plan_frames=None):
         """lib/impala_cnn.py:187-195 for a chunk of frames; writes the last stack's output (ZP [F, Hf+1, Wf+1, C2] bf16) into
         `out` and returns (out, per-frame stats).
         train: the training layout (no stack-norm fold; each residual branch's output `r` kept apart, then `add_zp`), which the
         backward's recompute of a chunk reproduces bit for bit.  stacks: a list that receives, per stack, what the backward needs
-        (training layout only; None records nothing), or None for the stacks below `record_from`, which the backward does not enter."""
+        (training layout only; None records nothing), or None for the stacks below `record_from`, which the backward does not enter.
+        plan_frames: the convolutions and pools run the launch plan of a chunk of that many frames (None: the chunk's own)."""
         cfg = self.cfg
+        conv, pool = ops.conv3x3_zp, ops.maxpool3s2
+        if plan_frames is not None:
+            conv = functools.partial(ops.conv3x3_zp_plan, plan_frames=plan_frames)
+            pool = functools.partial(ops.maxpool3s2_plan, plan_frames=plan_frames)
         H, W = cfg.img_shape[0], cfg.img_shape[1]
         x, mr = None, None
         assert train or stacks is None
@@ -843,8 +859,8 @@ class MinecraftPolicy(nn.Module):
                 y1, mr1, chan = ops.firstconv_pool(img, st["fc_w"], st["fc_b"], c, zp=True, want_chan=True)
             else:
                 Wb, S1, S2 = st["first"]
-                full, _ = ops.conv3x3_zp(x, Wb, H, W, mr=mr, S1=S1, S2=S2, relu=1, want_stats=False)
-                y1, mr1, chan = ops.maxpool3s2(full, zp=True, want_chan=True)
+                full, _ = conv(x, Wb, H, W, mr=mr, S1=S1, S2=S2, relu=1, want_stats=False)
+                y1, mr1, chan = pool(full, zp=True, want_chan=True)
                 if rec is not None:
                     rec["full"] = full
                 del full
@@ -855,10 +871,10 @@ class MinecraftPolicy(nn.Module):
                 Wb0, tabs = st["conv0n"]
                 mrE, Ef, rs, rb = ops.norm2_fold(chan, H * W, st["n_g"], st["n_b"], tabs)
                 del chan
-                hmid, mrh = ops.conv3x3_zp(y1, Wb0, H, W, mr=mrE, Ef=Ef, relu=1)
+                hmid, mrh = conv(y1, Wb0, H, W, mr=mrE, Ef=Ef, relu=1)
                 self._tap(f"{pfx}.stacks.{i}.blocks.0.conv0", hmid)
                 Wb, S1, S2 = st["convs"][1]
-                x, mr = ops.conv3x3_zp(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, residual=y1, res_scale=rs, res_shift=rb)
+                x, mr = conv(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, residual=y1, res_scale=rs, res_shift=rb)
                 del y1, hmid
                 self._tap(f"{pfx}.stacks.{i}.blocks.0", x)
                 first_block = 1
@@ -873,16 +889,16 @@ class MinecraftPolicy(nn.Module):
                 first_block = 0
             for j in range(first_block, 2):
                 Wb, S1, S2 = st["convs"][2 * j]
-                hmid, mrh = ops.conv3x3_zp(x, Wb, H, W, mr=mr, S1=S1, S2=S2, relu=1)
+                hmid, mrh = conv(x, Wb, H, W, mr=mr, S1=S1, S2=S2, relu=1)
                 self._tap(f"{pfx}.stacks.{i}.blocks.{j}.conv0", hmid)
                 Wb, S1, S2 = st["convs"][2 * j + 1]
                 last = (i == len(cfg.chans) - 1) and j == 1
                 if not train:
-                    x, mr = ops.conv3x3_zp(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, residual=x, out=out if last else None)
+                    x, mr = conv(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, residual=x, out=out if last else None)
                 else:
                     # training: the branch output r = relu(conv1(..)) is kept on its own (its sign pattern IS the ReLU mask the
                     # backward needs; x + r rounded to bf16 no longer shows which small r were positive), then added
-                    r, _ = ops.conv3x3_zp(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, want_stats=False)
+                    r, _ = conv(hmid, Wb, H, W, mr=mrh, S1=S1, S2=S2, relu=1, want_stats=False)
                     x, mr = ops.add_zp(x, r, H, W, out=out if last else None)
                     if rec is not None:
                         rec["blocks"].append(dict(h=hmid, mrh=mrh, r=r, x=x, mr=mr))
@@ -894,7 +910,8 @@ class MinecraftPolicy(nn.Module):
 
     # -- transformer -----------------------------------------------------------------------------------------
     def _linear(self, x, fold, N, *, mr=None, relu=0, residual=None, out=None, out_dtype=None, seg=None, want_stats=False,
-                out_scale=1.0, ld_out=None):
+                out_scale=1.0, ld_out=None, rowwise=False):
+        """rowwise: every row computed as a one-row call computes it (`ops.gemm_rowwise`, the batch-invariant mode)."""
         Wb, S1, S2 = fold
         M, K = x.shape[0], x.shape[1]
         if out is None:
@@ -902,14 +919,19 @@ class MinecraftPolicy(nn.Module):
         part, P = None, ops.gemm_stat_parts(N)
         if want_stats:
             part = torch.empty((M, P, 2), dtype=F32, device=x.device)
-        ops.gemm(x, Wb, out, M, N, K, mr=mr, rows_per_group=1, S1=S1 if mr is not None else None, S2=S2, relu=relu,
-                 residual=residual, seg=seg, stat_part=part, stat_mode=1 if want_stats else 0, out_scale=out_scale, ld_out=ld_out)
+        (ops.gemm_rowwise if rowwise else ops.gemm)(x, Wb, out, M, N, K, mr=mr, rows_per_group=1, S1=S1 if mr is not None else None, S2=S2,
+                                                    relu=relu, residual=residual, seg=seg, stat_part=part, stat_mode=1 if want_stats else 0,
+                                                    out_scale=out_scale, ld_out=ld_out)
         mr_out = ops.stats_finalize(part, M, P, N) if want_stats else None
         return out, mr_out
 
-    def _block(self, l, x, mr_x, first_u8, state, B, t, prep: _Prepared, last: bool):
+    def _block(self, l, x, mr_x, first_u8, state, B, t, prep: _Prepared, last: bool, inv: bool = False):
         """lib/util.py:193-211: x_hat = LN(x); y = x_hat + Proj(Attn(x_hat)); z = y + mlp1(relu(mlp0(LN(y)))).
-        state: the layer's (mask, (K, V)), or a RingState or RingRows (t = 1), updated in place (returns None for the state)."""
+        state: the layer's (mask, (K, V)), or a RingState or RingRows (t = 1), updated in place (returns None for the state).
+        inv: the batch-invariant mode (t = 1): row-wise GEMMs and the attention's one-row plan."""
+        gemm, attention, attention_ring = ops.gemm, ops.attention, ops.attention_ring
+        if inv:
+            gemm, attention, attention_ring = ops.gemm_rowwise, ops.attention_plan, ops.attention_ring_plan
         cfg, L = self.cfg, prep.layers[l]
         h, heads, maxlen = cfg.hidsize, cfg.heads, cfg.maxlen
         causal = cfg.mask_style == "clipped_causal"
@@ -942,38 +964,38 @@ class MinecraftPolicy(nn.Module):
                 R = torch.empty((B * t, NBASIS * heads), dtype=F32, device=x.device)
                 dsts.append((3 * h, R, NBASIS * heads, False))
             Wc, _, bc = L["qkvr"]
-            ops.gemm(xhat, Wc, q, B * t, Wc.shape[0], h, S2=bc, seg=seg, dsts=dsts)
+            gemm(xhat, Wc, q, B * t, Wc.shape[0], h, S2=bc, seg=seg, dsts=dsts)
         else:  # hidsize not a multiple of the N tile: four launches
-            q, _ = self._linear(xhat, L["q"], h)
-            self._linear(xhat, L["k"], h, out=full_k, seg=seg, ld_out=h)
-            self._linear(xhat, L["v"], h, out=full_v, seg=seg, ld_out=h)
+            q, _ = self._linear(xhat, L["q"], h, rowwise=inv)
+            self._linear(xhat, L["k"], h, out=full_k, seg=seg, ld_out=h, rowwise=inv)
+            self._linear(xhat, L["v"], h, out=full_v, seg=seg, ld_out=h, rowwise=inv)
             if causal:
-                R, _ = self._linear(xhat, L["r"], NBASIS * heads, out_dtype=F32)
+                R, _ = self._linear(xhat, L["r"], NBASIS * heads, out_dtype=F32, rowwise=inv)
         if ring is not None:
             # a view steps some environments: batch row b is ring row idx[b] (-1: an inert row)
             rr, rows = (ring.ring, ring.idx) if isinstance(ring, RingRows) else (ring, None)
             # the step's rows go to their ring slot first: it held memory key 0, which a t = 1 query does not see
             if rr.row_off is None:  # every row at `off`
                 ops.ring_write(full_k, full_v, rr.k[l], rr.v[l], rr.mask[l], rr.off, first_u8)
-                a = ops.attention_ring(q, rr.k[l], rr.v[l], R, L["b_nd"], first_u8, rr.mask[l], rr.off, heads)
+                a = attention_ring(q, rr.k[l], rr.v[l], R, L["b_nd"], first_u8, rr.mask[l], rr.off, heads)
             else:
                 ops.ring_write(full_k, full_v, rr.k[l], rr.v[l], rr.mask[l], rr.off, first_u8, rows=rows, row_off=rr.row_off)
-                a = ops.attention_ring(q, rr.k[l], rr.v[l], R, L["b_nd"], first_u8, rr.mask[l], rr.off, heads, rows=rows, row_off=rr.row_off)
+                a = attention_ring(q, rr.k[l], rr.v[l], R, L["b_nd"], first_u8, rr.mask[l], rr.off, heads, rows=rows, row_off=rr.row_off)
             new_state = None
         else:
             smask_u8 = state_mask.contiguous().view(torch.uint8) if state_mask is not None else None
-            a = ops.attention(q, full_k, full_v, R, L["b_nd"], first_u8, smask_u8, B, t, maxlen, heads, causal=causal)
+            a = attention(q, full_k, full_v, R, L["b_nd"], first_u8, smask_u8, B, t, maxlen, heads, causal=causal)
             # new state (lib/xf.py:380-381: last `maxlen` rows of full; lib/masked_attention.py:86-92)
             new_k = torch.empty((B, maxlen, h), dtype=F32, device=x.device)
             new_v = torch.empty((B, maxlen, h), dtype=F32, device=x.device)
             ops.copy_rows2(full_k, full_v, T - maxlen, new_k, new_v, 0, maxlen)
             new_mask = ops.state_mask_update(smask_u8, first_u8, t, maxlen) if causal else state_mask
             new_state = (new_mask, (new_k, new_v))
-        y, mr_y = self._linear(a, L["proj"], h, residual=xhat, want_stats=True)
+        y, mr_y = self._linear(a, L["proj"], h, residual=xhat, want_stats=True, rowwise=inv)
         self._tap(f"recurrent_layer.blocks.{l}.attn", y)
-        hmid, _ = self._linear(y, L["mlp0"], h * cfg.pointwise_ratio, mr=mr_y, relu=1)
+        hmid, _ = self._linear(y, L["mlp0"], h * cfg.pointwise_ratio, mr=mr_y, relu=1, rowwise=inv)
         # the F.relu of lib/policy.py:211 is fused into the last block's epilogue (relu after the residual add)
-        z, mr_z = self._linear(hmid, L["mlp1"], h, residual=y, relu=2 if last else 0, want_stats=True)
+        z, mr_z = self._linear(hmid, L["mlp1"], h, residual=y, relu=2 if last else 0, want_stats=True, rowwise=inv)
         if not last:
             self._tap(f"recurrent_layer.blocks.{l}", z)
         if self._tape is not None:  # (None for a block below the backward's lowest unit)
@@ -1025,8 +1047,9 @@ class MinecraftPolicy(nn.Module):
 
     # -- whole net -------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def _forward_impl(self, img, first, state_in):
-        """img: frames (B, T, H, W, 3), or FrameLatents (B, T): the CNN part is then skipped."""
+    def _forward_impl(self, img, first, state_in, invariant: bool = False):
+        """img: frames (B, T, H, W, 3), or FrameLatents (B, T): the CNN part is then skipped.  invariant: the batch-invariant mode of a
+        one-frame inference call (`MinecraftAgentPolicy.set_batch_invariant`): every launch runs the plan of a one-row call."""
         cfg = self.cfg
         latents = isinstance(img, FrameLatents)
         if latents:
@@ -1065,10 +1088,10 @@ class MinecraftPolicy(nn.Module):
         else:
             frames = img.reshape(N, *frame_shape).contiguous()
             first_u8 = first.to(device=img.device, dtype=torch.bool).contiguous().view(torch.uint8)
-            xd, mr_d = self._cnn_part(frames, t, prep, train=tape is not None)
+            xd, mr_d = self._cnn_part(frames, t, prep, train=tape is not None, inv=invariant)
         if tape is not None:
             tape.update(first_u8=first_u8)
-        return self._upper_part(xd, mr_d, first_u8, state_in, B, t, prep)
+        return self._upper_part(xd, mr_d, first_u8, state_in, B, t, prep, inv=invariant)
 
     def _batch_plan_frames(self, t):
         """Frames per CNN chunk from which every launch plan of this net's CNN is the one of a full chunk (`ops.cnn_batch_plan_frames`);
@@ -1084,10 +1107,10 @@ class MinecraftPolicy(nn.Module):
         n = ops.cnn_batch_plan_frames(tuple(stacks), max(t, self.idm_chunk_frames // t * t))
         return -(-n // t) * t
 
-    def _cnn_part(self, frames, t, prep: _Prepared, train: bool):
+    def _cnn_part(self, frames, t, prep: _Prepared, train: bool, inv: bool = False):
         """frames [N, H, W, 3] (whole sequences of t frames) -> (xd bf16 [N, cnn_outsize], mr_d fp32 [N, 2]): the conv3d pre-stage (IDM),
         the ImpalaCNN in frame chunks and the dense layer.  train: the training layout (`_cnn_chunk`); with a tape (self._tape) it also
-        records what the backward needs."""
+        records what the backward needs.  inv: the batch-invariant mode (inference): every chunk runs the plan of one frame."""
         cfg = self.cfg
         N = frames.shape[0]
         frame_shape = tuple(frames.shape[1:])
@@ -1124,11 +1147,11 @@ class MinecraftPolicy(nn.Module):
             if cfg.conv3d_out is not None:
                 chunk = chunk.view(Fr // t, t, *frame_shape)
             _, mr = self._cnn_chunk(chunk, prep, cnn_out[f0:f0 + Fr], train=train, stacks=stacks,
-                                    record_from=0 if tape is None else tape["stacks_from"])
+                                    record_from=0 if tape is None else tape["stacks_from"], plan_frames=1 if inv else None)
             mrs.append(mr)
         mr_c = mrs[0] if len(mrs) == 1 else torch.cat(mrs, 0)
         Kd = (Hf + 1) * (Wf + 1) * C2  # ZP rows flattened; the zero row / column meets zero weight columns
-        xd, mr_d = self._linear(cnn_out.view(Nr, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True)
+        xd, mr_d = self._linear(cnn_out.view(Nr, Kd), prep.dense, cfg.cnn_outsize, mr=mr_c, relu=1, want_stats=True, rowwise=inv)
         if Nr > N:
             cnn_out, mr_c, xd, mr_d = cnn_out[:N], mr_c[:N], xd[:N], mr_d[:N]
         if tape is not None:
@@ -1137,13 +1160,13 @@ class MinecraftPolicy(nn.Module):
                         cnn_chunks=[(f0, min(f0 + step, N)) for f0 in range(0, N, step)] if cnn_bwd else [])
         return xd, mr_d
 
-    def _upper_part(self, xd, mr_d, first_u8, state_in, B, t, prep: _Prepared):
+    def _upper_part(self, xd, mr_d, first_u8, state_in, B, t, prep: _Prepared, inv: bool = False):
         """(xd, mr_d) of `_cnn_part` or of cached latents -> img_process.linear -> the transformer -> lastlayer -> final_ln:
         (latent bf16 [N, h], latent fp32 (B, t, h), state_out).  Records into the tape (self._tape) when there is one."""
         cfg = self.cfg
         tape = self._tape
         self._tap("img_process.cnn.dense", xd)
-        x, mr_x = self._linear(xd, prep.linear, cfg.hidsize, mr=mr_d, relu=1, want_stats=True)
+        x, mr_x = self._linear(xd, prep.linear, cfg.hidsize, mr=mr_d, relu=1, want_stats=True, rowwise=inv)
         self._tap("img_process", x)
         if tape is not None:
             tape.update(x0=x, mr_x0=mr_x)
@@ -1151,7 +1174,7 @@ class MinecraftPolicy(nn.Module):
         ring = isinstance(state_in, _RING_STATES)
         state_out = state_in if ring else []
         for l in range(cfg.n_layers):
-            x, mr_x, s = self._block(l, x, mr_x, first_u8, state_in if ring else state_in[l], B, t, prep, last=(l == cfg.n_layers - 1))
+            x, mr_x, s = self._block(l, x, mr_x, first_u8, state_in if ring else state_in[l], B, t, prep, last=(l == cfg.n_layers - 1), inv=inv)
             if not ring:
                 state_out.append(s)
         # every layer has written its row at its slot: the next step's oldest row is one further on
@@ -1162,7 +1185,7 @@ class MinecraftPolicy(nn.Module):
         # x is relu(recurrent output) here
         if self.use_lastlayer:
             z_last, mr_zl = x, mr_x
-            x, mr_x = self._linear(x, prep.last, cfg.hidsize, mr=mr_x, relu=1, want_stats=True)
+            x, mr_x = self._linear(x, prep.last, cfg.hidsize, mr=mr_x, relu=1, want_stats=True, rowwise=inv)
             if tape is not None:
                 tape.update(z_last=z_last, mr_zl=mr_zl, xl=x, mr_xl=mr_x)
         lat_bf16, lat_f32, _ = ops.affine_norm(x, mr_x, prep.fin_g, prep.fin_b, rows_per_group=1, want_f32=True)
@@ -1391,8 +1414,8 @@ class _PolicyBase(nn.Module):
         return {**super().__getstate__(), "_relayout": None, "_relayout_seen": 0}  # a copy captures its own graph (a CUDA graph cannot be copied)
 
     @torch.no_grad()
-    def _heads(self, lat_bf16, B, t, mask=None):
-        """lib/action_head.py:163-174 for every head + lib/scaled_mse_head.py:34-35."""
+    def _heads(self, lat_bf16, B, t, mask=None, rowwise=False):
+        """lib/action_head.py:163-174 for every head + lib/scaled_mse_head.py:34-35.  rowwise: the batch-invariant mode's GEMMs."""
         if isinstance(lat_bf16, tuple):  # fp32-parity mode: (latent hi, latent lo)
             from . import precise
             return precise.heads(self, lat_bf16, B, t, mask)
@@ -1401,7 +1424,7 @@ class _PolicyBase(nn.Module):
         ntot = hp["ntot"]
         ld = (ntot + 7) // 8 * 8
         raw = torch.empty((N, ld), dtype=F32, device=lat_bf16.device)
-        self.net._linear(lat_bf16, hp["pi"], ntot, out=raw, out_scale=1.0 / self.temperature, ld_out=ld)
+        self.net._linear(lat_bf16, hp["pi"], ntot, out=raw, out_scale=1.0 / self.temperature, ld_out=ld, rowwise=rowwise)
         pd = OrderedDict()
         for name, (shape, n) in self.head_specs.items():
             c0, width = hp["cols"][name]
@@ -1418,7 +1441,7 @@ class _PolicyBase(nn.Module):
             pd[name] = lp.view(B, t, *shape, n)
         if not self.has_value_head:
             return pd, None
-        vpred, _ = self.net._linear(lat_bf16, hp["v"], 1, out_dtype=F32)
+        vpred, _ = self.net._linear(lat_bf16, hp["v"], 1, out_dtype=F32, rowwise=rowwise)
         return pd, vpred.view(B, t, 1)
     # -- distribution helpers (lib/action_head.py:176-220, 250-260): the reference's policy calls them on its pi_head --------------
     def sample(self, pd, deterministic: bool = False):
@@ -1461,10 +1484,13 @@ class _CategoricalActionHead(_Node):
             lp = lp.sum(dim=-1)
         return lp
 
-    def sample(self, logits, deterministic: bool = False):
+    def sample(self, logits, deterministic: bool = False, keys=None, seed: int = 0, head: int = 0):
         """Gumbel-max sample (or the argmax); `torch.rand_like` supplies the uniforms so the Philox stream is consumed exactly like the
-        reference's (lib/action_head.py:200)."""
+        reference's (lib/action_head.py:200).  keys: device int64 (rows, 2) of (stream, step), one per row of the head's logits: the
+        counter-based noise of `ops.gumbel_argmax_keyed` under `seed`, with `head` the head's index (the batch-invariant mode)."""
         lg = logits.contiguous()
+        if keys is not None and not deterministic:
+            return ops.gumbel_argmax_keyed(lg, keys, seed, head)
         u = None if deterministic else torch.rand_like(lg)
         return ops.gumbel_argmax(lg, u)
 
@@ -1523,8 +1549,11 @@ class _DictActionHead(_Node):
     def logprob(self, actions, logits):
         return self._sum(head.logprob(actions[k], logits[k]) for k, head in self.items())
 
-    def sample(self, logits, deterministic: bool = False):
-        return OrderedDict((k, head.sample(logits[k], deterministic)) for k, head in self.items())
+    def sample(self, logits, deterministic: bool = False, keys=None, seed: int = 0):
+        """keys, seed: `_CategoricalActionHead.sample`; head i (in this dict's order) draws with head index i."""
+        if keys is None:
+            return OrderedDict((k, head.sample(logits[k], deterministic)) for k, head in self.items())
+        return OrderedDict((k, head.sample(logits[k], deterministic, keys=keys, seed=seed, head=i)) for i, (k, head) in enumerate(self.items()))
 
     def entropy(self, logits):
         return self._sum(head.entropy(logits[k]) for k, head in self.items())
@@ -1596,6 +1625,44 @@ class MinecraftAgentPolicy(_PolicyBase):
         self.net = MinecraftPolicy(**policy_kwargs)
         self._init_heads(action_space, pi_head_kwargs)
         self._denorm = _Versioned(self.value_head.normalizer.parameters, self._build_denorm)
+        self.batch_invariant, self.noise_seed = False, 0
+
+    def set_batch_invariant(self, on: bool = True, seed: int = 0):
+        """The batch-invariant mode of one-frame inference steps (`act`, `v`, `get_output_for_observation`, `forward` with T = 1; frames or
+        latents; a pytree state, a RingState or a view; eager or through `GraphedAct`).  Every output of a row (pd, vpred, log_prob, the
+        K / V row and mask it stores) then equals, bit for bit, the default-mode B = 1 step of that environment alone, whatever the batch,
+        the row's position, the other rows and the padding: every launch runs the plan of a one-row call.  A sampled action comes from
+        counter-based noise keyed by (seed, stream, step, head, column) (`ops.gumbel_argmax_keyed`): a ring's step of environment e uses
+        (e, RingState.steps[e]), a pytree `act` the caller's `noise_keys`.  Read when a call runs.  The differentiable forward and the
+        trainers ignore it.  Returns the policy."""
+        self.batch_invariant, self.noise_seed = bool(on), int(seed)
+        return self
+
+    def _invariant_call(self, t, differentiable: bool):
+        """Whether a forward call runs in the batch-invariant mode; raises, before any launch, for one the mode cannot serve."""
+        if not self.batch_invariant or differentiable:
+            return False
+        if self.net.precision != "bf16":
+            raise NotImplementedError("the batch-invariant mode runs in the bf16 mode only (set_precision('bf16'))")
+        if t != 1:
+            raise ValueError(f"the batch-invariant mode is for one-frame steps (T = 1, got T = {t})")
+        return True
+
+    def _check_noise_keys(self, B, state_in, sample: bool, noise_keys):
+        """Raises, before any launch, for `noise_keys` an `act` call cannot take or a keyed sample without them."""
+        if noise_keys is not None:
+            if not self.batch_invariant:
+                raise ValueError("noise_keys are for the batch-invariant mode (set_batch_invariant)")
+            if isinstance(state_in, _RING_STATES):
+                raise ValueError("a ring step samples with the keys of RingState.steps: noise_keys are for a pytree state")
+            if (not torch.is_tensor(noise_keys) or noise_keys.dtype != torch.int64 or tuple(noise_keys.shape) != (B, 2)
+                    or not noise_keys.is_contiguous()):
+                raise ValueError(f"noise_keys must be a contiguous CUDA int64 ({B}, 2) of (stream, step) (got "
+                                 f"{getattr(noise_keys, 'dtype', type(noise_keys))} {tuple(getattr(noise_keys, 'shape', ()))})")
+            ops.require_cuda(noise_keys)
+        elif self.batch_invariant and sample and not isinstance(state_in, _RING_STATES):
+            raise ValueError("a stochastic act on a pytree state in the batch-invariant mode needs noise_keys, (B, 2) of (stream, step): "
+                             "keys from the row's position would make its action depend on the batch")
 
     def forward(self, obs, first: torch.Tensor, state_in):
         """lib/policy.py:252-269 -> ((pi_logits, vpred, None), state_out)."""
@@ -1607,13 +1674,14 @@ class MinecraftAgentPolicy(_PolicyBase):
         img = _ob_input(obs)
         if isinstance(state_in, _RING_STATES):
             _check_ring_call(self.net, img, state_in, _differentiable(self, img))
+        inv = self._invariant_call(img.shape[1], _differentiable(self, img))
         if _differentiable(self, img):
             outs, state_out = _autograd_runner(self).run(img, first, state_in, mask)
             pi_logits = OrderedDict(zip(self.head_specs, outs[:-1]))
             return (pi_logits, outs[-1], None), state_out
-        lat_bf16, _, state_out = self.net._forward_impl(img, first, state_in)
+        lat_bf16, _, state_out = self.net._forward_impl(img, first, state_in, invariant=inv)
         B, t = img.shape[:2]
-        pi_logits, vpred = self._heads(lat_bf16, B, t, mask)
+        pi_logits, vpred = self._heads(lat_bf16, B, t, mask, rowwise=inv)
         return (pi_logits, vpred, None), state_out
 
     def denormalize(self, v):
@@ -1647,12 +1715,20 @@ class MinecraftAgentPolicy(_PolicyBase):
         return pd, self.denormalize(vpred)[:, 0], state_out
 
     @torch.no_grad()
-    def act(self, obs, first, state_in, stochastic: bool = True, taken_action=None, return_pd=False):
-        """lib/policy.py:307-328."""
+    def act(self, obs, first, state_in, stochastic: bool = True, taken_action=None, return_pd=False, noise_keys=None):
+        """lib/policy.py:307-328.  noise_keys: the batch-invariant mode's sampling keys for a pytree state, a CUDA int64 (B, 2) of
+        (stream, step) per row (`set_batch_invariant`; a ring step takes (e, RingState.steps[e]) and advances `steps`)."""
+        self._check_noise_keys(first.shape[0], state_in, stochastic and taken_action is None, noise_keys)
         obs = {k: v.unsqueeze(1) for k, v in obs.items()}
         first = first.unsqueeze(1)
         (pd, vpred, _), state_out = self(obs=obs, first=first, state_in=state_in)
-        if taken_action is None:
+        keys = noise_keys
+        if self.batch_invariant and isinstance(state_in, _RING_STATES):
+            ring, rows = (state_in.ring, state_in.idx) if isinstance(state_in, RingRows) else (state_in, None)
+            keys = ops.ring_noise_keys(ring._alloc_steps(), rows, ring.batch_size)
+        if taken_action is None and keys is not None:
+            ac = self.pi_head.sample(pd, deterministic=not stochastic, keys=keys, seed=self.noise_seed)
+        elif taken_action is None:
             ac = self.sample(pd, deterministic=not stochastic)
         else:
             ac = {k: v.unsqueeze(1) for k, v in taken_action.items()}
@@ -1734,7 +1810,11 @@ class GraphedAct:
     1 <= k <= batch_size: `step(obs_k, first_k, step.state.rows(idx))` with len(idx) = k.  The call pads its static buffers to batch_size
     rows with inert rows (-1, zero frames, first False), so one graph per `stochastic` serves every subset without a host sync, and
     returns the view with the first k rows of the outputs.  It takes only views of its own `state`: install a state with
-    `step.state.load_(...)` or `step.state.rows(idx).load_(...)`."""
+    `step.state.load_(...)` or `step.state.rows(idx).load_(...)`.
+
+    In the batch-invariant mode (`set_batch_invariant`) a graph computes every row as the eager B = 1 step computes it, and a ring samples
+    with the keys of `state.steps`, which the graph advances.  A pytree graph's stochastic call takes `noise_keys` (B, 2) as `act` does.
+    Graphs are keyed on the mode and the seed: toggling either captures again."""
 
     def __init__(self, policy: "MinecraftAgentPolicy", batch_size: int, pdl: bool = False, memory: str = "pytree",
                  envs: Optional[int] = None):
@@ -1752,6 +1832,7 @@ class GraphedAct:
         H, W = cfg.img_shape[0], cfg.img_shape[1]
         self.img = torch.zeros((B, H, W, 3), dtype=torch.uint8, device=dev)
         self.first = torch.zeros((B,), dtype=torch.bool, device=dev)
+        self.noise_keys = torch.zeros((B, 2), dtype=torch.int64, device=dev)  # a pytree graph's keys in the batch-invariant mode
         if envs is not None:
             self.state = RingState.zeros(policy, envs)
             self.state._alloc_row_off()
@@ -1767,10 +1848,10 @@ class GraphedAct:
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):  # warm-up outside capture (lazy function attributes, allocator pools)
-            for _ in range(2):
-                policy.act({"img": self.img}, self.first, self.state if envs is None else self._view)  # (a view: inert rows only)
+            for _ in range(2):  # (a view: inert rows only)
+                policy.act({"img": self.img}, self.first, self.state if envs is None else self._view, noise_keys=self._keys_arg(True))
             if memory == "ring" and envs is None:  # the warm-up stepped the ring in place: back to the empty state
-                for buf in self.state.k + self.state.v + self.state.mask + [self.state.off]:
+                for buf in self.state.k + self.state.v + self.state.mask + [self.state.off] + [x for x in [self.state.steps] if x is not None]:
                     buf.zero_()
         torch.cuda.current_stream(dev).wait_stream(side)
         self.graphs = {}
@@ -1782,7 +1863,12 @@ class GraphedAct:
         pol = self.policy
         return pol.net.prepared(), pol._heads_prepared(), pol._denorm.get()
 
+    def _keys_arg(self, stochastic: bool):
+        return self.noise_keys if self.policy.batch_invariant and self.memory == "pytree" and stochastic else None
+
     def _capture(self, stochastic: bool):
+        if self.policy.batch_invariant and self.memory == "ring":
+            self.state._alloc_steps()  # (outside the capture: the graph advances it in place)
         g = torch.cuda.CUDAGraph()
         # optional programmatic dependent launch: with the attribute the next kernel is scheduled while the previous one drains
         # (csrc/common.cuh pdl_sync).  Measured neutral for this graph (0.953 vs 0.957 ms), hence off by default.
@@ -1790,7 +1876,8 @@ class GraphedAct:
         try:
             with torch.cuda.graph(g):
                 state = self.state if self.envs is None else self._view
-                ac, st, res = self.policy.act({"img": self.img}, self.first, state, stochastic=stochastic, return_pd=True)
+                ac, st, res = self.policy.act({"img": self.img}, self.first, state, stochastic=stochastic, return_pd=True,
+                                              noise_keys=self._keys_arg(stochastic))
                 if self.memory == "pytree":
                     for (m_in, (k_in, v_in)), (m_out, (k_out, v_out)) in zip(self.state, st):  # roll the state inside the graph
                         m_in.copy_(m_out)
@@ -1811,10 +1898,22 @@ class GraphedAct:
         return ac, res
 
     def _key(self, stochastic: bool):
-        # a ring given per-row offsets (copied in from a ring that has them) runs other kernels than the graph captured without them
-        return stochastic, self.memory == "ring" and self.state.row_off is not None
+        # a ring given per-row offsets (copied in from a ring that has them) runs other kernels than the graph captured without them; the
+        # batch-invariant mode runs other kernels, samples under its seed, and advances the ring's `steps` through its address
+        key = stochastic, self.memory == "ring" and self.state.row_off is not None
+        pol = self.policy
+        if not pol.batch_invariant:
+            return key
+        steps = self.state.steps.data_ptr() if self.memory == "ring" and self.state.steps is not None else None
+        return key + (pol.noise_seed, steps)
 
-    def _call_rows(self, obs, first, view, stochastic: bool, return_pd: bool):
+    def _check_invariant(self, stochastic: bool, noise_keys):
+        """The batch-invariant mode's refusals of `act` (its T = 1 and fp32 rules, `noise_keys`), before any copy."""
+        pol = self.policy
+        pol._invariant_call(1, False)
+        pol._check_noise_keys(self.B, self.state if self.memory == "ring" else None, stochastic, noise_keys)
+
+    def _call_rows(self, obs, first, view, stochastic: bool, return_pd: bool, noise_keys=None):
         """envs=E: step the k environments of `view` as rows 0..k-1 of the graph, inert rows after them."""
         if not isinstance(view, RingRows) or view.ring is not self.state:
             raise ValueError("GraphedAct(envs=E) steps views of its own ring, `step.state.rows(idx)`; install other states with "
@@ -1824,6 +1923,7 @@ class GraphedAct:
             raise ValueError(f"GraphedAct: a view of {k} rows for a graph of batch size {B}")
         if obs["img"].shape[0] != k or first.shape[0] != k:
             raise ValueError(f"GraphedAct: {obs['img'].shape[0]} frames and {first.shape[0]} `first` flags for a view of {k} rows")
+        self._check_invariant(stochastic, noise_keys)
         self.idx[:k].copy_(view.idx)
         self.img[:k].copy_(obs["img"])
         self.first[:k].copy_(first)
@@ -1838,13 +1938,16 @@ class GraphedAct:
         return {n: x[:k] for n, x in ac.items()}, view, out
 
     @torch.no_grad()
-    def __call__(self, obs, first, state_in, stochastic: bool = True, taken_action=None, return_pd: bool = False):
+    def __call__(self, obs, first, state_in, stochastic: bool = True, taken_action=None, return_pd: bool = False, noise_keys=None):
         if taken_action is not None:
             raise NotImplementedError("GraphedAct: taken_action is only supported by the eager act()")
         if self.envs is not None:
-            return self._call_rows(obs, first, state_in, stochastic, return_pd)
+            return self._call_rows(obs, first, state_in, stochastic, return_pd, noise_keys)
         if isinstance(state_in, RingRows):
             raise ValueError("GraphedAct: a view of a ring needs GraphedAct(..., memory='ring', envs=E)")
+        self._check_invariant(stochastic, noise_keys)
+        if noise_keys is not None:
+            self.noise_keys.copy_(noise_keys)
         self.img.copy_(obs["img"])
         self.first.copy_(first)
         if state_in is not self.state and self.memory == "ring":
