@@ -382,6 +382,19 @@ int vpt_resize_bilinear_u8(const uint8_t* src, uint8_t* dst, const int32_t* xidx
  * clipped at the right / bottom border; xy[f].x < 0 = no cursor.  cursor u8 [ch][cw][3], alpha f64 [ch][cw]. */
 int vpt_composite_cursor_u8(uint8_t* frames, const uint8_t* cursor, const double* alpha, const int32_t* xy, int32_t F, int32_t H, int32_t W,
                             int32_t ch, int32_t cw, void* stream);
+/* Training-time augmentation (agent.py augment_frames): src u8 [F][H][W][3] -> dst [F][H][W][3], u8 (out_f32 = 0) or fp32 on the uint8
+ * scale (out_f32 = 1).  params fp32 [F][10] per frame = (A[2][3], b, c, s, h), A the inverse affine map output pixel -> source point:
+ *   1. (u, v) = A . (x, y, 1) (pixel centres at integers; fp64 from the fp32 A), bilinear p00 + fx (p01 - p00) ..., 0 outside the frame
+ *   2. b != 1: p = clamp(b p, 0, 255)
+ *   3. c != 1: p = clamp(c p + (1 - c) m, 0, 255), m = frame mean of 0.299 R + 0.587 G + 0.114 B after step 2
+ *   4. s != 1: p = clamp(s p + (1 - s) grey(p), 0, 255)
+ *   5. h != 0: torchvision's RGB -> HSV on [0, 1], H = (H + h) mod 1, -> RGB, times 255, clamped
+ *   6. u8: round to nearest even; fp32: the clamped value
+ * fp32 per channel, one CTA per frame, fixed-order sums without atomics: a frame's output depends on its own bytes and parameters only.
+ * Refuses (VPT_ERR_ARG) a frame of more than vpt_augment_max_frame_bytes() bytes (3 H W), the shared memory a CTA can opt in to, less the
+ * kernel's own; vpt_augment_max_frame_bytes() is 0 without a device. */
+int vpt_augment_frames(const uint8_t* src, void* dst, int32_t out_f32, const float* params, int32_t F, int32_t H, int32_t W, void* stream);
+int vpt_augment_max_frame_bytes(void);
 
 /* ----------------------------------------------------------------------------------------------------------
  * BC step groundwork (behavioural_cloning.py:63-67,119-123): fused torch.optim.Adam(lr, weight_decay) step over ONE flat fp32

@@ -10,7 +10,8 @@ of the forward path runs in csrc/*.cuh behind the C ABI of include/vpt_b200.h.  
 """
 from . import _native  # noqa: F401
 from .types import DictType, Discrete, TensorType, idm_action_space, minecraft_action_space  # noqa: F401
-from .agent import ActionCodec, IDMAgent, MineRLAgent, composite_cursor, ingest_frames, resize_frames  # noqa: F401
+from .agent import (ActionCodec, IDMAgent, MineRLAgent, augment_frames, augment_matrices, augment_params, composite_cursor,  # noqa: F401
+                    ingest_frames, resize_frames)
 from .policy import FrameLatents, InverseActionNet, InverseActionPolicy, MinecraftAgentPolicy, MinecraftPolicy, NetConfig, RingRows, RingState  # noqa: F401
 from .checkpoint import load_model_parameters, load_training_state, load_weights, resize_memory, save_training_state, save_weights  # noqa: F401
 from .training import BCTrainer, IDMTrainer, RLTrainer  # noqa: F401

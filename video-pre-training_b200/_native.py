@@ -136,6 +136,8 @@ SIGNATURES = {
     "vpt_gather_logprob": (_I, [_P, _P, _P, _L, _I, _I, _P]),
     "vpt_resize_bilinear_u8": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "vpt_composite_cursor_u8": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vpt_augment_frames": (_I, [_P, _P, _I, _P, _I, _I, _I, _P]),
+    "vpt_augment_max_frame_bytes": (_I, []),
     "vpt_adam_step": (_I, [_P, _P, _P, _P, _L, _F, _F, _F, _F, _F, _F, _I, _P]),
     # BC backward (training.py)
     "vpt_relu_mask": (_I, [_P, _P, _P, _L, _P]),

@@ -251,6 +251,122 @@ def ingest_frames(frames_bgr: torch.Tensor, cursor=None, alpha=None, cursor_xy=N
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# training-time augmentation
+# ---------------------------------------------------------------------------------------------------------------------
+AUGMENT_PARAMS = ("rotate", "scale", "shear", "translate_x", "translate_y", "brightness", "contrast", "saturation", "hue")
+
+
+def _check_range(name, r, lo_min, strict=False):
+    lo, hi = (float(v) for v in r)
+    if not (np.isfinite(lo) and np.isfinite(hi)) or lo > hi or (lo <= lo_min if strict else lo < lo_min):
+        raise ValueError(f"augment_params: {name} must be a finite (lo, hi) with {lo_min} {'<' if strict else '<='} lo <= hi (got {r})")
+    return lo, hi
+
+
+def augment_params(B, T=None, *, generator, rotate=0.0, scale=(1.0, 1.0), shear=0.0, translate=0.0, brightness=(1.0, 1.0),
+                   contrast=(1.0, 1.0), saturation=(1.0, 1.0), hue=0.0, per_frame=False) -> torch.Tensor:
+    """Uniform augmentation parameters for `augment_frames`, fp32 (B, 9) -- one draw per sequence -- or (B, T, 9) with per_frame=True.
+    Columns (`AUGMENT_PARAMS`): rotate and shear in degrees, drawn from [-rotate, rotate] and [-shear, shear]; scale from (lo, hi);
+    translate_x and translate_y in pixels, each from [-translate, translate]; brightness, contrast and saturation from their (lo, hi);
+    hue from [-hue, hue] (hue <= 0.5).  The defaults are the identity.  Every call draws 9 uniforms per row from `generator` (on its
+    device) whatever the ranges, so a seeded generator gives the same parameters for the same B, T and per_frame.
+
+    One draw per sequence is the default because the models read motion from differences between neighbouring frames: both policies
+    infer the camera action from frame-to-frame image shifts, and the IDM's conv3d mixes five neighbouring frames.  A warp drawn per
+    frame would add shifts and rotations that no action caused, contradicting the action labels; `augment_frames` broadcasts a (B, 9)
+    draw over the T frames of each sequence."""
+    if int(B) != B or B <= 0:
+        raise ValueError(f"augment_params: B must be a positive integer (got {B})")
+    if per_frame and (T is None or int(T) != T or T <= 0):
+        raise ValueError(f"augment_params: per_frame=True needs a positive integer T (got {T})")
+    for name, v, ok in (("rotate", rotate, True), ("shear", shear, float(shear) < 90.0), ("translate", translate, True),
+                        ("hue", hue, float(hue) <= 0.5)):
+        if not (np.isfinite(float(v)) and float(v) >= 0 and ok):
+            raise ValueError(f"augment_params: {name} must be a finite half-width >= 0 (shear < 90 degrees, hue <= 0.5; got {v})")
+    ranges = [_check_range("scale", scale, 0.0, strict=True), _check_range("brightness", brightness, 0.0),
+              _check_range("contrast", contrast, 0.0), _check_range("saturation", saturation, 0.0)]
+    n = int(B) * (int(T) if per_frame else 1)
+    u = torch.rand((n, 9), generator=generator, dtype=torch.float64, device=generator.device)
+    sym = lambda col, r: (2.0 * u[:, col] - 1.0) * float(r)
+    lin = lambda col, lh: lh[0] + (lh[1] - lh[0]) * u[:, col]
+    p = torch.stack([sym(0, rotate), lin(1, ranges[0]), sym(2, shear), sym(3, translate), sym(4, translate), lin(5, ranges[1]),
+                     lin(6, ranges[2]), lin(7, ranges[3]), sym(8, hue)], dim=1).to(torch.float32)
+    return p.reshape(int(B), int(T), 9) if per_frame else p
+
+
+def augment_matrices(params, H, W) -> np.ndarray:
+    """float64 (N, 2, 3) inverse affine maps (output pixel -> source point) of `augment_frames` for (N, 9) parameters, about the frame
+    centre c = ((W - 1) / 2, (H - 1) / 2), pixel centres at integer coordinates, x right and y down.  The forward map is
+        out = c + t + s R(rotate) Sh(shear) (src - c),   R = [[cos, -sin], [sin, cos]],  Sh = [[1, tan], [0, 1]],  t = (tx, ty),
+    so a positive rotate turns the content clockwise on screen; the inverse is src = c + L^-1 (out - c - t) with L = s R Sh."""
+    p = np.asarray(params, dtype=np.float64).reshape(-1, 9)
+    th, s, ph = np.deg2rad(p[:, 0]), p[:, 1], np.deg2rad(p[:, 2])
+    cos, sin, tan = np.cos(th), np.sin(th), np.tan(ph)
+    # L^-1 = (1/s) Sh^-1 R^T = (1/s) [[cos + tan sin, sin - tan cos], [-sin, cos]]
+    li = np.stack([np.stack([cos + tan * sin, sin - tan * cos], -1), np.stack([-sin, cos], -1)], 1) / s[:, None, None]
+    c = np.array([(W - 1) / 2.0, (H - 1) / 2.0])
+    ct = c[None] + p[:, 3:5]
+    off = c[None] - np.einsum("nij,nj->ni", li, ct)
+    return np.concatenate([li, off[:, :, None]], axis=2)
+
+
+def augment_frames(frames: torch.Tensor, params: torch.Tensor, out_dtype=torch.uint8) -> torch.Tensor:
+    """Affine and colour jitter of uint8 CUDA frames (N, H, W, 3) or (B, T, H, W, 3) in one kernel (`vpt_augment_frames`): per frame an
+    inverse-mapped bilinear warp with zero fill, then brightness, contrast (about the frame's mean grey), saturation and hue, with
+    torchvision's `adjust_*` formulas (include/vpt_b200.h states the arithmetic).  `params` (`augment_params`) holds one row per frame,
+    (N, 9) or (B, T, 9), or for (B, T, ...) frames (B, 9), one row per sequence broadcast over T.  The output has the frames' shape, uint8
+    (rounded to nearest even) or float32 on the uint8 scale (unrounded), which the forward and the trainers take as they are.  The
+    inverse matrices are built on the host in float64 (`augment_matrices`) and rounded to fp32; params on the GPU are copied to the host
+    first.  Identity parameters return the frames bit for bit.  The output depends on each frame's own bytes and parameters only."""
+    if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+        raise TypeError(f"augment_frames: frames must be a uint8 tensor (got {getattr(frames, 'dtype', type(frames))})")
+    if frames.dim() not in (4, 5) or frames.shape[-1] != 3 or frames.numel() == 0:
+        raise ValueError(f"augment_frames: frames must be non-empty (N, H, W, 3) or (B, T, H, W, 3) (got {tuple(frames.shape)})")
+    if out_dtype not in (torch.uint8, torch.float32):
+        raise TypeError(f"augment_frames: out_dtype must be torch.uint8 or torch.float32 (got {out_dtype})")
+    rows = augment_rows(params, tuple(frames.shape))
+    if not frames.is_cuda:
+        raise nat.NativeError("augment_frames needs a CUDA tensor (no CPU fallback)")
+    from . import ops
+    n, H, W = rows.shape[0], frames.shape[-3], frames.shape[-2]
+    frames = frames.contiguous()
+    out = torch.empty(frames.shape, dtype=out_dtype, device=frames.device)
+    ops.augment(frames.view(n, H, W, 3), torch.from_numpy(rows).to(frames.device), out.view(n, H, W, 3))
+    return out
+
+
+def augment_rows(params, frames_shape) -> np.ndarray:
+    """The kernel's per-frame parameters, fp32 (N, 10) = (inverse matrix (2, 3) row-major, brightness, contrast, saturation, hue), for
+    `augment_frames` params and frames of shape `frames_shape`; raises ValueError / TypeError on parameters it refuses."""
+    if not isinstance(params, torch.Tensor) or not params.dtype.is_floating_point:
+        raise TypeError(f"augment_frames: params must be a floating tensor (got {getattr(params, 'dtype', type(params))})")
+    lead, (H, W) = tuple(frames_shape[:-3]), tuple(frames_shape[-3:-1])
+    n = int(np.prod(lead))
+    shapes = [lead + (9,)] + ([(lead[0], 9)] if len(lead) == 2 else [])
+    if tuple(params.shape) not in shapes:
+        raise ValueError(f"augment_frames: params must be {' or '.join(str(s) for s in shapes)} for frames {tuple(frames_shape)} "
+                         f"(got {tuple(params.shape)})")
+    p = params.detach().to("cpu", torch.float64).reshape(-1, 9).numpy()
+    if p.shape[0] != n:
+        p = np.repeat(p, lead[1], axis=0)
+    if not np.isfinite(p).all():
+        raise ValueError("augment_frames: params must be finite")
+    if (p[:, 1] <= 0).any():
+        raise ValueError("augment_frames: scale must be > 0")
+    if (np.abs(p[:, 2]) >= 90).any():
+        raise ValueError("augment_frames: shear must lie in (-90, 90) degrees")
+    if (p[:, 5:8] < 0).any():
+        raise ValueError("augment_frames: brightness, contrast and saturation must be >= 0")
+    if (np.abs(p[:, 8]) > 0.5).any():
+        raise ValueError("augment_frames: |hue| must be <= 0.5")
+    with np.errstate(over="ignore"):
+        A = augment_matrices(p, H, W).astype(np.float32)
+    if not np.isfinite(A).all():
+        raise ValueError("augment_frames: params give an inverse matrix that is not finite in fp32")
+    return np.ascontiguousarray(np.concatenate([A.reshape(n, 6), p[:, 5:9].astype(np.float32)], axis=1))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # MineRLAgent
 # ---------------------------------------------------------------------------------------------------------------------
 class MineRLAgent:

@@ -27,6 +27,7 @@ void set_error(const char* fmt, ...) {
 #include "heads.cuh"
 #include "adam.cuh"
 #include "resize.cuh"
+#include "augment.cuh"
 #include "backward.cuh"
 #include "attention_bwd.cuh"
 #include "attention_full_bwd.cuh"

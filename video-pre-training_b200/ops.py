@@ -606,6 +606,7 @@ from .ops_bptt import attention_bwd_state  # noqa: E402,F401  (gradients through
 from .ops_pixel import conv3d_t5_dimg, firstconv_dimg  # noqa: E402,F401  (image gradients, csrc/firstconv_bwd.cuh, csrc/idm_bwd.cuh)
 from .ops_ring import attention_ring, attention_ring_plan, ring_advance, ring_advance_rows, ring_noise_keys, ring_write  # noqa: E402,F401  (the KV memory as a ring, csrc/ring.cuh)
 from .ops_invariant import attention_plan, conv3x3_zp_plan, gemm_rowwise, gumbel_argmax_keyed, maxpool3s2_plan  # noqa: E402,F401  (batch-invariant mode)
+from .ops_augment import augment  # noqa: E402,F401  (training-time augmentation, csrc/augment.cuh)
 
 
 # ---- on-device action codec (csrc/codec.cuh) -----------------------------------------------------------------------------
